@@ -9,8 +9,10 @@
 //   radix sort (4 passes)   primitives.cu (stable: insertion order inside a cell)
 //   kd_finalize_kernel      sorted float4 copy + the hashed cell tables of all levels
 // Tables and cached normals carry the build's generation number: nothing is cleared between frames.
-// Search (local_map.py:372-422): whole warps per query, see kdmap_device.cuh; one ICP iteration = three launches
-// (kd_nn_warp_kernel, kd_normals_warp_kernel, kd_residual_kernel which also runs the solve in its last block).
+// Search (local_map.py:372-422): whole warps per query, see kdmap_device.cuh.  A frame's first ICP iteration = three
+// launches (kd_nn_warp_kernel, kd_normals_warp_kernel, kd_residual_kernel which also runs the solve in its last block);
+// every later iteration = one (kd_icp_refine_kernel) or, on maps of KD_COLD_MAP_POINTS or more, four (verify, 1-NN of the
+// unproven queries, normals, residual).
 #include <stdlib.h>
 
 #include "gn_device.cuh"
@@ -234,6 +236,7 @@ __global__ void kd_export_kernel(const float4* __restrict__ pts, int64_t n, floa
 //   kd_normals_warp_kernel  exact (k+1)-NN of every queued map point, second moments, lane-parallel eigen-solves
 //   kd_residual_kernel      a thread per query: r, J, robust weight, the 30 fp64 accumulators -> block partials; the
 //                           last block sums them in fixed order and runs the solve / stop test / pose update
+// Below KD_COLD_MAP_POINTS, the iterations after a frame's first run all of that as ONE launch, kd_icp_refine_kernel.
 constexpr int KD_THREADS = 256;
 constexpr int KD_WARPS = KD_THREADS / 32;
 
@@ -385,11 +388,13 @@ __global__ void __launch_bounds__(KD_THREADS)
 kd_normals_warp_kernel(KdIndex ix, int k_normals, const int* __restrict__ worklist, const uint32_t* __restrict__ wl_count,
                        const int* __restrict__ done, unsigned long long* __restrict__ counters) {
     if (done && *done) return;
+    __shared__ unsigned long long s_stage[KD_WARPS][KNN_STAGE];
     const int n = (int)*wl_count;
     const int lane = threadIdx.x & 31;
     const int warp_global = blockIdx.x * KD_WARPS + (threadIdx.x >> 5);
     const int total_warps = gridDim.x * KD_WARPS;
     if (warp_global >= n) return;
+    unsigned long long* stage = s_stage[threadIdx.x >> 5];
     const KdGridLocal g = kd_load_grid(ix);
     const float valid = __uint_as_float(kd_normal_valid(ix.gen));
     float mycov[6];
@@ -406,9 +411,8 @@ kd_normals_warp_kernel(KdIndex ix, int k_normals, const int* __restrict__ workli
             posn = worklist[en];
             cn = __ldg(ix.sorted + posn);
         }
-        float nd;
         int ni;
-        const int found = warp_knn(ix, g, c.x, c.y, c.z, k_normals + 1, lane, nd, ni, &cand);
+        const int found = warp_knn(ix, g, c.x, c.y, c.z, k_normals + 1, lane, ni, &cand, stage);
         float cov[6];
         warp_second_moments(ix, c, k_normals, found, ni, lane, cov);
         if (lane == held) {
@@ -464,6 +468,120 @@ kd_residual_kernel(KdIndex ix, const float4* __restrict__ queries, const uint32_
         p[2] = p0.x * sT[8] + p0.y * sT[9] + p0.z * sT[10] + sT[11];
         const int pos = match[qi];
         if (pos < 0) continue;
+        const float4 qq = __ldg(ix.sorted + pos);
+        const float4 nv = __ldcg(ix.normals + pos);
+        float q[3] = {qq.x, qq.y, qq.z};
+        float nn[3] = {nv.x, nv.y, nv.z};
+        float J[6];
+        const float r = p2plane_residual_jacobian_identity(p, q, nn, J);
+        const float w = ls_weight<float>(scheme, sigma, r, p, q);
+        accumulate_normal_equations<float>(acc, J, w, r * w, r);
+    }
+    block_reduce_store<KD_RES_THREADS>(acc, partials + (size_t)blockIdx.x * NACC);
+    if (fuse_threshold >= 0.f) icp_finish_in_last_block(fr, partials, fuse_threshold);
+}
+
+// ICP iterations after a frame's first, in ONE launch.  Each block takes the queries kd_residual_kernel would give it
+// (same grid, same striding, so the block partials are the same bits):
+//   1. per round of 256 of them, a thread per query VERIFIES instead of searching.  The full search stored, per query,
+//      where the query stood (its transformed position) and a lower bound of the distance to every map point other
+//      than its match.  If the query has moved by eps since then and its match is now at distance d, every other point
+//      is still at least (bound - eps) away, so d + eps < bound proves the match unchanged -- one point load and a
+//      dozen flops per query;
+//   2. the block's warps re-search the round's unproven queries (warp_nearest, seeded with the previous match) and
+//      compute the normal of every new match that has none cached (warp_knn, second moments, eigen-solve).  Another
+//      block may compute the same normal at the same time: the computation is deterministic, so both store the same
+//      bits, and no block ever waits for another;
+//   3. once every round is searched, a thread per query: residual, Jacobian, weight, fp64 accumulation -- then the block
+//      partial and, fused, the solve in the last block.  The accumulators are not live during the searches.
+__global__ void __launch_bounds__(KD_THREADS)
+kd_icp_refine_kernel(KdIndex ix, const float4* __restrict__ queries, const uint32_t* __restrict__ nq_dev, int64_t q_begin,
+                     int64_t q_stride, FrameResult* fr, int scheme, float sigma, int k_normals, int* __restrict__ match,
+                     float4* __restrict__ nn_state, double* __restrict__ partials, float fuse_threshold,
+                     unsigned long long* __restrict__ counters) {
+    if (fr->done) return;
+    __shared__ float sT[12];
+    __shared__ int s_hard[KD_THREADS];
+    __shared__ int s_nh;
+    __shared__ unsigned long long s_stage[KD_WARPS][KNN_STAGE];
+    if (threadIdx.x < 12) sT[threadIdx.x] = fr->T[threadIdx.x];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int64_t nq = (int64_t)*nq_dev;
+    const uint32_t valid = kd_normal_valid(ix.gen);
+    int cand_nn = 0, cand_knn = 0, normals_here = 0;
+    for (int64_t round = (int64_t)blockIdx.x * KD_THREADS;; round += (int64_t)gridDim.x * KD_THREADS) {
+        if (q_begin + round * q_stride >= nq) break;  // block-uniform
+        if (threadIdx.x == 0) s_nh = 0;
+        __syncthreads();
+        const int64_t qi = q_begin + (round + threadIdx.x) * q_stride;
+        if (qi < nq) {
+            const float4 p0 = queries[qi];
+            const float px = p0.x * sT[0] + p0.y * sT[1] + p0.z * sT[2] + sT[3];
+            const float py = p0.x * sT[4] + p0.y * sT[5] + p0.z * sT[6] + sT[7];
+            const float pz = p0.x * sT[8] + p0.y * sT[9] + p0.z * sT[10] + sT[11];
+            const int pos = match[qi];
+            bool proven = false;
+            if (pos >= 0) {
+                const float4 s = nn_state[qi];
+                const float d = sqrtf(dist2_point(px, py, pz, __ldg(ix.sorted + pos)));
+                const float eps = sqrtf(dist2_point(px, py, pz, s));
+                proven = (d + eps) * 1.00001f + 1e-6f < sqrtf(s.w);
+            }
+            if (!proven) s_hard[atomicAdd(&s_nh, 1)] = threadIdx.x;
+        }
+        __syncthreads();
+        const int nh = s_nh;
+        if (warp < nh) {
+            const KdGridLocal g = kd_load_grid(ix);
+            for (int e = warp; e < nh; e += KD_WARPS) {
+                const int64_t q = q_begin + (round + s_hard[e]) * q_stride;
+                const float4 p0 = queries[q];
+                const float px = p0.x * sT[0] + p0.y * sT[1] + p0.z * sT[2] + sT[3];
+                const float py = p0.x * sT[4] + p0.y * sT[5] + p0.z * sT[6] + sT[7];
+                const float pz = p0.x * sT[8] + p0.y * sT[9] + p0.z * sT[10] + sT[11];
+                float second;
+                const int pos = warp_nearest(ix, g, px, py, pz, match[q], lane, &cand_nn, &second);
+                if (lane == 0) {
+                    match[q] = pos;
+                    nn_state[q] = make_float4(px, py, pz, second);
+                }
+                if (pos < 0) continue;
+                const uint32_t state = __shfl_sync(FULL, __ldcg(reinterpret_cast<const uint32_t*>(&ix.normals[pos].w)), 0);
+                if (state == valid) continue;
+                const float4 c = __ldg(ix.sorted + pos);
+                int ni;
+                const int found = warp_knn(ix, g, c.x, c.y, c.z, k_normals + 1, lane, ni, &cand_knn, s_stage[warp]);
+                float cov[6];
+                warp_second_moments(ix, c, k_normals, found, ni, lane, cov);
+                if (lane == 0) {
+                    float nn[3];
+                    smallest_eigenvector(cov, nn);
+                    __stcg(ix.normals + pos, make_float4(nn[0], nn[1], nn[2], __uint_as_float(valid)));
+                }
+                ++normals_here;
+            }
+        }
+        __syncthreads();  // s_hard / s_nh are reused by the next round
+    }
+    if (counters && lane == 0) {
+        if (cand_nn) atomicAdd(counters + KDC_NN_CAND, (unsigned long long)cand_nn);
+        if (cand_knn) atomicAdd(counters + KDC_KNN_CAND, (unsigned long long)cand_knn);
+        if (normals_here) atomicAdd(counters + KDC_NORMALS, (unsigned long long)normals_here);
+    }
+    // every match and normal of this block's queries is in place (the last round ended on a barrier)
+    double acc[NACC];
+#pragma unroll
+    for (int a = 0; a < NACC; ++a) acc[a] = 0.0;
+    for (int64_t s = (int64_t)blockIdx.x * KD_THREADS + threadIdx.x;; s += (int64_t)gridDim.x * KD_THREADS) {
+        const int64_t qi = q_begin + s * q_stride;
+        if (qi >= nq) break;
+        const int pos = match[qi];
+        if (pos < 0) continue;
+        const float4 p0 = queries[qi];
+        float p[3];
+        p[0] = p0.x * sT[0] + p0.y * sT[1] + p0.z * sT[2] + sT[3];
+        p[1] = p0.x * sT[4] + p0.y * sT[5] + p0.z * sT[6] + sT[7];
+        p[2] = p0.x * sT[8] + p0.y * sT[9] + p0.z * sT[10] + sT[11];
         const float4 qq = __ldg(ix.sorted + pos);
         const float4 nv = __ldcg(ix.normals + pos);
         float q[3] = {qq.x, qq.y, qq.z};
@@ -801,6 +919,12 @@ static void launch_search(pls_context* ctx, const KdIndex& ix, const float4* que
     PLS_CHECK_LAUNCH();
 }
 
+// Later ICP iterations run as one kd_icp_refine_kernel, except on maps of this many points or more.  On the 5 M-point
+// map of BASELINE config 4 the single kernel was slower on H100 (1.10-1.22 ms per registration against 0.91-0.92 with
+// the four launches; the same with the kernel at 120 registers and no spills), on the 0.65 M-point cfg2 map faster.
+// The cut-off between the two is not tuned: no map size in between has been measured.
+constexpr int64_t KD_COLD_MAP_POINTS = 2000000;
+
 // One ICP iteration over the device-resident queries (float4 in ctx->query_ptr, count in the FrameResult); writes
 // block partials to ctx->partials and returns the block count.
 int kdmap_icp_iteration(pls_context* ctx, int64_t query_bound, int rank, int num_ranks, int it, float fuse_threshold,
@@ -813,15 +937,24 @@ int kdmap_icp_iteration(pls_context* ctx, int64_t query_bound, int rank, int num
     // credited per executed iteration by the caller (the launch is a no-op once ICP converged)
     ProfileScope ps(ctx, 0, 0.0, false);
     const KdIndex ix = make_index(ctx);
-    launch_search(ctx, ix, ctx->query_ptr, nq_dev, mine, rank, num_ranks, fr->T, &fr->done, ctx->nn_prev.as<int>(), it == 0, true,
-                  it & 1);
     const int blocks = grid_for(mine, KD_RES_THREADS, 8 * kNumSMs);
     ctx->partials.reserve((size_t)blocks * NACC * sizeof(double), st);
-    ProfileScope p10(ctx, 10, 0.0);
-    kd_residual_kernel<<<blocks, KD_RES_THREADS, 0, st>>>(ix, ctx->query_ptr, nq_dev, (int64_t)rank, (int64_t)num_ranks, fr,
-                                                          ctx->cfg.scheme, ctx->cfg.sigma, ctx->nn_prev.as<int>(),
-                                                          ctx->partials.as<double>(), fuse_threshold);
-    PLS_CHECK_LAUNCH();
+    if (it == 0 || ctx->kd.indexed >= KD_COLD_MAP_POINTS) {
+        launch_search(ctx, ix, ctx->query_ptr, nq_dev, mine, rank, num_ranks, fr->T, &fr->done, ctx->nn_prev.as<int>(), it == 0,
+                      true, it & 1);
+        ProfileScope p10(ctx, 10, 0.0);
+        kd_residual_kernel<<<blocks, KD_RES_THREADS, 0, st>>>(ix, ctx->query_ptr, nq_dev, (int64_t)rank, (int64_t)num_ranks, fr,
+                                                              ctx->cfg.scheme, ctx->cfg.sigma, ctx->nn_prev.as<int>(),
+                                                              ctx->partials.as<double>(), fuse_threshold);
+        PLS_CHECK_LAUNCH();
+    } else {
+        ProfileScope p11(ctx, 11, 0.0);
+        kd_icp_refine_kernel<<<blocks, KD_THREADS, 0, st>>>(ix, ctx->query_ptr, nq_dev, (int64_t)rank, (int64_t)num_ranks, fr,
+                                                            ctx->cfg.scheme, ctx->cfg.sigma, ctx->cfg.num_neighbors_normals,
+                                                            ctx->nn_prev.as<int>(), ctx->kd_nn_state.as<float4>(),
+                                                            ctx->partials.as<double>(), fuse_threshold, kd_counters(ctx));
+        PLS_CHECK_LAUNCH();
+    }
     *solved = fuse_threshold >= 0.f;
     return blocks;
 }

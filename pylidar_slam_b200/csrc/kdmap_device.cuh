@@ -200,7 +200,7 @@ __device__ __forceinline__ int warp_candidate(int incl, int adj /* = start - exc
 // *second_out receives a lower bound of the squared distance from the query to every map point OTHER than the winner
 // (the runner-up inside the scanned block, the boxes of the cells that were pruned, the block's exactness radius):
 // as long as the query moves by less than the gap between the two, the winner stays the nearest neighbour -- the next
-// ICP iterations verify that instead of searching again (kd_nn_verify_kernel).
+// ICP iterations verify that instead of searching again (kd_icp_refine_kernel).
 __device__ __forceinline__ int warp_nearest(const KdIndex& ix, const KdGridLocal& g, float x, float y, float z, int hint,
                                             int lane, int* cand_out, float* second_out) {
     float best = FLT_MAX, second = FLT_MAX;
@@ -261,105 +261,168 @@ __device__ __forceinline__ int warp_nearest(const KdIndex& ix, const KdGridLocal
     return best_i;
 }
 
-// One chunk of the K-NN selection: R fresh candidates per lane (t = chunk + s * 32 + lane) plus the lane's entry of the
-// list kept so far compete; on return lane r < K holds the r-th smallest of them.
-//   * every lane sorts its R + 1 entries ascending (a small compare-exchange network, no communication);
-//   * K rounds: the warp's minimum over the lane heads (two REDUX), the owner pops its head (a register shift).
-template <int R>
-__device__ __forceinline__ void knn_select_chunk(const KdIndex& ix, float x, float y, float z, int K, int lane, int incl, int adj,
-                                                 int total, int chunk, float& keep_d, int& keep_i) {
-    float sd[R + 1];
-    int si[R + 1];
-#pragma unroll
-    for (int s = 0; s < R; ++s) {
-        const int t = chunk + s * 32 + lane;
-        const bool active = t < total;
-        const int idx = warp_candidate(incl, adj, active ? t : total - 1);
-        sd[s] = active ? dist2_point(x, y, z, __ldg(ix.sorted + idx)) : FLT_MAX;
-        si[s] = active ? idx : -1;
-    }
-    sd[R] = keep_d;
-    si[R] = keep_i;
-    // insertion network: after pass p the first p + 2 entries are ordered
-#pragma unroll
-    for (int p = 1; p <= R; ++p) {
-#pragma unroll
-        for (int q = p; q >= 1; --q) {
-            const bool sw = sd[q] < sd[q - 1] || (sd[q] == sd[q - 1] && (unsigned)si[q] < (unsigned)si[q - 1]);
-            const float td = sw ? sd[q - 1] : sd[q];
-            const int ti = sw ? si[q - 1] : si[q];
-            sd[q - 1] = sw ? sd[q] : sd[q - 1];
-            si[q - 1] = sw ? si[q] : si[q - 1];
-            sd[q] = td;
-            si[q] = ti;
-        }
-    }
-    float nd = FLT_MAX;
-    int ni = -1;
-    for (int r = 0; r < K; ++r) {
-        float wd = sd[0];
-        int wi = si[0];
-        const int mine = wi;
-        warp_argmin(wd, wi);
-        if (wi < 0) break;  // nothing left anywhere
-        if (mine == wi) {   // indices are unique: exactly one lane pops
-#pragma unroll
-            for (int s = 0; s < R; ++s) {
-                sd[s] = sd[s + 1];
-                si[s] = si[s + 1];
-            }
-            sd[R] = FLT_MAX;
-            si[R] = -1;
-        }
-        if (lane == r) {
-            nd = wd;
-            ni = wi;
-        }
-    }
-    keep_d = nd;
-    keep_i = ni;
+// K-NN candidates compare as ONE 64-bit key: the bits of d^2 (>= 0, so they order like the value) above the sorted
+// position -- the order (distance, then position) of the neighbour lists.  KNN_NONE: no candidate.
+constexpr unsigned long long KNN_NONE = ~0ull;
+__device__ __forceinline__ unsigned long long knn_key(float d, int idx) {
+    return ((unsigned long long)__float_as_uint(d) << 32) | (unsigned)idx;
 }
 
-// Exact K-NN (K <= 32, warp-uniform) of (x, y, z): on return lane r < found holds the r-th nearest point
-// (out_d, out_i), ascending by (distance, index); returns the number found (min(K, M)).
-// The candidates of a block are taken in chunks of 32 * R, R = 2, 4 or 8 register slots per lane by block size
-// (a 27-cell block of the BASELINE maps holds 30-80 points: one chunk of R = 2 or 4).
+// The warp's smallest key (two REDUX: the distance bits, then the position among the lanes that hold that distance).
+__device__ __forceinline__ unsigned long long warp_min_key(unsigned long long k) {
+    const unsigned hi = __reduce_min_sync(FULL, (unsigned)(k >> 32));
+    const unsigned lo = __reduce_min_sync(FULL, (unsigned)(k >> 32) == hi ? (unsigned)k : 0xffffffffu);
+    return ((unsigned long long)hi << 32) | lo;
+}
+
+// Level 0, at most 32 R candidates: lane r < K returns the r-th smallest key (KNN_NONE past the last candidate).
+//   * every lane sorts its R candidates (t = s * 32 + lane) ascending (a small compare-exchange network);
+//   * K rounds: the warp's minimum over the lane heads, the owner pops its head (a register shift).
+template <int R>
+__device__ __forceinline__ unsigned long long knn_select_small(const KdIndex& ix, float x, float y, float z, int K, int lane,
+                                                               int incl, int adj, int total) {
+    unsigned long long s[R];
+#pragma unroll
+    for (int j = 0; j < R; ++j) {
+        const int t = j * 32 + lane;
+        const bool active = t < total;
+        const int idx = warp_candidate(incl, adj, active ? t : total - 1);
+        s[j] = active ? knn_key(dist2_point(x, y, z, __ldg(ix.sorted + idx)), idx) : KNN_NONE;
+    }
+    // insertion network: after pass p the first p + 1 entries are ordered
+#pragma unroll
+    for (int p = 1; p < R; ++p) {
+#pragma unroll
+        for (int q = p; q >= 1; --q) {
+            const unsigned long long lo = min(s[q - 1], s[q]), hi = max(s[q - 1], s[q]);
+            s[q - 1] = lo;
+            s[q] = hi;
+        }
+    }
+    unsigned long long out = KNN_NONE;
+    for (int r = 0; r < K; ++r) {
+        const unsigned long long m = warp_min_key(s[0]);
+        if (m == KNN_NONE) break;  // nothing left anywhere
+        if (s[0] == m) {           // keys are unique: exactly one lane pops
+#pragma unroll
+            for (int j = 0; j + 1 < R; ++j) s[j] = s[j + 1];
+            s[R - 1] = KNN_NONE;
+        }
+        if (lane == r) out = m;
+    }
+    return out;
+}
+
+// Bitonic sort of one key per lane, ascending with the lane index (15 compare-exchange stages over shuffles).
+__device__ __forceinline__ unsigned long long warp_sort_keys(unsigned long long v, int lane) {
+#pragma unroll
+    for (int k = 2; k <= 32; k <<= 1) {
+#pragma unroll
+        for (int j = k >> 1; j > 0; j >>= 1) {
+            const unsigned long long o = __shfl_xor_sync(FULL, v, j);
+            v = (((lane & j) == 0) == ((lane & k) == 0)) ? min(v, o) : max(v, o);
+        }
+    }
+    return v;
+}
+
+// The 32 smallest of two ascending lane-sorted lists, ascending: the element-wise minimum of one list and the other
+// reversed is a bitonic sequence holding them, which five merge stages sort.
+__device__ __forceinline__ unsigned long long warp_merge_keys(unsigned long long a, unsigned long long b, int lane) {
+    unsigned long long v = min(a, __shfl_sync(FULL, b, 31 - lane));
+#pragma unroll
+    for (int j = 16; j > 0; j >>= 1) {
+        const unsigned long long o = __shfl_xor_sync(FULL, v, j);
+        v = (lane & j) ? max(v, o) : min(v, o);
+    }
+    return v;
+}
+
+// Exact K-NN (K <= 32, warp-uniform) of (x, y, z): on return lane r < found holds the sorted position of the r-th
+// nearest point (ascending by (distance, position)), other lanes -1; returns the number found (min(K, M)).
+// `stage` is a warp-private shared buffer of KNN_STAGE keys.
+//   * Level 0 (a 27-cell block of the BASELINE maps holds 30-80 points): up to 128 candidates are selected by
+//     knn_select_small.
+//   * Every coarser level (and a denser level-0 block) streams its candidates through a filter: the K-th key of the
+//     previous level bounds this level's K-th from above (its block is a superset), so only keys <= that bound survive.
+//     Survivors are compacted into `stage` with a ballot; every 32 of them are sorted and merged into the running 32
+//     best.  If exactly K survive, they are the previous level's K: the list stands as it is.  A level whose table
+//     overflowed is skipped: it scans nothing and leaves the list and its bound alone.
+constexpr int KNN_STAGE = 64;
 __device__ __forceinline__ int warp_knn(const KdIndex& ix, const KdGridLocal& g, float x, float y, float z, int K, int lane,
-                                        float& out_d, int& out_i, int* cand_out) {
-    float keep_d = FLT_MAX;   // lane r: r-th best so far (carried between chunks / the result)
-    int keep_i = -1;
+                                        int& out_i, int* cand_out, unsigned long long* stage) {
+    unsigned long long kept = KNN_NONE;   // lane r < K: r-th smallest key so far
+    unsigned long long bound = KNN_NONE;  // K-th key of the previous (finer) level
+    float bound_d = FLT_MAX;              // ... its distance
     int found = 0;
     if (lane == 0) kd_stat(ix, 4);
-    float bound = FLT_MAX;    // K-th distance of the previous (finer) level: an upper bound for this one
+    const unsigned lanes_below = (1u << lane) - 1u;
     for (int level = 0; level <= g.top; ++level) {
         int start, count;
         float box2;
         const float r2 = warp_probe_block(ix, g, level, x, y, z, lane, start, count, box2);
-        if (box2 > bound) count = 0;
+        if (r2 < 0.f) {  // this level's table overflowed: nothing scanned, the list of the finer level stands
+            if (ix.stats && lane == 0 && level == 0) kd_stat(ix, 6);
+            continue;
+        }
+        if (box2 > bound_d) count = 0;
         int incl;
         const int total = warp_scan_counts(count, lane, incl);
         const int adj = start - (incl - count);
         if (cand_out) *cand_out += total;
         if (ix.stats && lane == 0) kd_stat(ix, 7, (unsigned long long)total);
-        keep_d = FLT_MAX;     // this level's block is a superset of the previous one: select afresh
-        keep_i = -1;
-        if (total <= 64) {
-            knn_select_chunk<2>(ix, x, y, z, K, lane, incl, adj, total, 0, keep_d, keep_i);
-        } else if (total <= 128) {
-            knn_select_chunk<4>(ix, x, y, z, K, lane, incl, adj, total, 0, keep_d, keep_i);
+        if (bound == KNN_NONE && total <= 64) {
+            kept = knn_select_small<2>(ix, x, y, z, K, lane, incl, adj, total);
+        } else if (bound == KNN_NONE && total <= 128) {
+            kept = knn_select_small<4>(ix, x, y, z, K, lane, incl, adj, total);
         } else {
-            for (int chunk = 0; chunk < total; chunk += 256)
-                knn_select_chunk<8>(ix, x, y, z, K, lane, incl, adj, total, chunk, keep_d, keep_i);
+            unsigned long long best = KNN_NONE;
+            int staged = 0, survivors = 0;
+            bool merged = false;
+            for (int base = 0; base < total; base += 32) {
+                const int t = base + lane;
+                const bool active = t < total;
+                const int idx = warp_candidate(incl, adj, active ? t : total - 1);
+                unsigned long long key = KNN_NONE;
+                if (active) key = knn_key(dist2_point(x, y, z, __ldg(ix.sorted + idx)), idx);
+                const bool keep = active && key <= bound;
+                const unsigned b = __ballot_sync(FULL, keep);
+                if (keep) stage[staged + __popc(b & lanes_below)] = key;
+                staged += __popc(b);
+                survivors += __popc(b);
+                if (staged >= 32) {
+                    __syncwarp();
+                    const unsigned long long c = warp_sort_keys(stage[lane], lane);
+                    best = merged ? warp_merge_keys(best, c, lane) : c;
+                    merged = true;
+                    __syncwarp();
+                    if (lane < staged - 32) stage[lane] = stage[32 + lane];
+                    staged -= 32;
+                    __syncwarp();
+                }
+            }
+            // `kept` still holds the K keys that set `bound` (found == K): if exactly K survive, they are those K
+            if (found != K || survivors != K) {
+                if (staged > 0) {
+                    __syncwarp();
+                    const unsigned long long c = warp_sort_keys(lane < staged ? stage[lane] : KNN_NONE, lane);
+                    best = merged ? warp_merge_keys(best, c, lane) : c;
+                }
+                kept = lane < K ? best : KNN_NONE;
+            }
+            __syncwarp();  // `stage` is reused by the next level
         }
-        found = __popc(__ballot_sync(FULL, keep_i >= 0));
-        const float kth = __shfl_sync(FULL, keep_d, K - 1);
-        const bool exact = (found == K && kth <= r2) || level >= g.top;
+        found = __popc(__ballot_sync(FULL, kept != KNN_NONE));
+        const unsigned long long kth = __shfl_sync(FULL, kept, K - 1);
+        const bool exact = (found == K && __uint_as_float((unsigned)(kth >> 32)) <= r2) || level >= g.top;
         if (ix.stats && lane == 0 && level == 0) kd_stat(ix, exact ? 5 : 6);
         if (exact) break;
-        if (found == K) bound = kth;
+        if (found == K) {
+            bound = kth;
+            bound_d = __uint_as_float((unsigned)(kth >> 32));
+        }
     }
-    out_d = keep_d;
-    out_i = keep_i;
+    out_i = kept != KNN_NONE ? (int)(unsigned)kept : -1;
     return found;
 }
 

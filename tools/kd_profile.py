@@ -1,5 +1,7 @@
 """Development helper: in-pipeline (L2-warm) CUDA-event times of the single kernels of the cfg2 frame
-(profile slots 6..15), one slot per pass so that the event records of one kernel do not perturb another."""
+(profile slots 6..15), one slot per pass so that the event records of one kernel do not perturb another.
+Slot 0 covers every ICP iteration; 7 / 9 / 10 are the three kernels of a frame's first iteration, 11 the one kernel of
+each later iteration."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import ctypes as C
@@ -11,8 +13,9 @@ H, W, F, WARM = 64, 2048, 44, 24
 scans = [syn.scan(k, H, W) for k in range(F)]
 dev = torch.device("cuda", 0)
 dscans = torch.from_numpy(np.stack(scans)).to(dev)
-names = {0: "icp iteration (all)", 3: "index build", 4: "grid sample", 6: "nn verify", 7: "nn search", 9: "normals", 10: "residual+solve"}
-for slot in (int(a) for a in (sys.argv[1:] or ["0", "3", "4", "6", "7", "9", "10"])):
+names = {0: "icp iteration (all)", 3: "index build", 4: "grid sample", 7: "nn search", 9: "normals", 10: "residual+solve",
+         11: "later iteration"}
+for slot in (int(a) for a in (sys.argv[1:] or ["0", "3", "4", "7", "9", "10", "11"])):
     cfg = b200.ICPFrameToModelConfig(local_map=b200.KdTreeLocalMapConfig(local_map_size=20),
         alignment=b200.GaussNewtonPointToPlaneConfig(gauss_newton_config=dict(scheme="geman_mcclure", sigma=0.3, max_iters=1)),
         max_num_alignments=10, data_key="input_data")
