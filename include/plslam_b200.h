@@ -206,6 +206,16 @@ PLS_API int pls_kdmap_points(pls_context* ctx, float* out /* [M,3], insertion or
  * cached per map point until the next update.  out_idx [n] (int64, insertion order) or NULL. */
 PLS_API int pls_kdmap_nn_search(pls_context* ctx, const float* queries, int64_t n,
                         float* out_neighbors, float* out_normals, int64_t* out_idx);
+/* Test / debug aid: the correspondences of the last kd search of this context -- the last executed iteration of
+ * pls_register_frame or pls_process_frame, or pls_kdmap_nn_search.  n = number of queries of that search (the valid
+ * rows, in input order).  out_idx [n] insertion index of the match or -1; out_neighbors / out_normals [n,3] (normals
+ * NaN after a search without normals); out_search_state [n,4] = the position the query stood at in its last full
+ * search and the squared lower bound of its distance to every map point other than its match; out_sums [30] = the
+ * accumulators of the last executed ICP iteration (21 JtJ upper, 6 Jtr, sum (w r)^2, sum r^2, count; NaN after
+ * pls_kdmap_nn_search).  Every output nullable.  A pending map update is not flushed.  PLS_E_STATE if no kd search has
+ * run, if the map was rebuilt since, or if the last ICP split its queries over several ranks. */
+PLS_API int pls_kdmap_last_correspondences(pls_context* ctx, int64_t n, int64_t* out_idx, float* out_neighbors,
+                                           float* out_normals, float* out_search_state, double* out_sums);
 /* ProjectiveLocalMap.update (local_map.py:126-202): rel_pose [16]; vertex_map [3,H,W] or NULL. */
 PLS_API int pls_projmap_update(pls_context* ctx, const float* rel_pose, const float* vertex_map);
 PLS_API int pls_projmap_num_frames(pls_context* ctx, int* num_frames);

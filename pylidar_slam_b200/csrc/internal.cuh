@@ -119,6 +119,14 @@ struct KdMap {
     bool valid = false;
     int64_t cap_points = 0; // every per-point array holds this many points (kd_reserve_capacity)
     int64_t max_frame = 0;  // largest frame inserted so far (sizes the steady state: local_map_size frames)
+    // the last search (an ICP iteration or pls_kdmap_nn_search), whose matches and states nn_prev / kd_nn_state hold
+    // (read back by pls_kdmap_last_correspondences)
+    bool searched = false;
+    bool searched_icp = false;      // an ICP iteration: the query count is the FrameResult's, the sums its last_sums
+    bool searched_sharded = false;  // the queries were split over ranks: this rank holds only its share
+    bool searched_normals = false;  // the normals of the matched points were computed
+    uint32_t searched_gen = 0;      // index generation the matches refer to
+    int64_t searched_n = 0;         // query count (pls_kdmap_nn_search)
 };
 
 struct ProjMap {

@@ -733,6 +733,7 @@ void kdmap_reset(pls_context* ctx) {
     ctx->kd.bbox_clean = false;
     ctx->kd.max_frame = 0;   // the buffers (cap_points) and the generation counter are kept: a re-initialised
                              // sequence reuses them
+    ctx->kd.searched = false;
 }
 
 template <typename T>
@@ -939,6 +940,12 @@ int kdmap_icp_iteration(pls_context* ctx, int64_t query_bound, int rank, int num
     const KdIndex ix = make_index(ctx);
     const int blocks = grid_for(mine, KD_RES_THREADS, 8 * kNumSMs);
     ctx->partials.reserve((size_t)blocks * NACC * sizeof(double), st);
+    KdMap& kd = ctx->kd;
+    kd.searched = true;
+    kd.searched_icp = true;
+    kd.searched_sharded = num_ranks > 1;
+    kd.searched_normals = true;
+    kd.searched_gen = kd.gen;
     if (it == 0 || ctx->kd.indexed >= KD_COLD_MAP_POINTS) {
         launch_search(ctx, ix, ctx->query_ptr, nq_dev, mine, rank, num_ranks, fr->T, &fr->done, ctx->nn_prev.as<int>(), it == 0,
                       true, it & 1);
@@ -1053,6 +1060,13 @@ int pls_kdmap_nn_search(pls_context* ctx, const float* queries, int64_t n, float
     const KdIndex ix = make_index(ctx);
     launch_search(ctx, ix, ctx->queries.as<float4>(), nq, n, 0, 1, ctx->tmp[6].as<float>(), nullptr, ctx->nn_prev.as<int>(), true,
                   out_normals != nullptr, 0);
+    KdMap& kd = ctx->kd;
+    kd.searched = true;
+    kd.searched_icp = false;
+    kd.searched_sharded = false;
+    kd.searched_normals = out_normals != nullptr;
+    kd.searched_gen = kd.gen;
+    kd.searched_n = n;
     kd_search_export_kernel<<<grid_for(n, 256, 8 * kNumSMs), 256, 0, st>>>(ix, ctx->nn_prev.as<int>(), n, (float*)onb.dev,
                                                                             (float*)onr.dev, (long long*)oix.dev);
     PLS_CHECK_LAUNCH();
@@ -1060,6 +1074,60 @@ int pls_kdmap_nn_search(pls_context* ctx, const float* queries, int64_t n, float
     finish_out(ctx, onr);
     finish_out(ctx, oix);
     PLS_CUDA(cudaStreamSynchronize(ctx->stream));
+    PLS_API_END(ctx)
+}
+
+// A read-only look at the last search.  PLS_API_BEGIN_FRAME: a pending map update stays pending -- flushing it would
+// rebuild the index the stored positions refer to.
+int pls_kdmap_last_correspondences(pls_context* ctx, int64_t n, int64_t* out_idx, float* out_neighbors, float* out_normals,
+                                   float* out_search_state, double* out_sums) {
+    PLS_API_BEGIN_FRAME(ctx)
+    const KdMap& kd = ctx->kd;
+    if (!kd.searched) throw pls::Error{PLS_E_STATE, "pls_kdmap_last_correspondences: no kd search has run"};
+    if (!kd.valid || kd.searched_gen != kd.gen)
+        throw pls::Error{PLS_E_STATE, "pls_kdmap_last_correspondences: the map was rebuilt since the last search"};
+    if (kd.searched_sharded)
+        throw pls::Error{PLS_E_STATE, "pls_kdmap_last_correspondences: the last ICP split its queries over the ranks"};
+    cudaStream_t st = ctx->stream;
+    int64_t count = kd.searched_n;
+    if (kd.searched_icp) {
+        long long c = 0;
+        PLS_CUDA(cudaMemcpyAsync(&c, &frame_result_dev(ctx)->counts[1], sizeof(c), cudaMemcpyDeviceToHost, st));
+        PLS_CUDA(cudaStreamSynchronize(st));
+        count = (int64_t)c;
+    }
+    PLS_REQUIRE(n == count, "pls_kdmap_last_correspondences: n must be the query count of the last search");
+    if (n > 0 && (out_idx || out_neighbors || out_normals)) {
+        OutArg onb = out_arg(ctx, out_neighbors, (size_t)n * 3 * sizeof(float), ctx->stage_out[0]);
+        OutArg onr = out_arg(ctx, out_normals, (size_t)n * 3 * sizeof(float), ctx->stage_out[1]);
+        OutArg oix = out_arg(ctx, out_idx, (size_t)n * sizeof(int64_t), ctx->stage_out[2]);
+        float* nb = (float*)onb.dev;
+        if (!nb) {  // the export always writes the neighbours
+            ctx->stage_out[3].reserve((size_t)n * 3 * sizeof(float), st);
+            nb = ctx->stage_out[3].as<float>();
+        }
+        kd_search_export_kernel<<<grid_for(n, 256, 8 * kNumSMs), 256, 0, st>>>(
+            make_index(ctx), ctx->nn_prev.as<int>(), n, nb, kd.searched_normals ? (float*)onr.dev : nullptr,
+            (long long*)oix.dev);
+        PLS_CHECK_LAUNCH();
+        if (onr.dev && !kd.searched_normals)  // the search computed no normals: NaN
+            PLS_CUDA(cudaMemsetAsync(onr.dev, 0xff, onr.bytes, st));
+        finish_out(ctx, onb);
+        finish_out(ctx, onr);
+        finish_out(ctx, oix);
+    }
+    if (n > 0 && out_search_state)
+        PLS_CUDA(cudaMemcpyAsync(out_search_state, ctx->kd_nn_state.p, (size_t)n * sizeof(float4), cudaMemcpyDefault, st));
+    if (out_sums) {
+        if (kd.searched_icp) {
+            PLS_CUDA(cudaMemcpyAsync(out_sums, frame_result_dev(ctx)->last_sums, NACC * sizeof(double), cudaMemcpyDefault, st));
+        } else {
+            PLS_CUDA(cudaStreamSynchronize(st));
+            if (is_device_ptr(out_sums)) PLS_CUDA(cudaMemsetAsync(out_sums, 0xff, NACC * sizeof(double), st));
+            else memset(out_sums, 0xff, NACC * sizeof(double));
+        }
+    }
+    PLS_CUDA(cudaStreamSynchronize(st));
     PLS_API_END(ctx)
 }
 

@@ -312,6 +312,16 @@ def test_kd_exact_nn_vs_bruteforce(b200, M, N):
         dmin = dmin ** 2
     d_mine = ((q.astype(np.float64) - res.neighbor_points.astype(np.float64)) ** 2).sum(-1)
     np.testing.assert_allclose(d_mine, dmin, rtol=1e-5, atol=1e-9)
+    # the runner-up bound each search stored (what later ICP iterations verify against): every map point other than
+    # the match is at least sqrt(second) from the query position it stored
+    from pylidar_slam_b200 import _lib
+    from scipy.spatial import cKDTree
+    idx, state = np.empty(N, np.int64), np.empty((N, 4), np.float32)
+    lm.ctx.call("pls_kdmap_last_correspondences", N, _lib.ptr(idx), None, None, _lib.ptr(state), None)
+    assert np.array_equal(state[:, :3], q) and np.array_equal(m[idx], res.neighbor_points)
+    dd, ii = cKDTree(m.astype(np.float64)).query(q.astype(np.float64), k=2)
+    d_other = np.where(ii[:, 0] == idx, dd[:, 1], dd[:, 0])      # inf when the map has one point
+    assert (np.sqrt(state[:, 3].astype(np.float64)) <= d_other * 1.00001 + 1e-6).all()
 
 
 def test_a9_normals_per_point_bound(b200, syn):
