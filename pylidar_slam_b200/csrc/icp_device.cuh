@@ -6,13 +6,41 @@
 
 namespace pls {
 
-// Deterministic parallel sum of the block partial rows (THREADS = 256 or 128 threads, all must call): slice w of
+// Development builds only (-DPLS_KD_SPLIT, tools/kd_residual_split.py): %globaltimer and clock64 stamps of the kd
+// residual-and-solve phase, one record of KD_SPLIT_STAMPS (+ as many clock64 words) per block.  The default build
+// compiles none of it: PLS_SPLIT_ARG is empty and PLS_SPLIT(...) nothing.
+#ifdef PLS_KD_SPLIT
+constexpr int KD_SPLIT_STAMPS = 12;
+// `dep` only orders the stamp after the value it is given (no instruction of the stamp reads it)
+__device__ __forceinline__ unsigned long long split_now(double dep = 0.0) {
+    unsigned long long g;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(g) : "d"(dep) : "memory");
+    return g;
+}
+__device__ __forceinline__ void split_stamp(unsigned long long* rec, int i, double dep = 0.0) {
+    if (!rec) return;
+    rec[i] = split_now(dep);
+    rec[KD_SPLIT_STAMPS + i] = (unsigned long long)clock64();
+}
+#define PLS_SPLIT_ARG , unsigned long long* split = nullptr
+#define PLS_SPLIT_PASS , split
+#define PLS_SPLIT(...) split_stamp(split, __VA_ARGS__)
+#else
+#define PLS_SPLIT_ARG
+#define PLS_SPLIT_PASS
+#define PLS_SPLIT(...) \
+    do {           \
+    } while (0)
+#endif
+
+// Deterministic parallel sum of the block partial rows (THREADS = 512, 256 or 128 threads, all must call): slice w of
 // eight sums the rows w, w+8, ... of every accumulator (lane = accumulator, so a row is one coalesced 240-byte read and
 // the loads of a lane are independent), then the eight slices are added in fixed order -- the same additions in the
-// same order whatever the block size (a 128-thread block gives two slices to each warp).
+// same order whatever the block size (a 128-thread block gives two slices to each warp, a 512-thread block none to
+// its last eight).
 template <int THREADS = 256>
 __device__ __forceinline__ void sum_partials_256(const double* __restrict__ partials, int num_blocks, double* sums) {
-    static_assert(THREADS == 256 || THREADS == 128, "sum_partials: 4 or 8 warps");
+    static_assert(THREADS == 512 || THREADS == 256 || THREADS == 128, "sum_partials: 4, 8 or 16 warps");
     __shared__ double slice_sum[8][NACC];
     const int a = threadIdx.x & 31;
     if (a < NACC) {
@@ -43,7 +71,7 @@ __device__ __forceinline__ void sum_partials_256(const double* __restrict__ part
 }
 
 // The serial tail of an ICP iteration (thread 0): Gauss-Newton guards, 6x6 solve, stop test, pose update.
-__device__ __forceinline__ void icp_solve_and_update(FrameResult* fr, const double* sums, float threshold_delta) {
+__device__ __forceinline__ void icp_solve_and_update(FrameResult* fr, const double* sums, float threshold_delta PLS_SPLIT_ARG) {
     const int it = fr->iters;
     fr->iters = it + 1;
     // optimization.py:323-327: |r| < 1e-7 -> warning, x stays 0, the residuals are r^2.  The ICP loop then sees delta = 0:
@@ -64,6 +92,7 @@ __device__ __forceinline__ void icp_solve_and_update(FrameResult* fr, const doub
     }
     double dx[6];
     const double det = solve6(sums, dx);
+    PLS_SPLIT(7, det + dx[0] + dx[5]);
     if (!(fabs(det) >= 1e-7)) {  // optimization.py:334-336
         fr->status = PLS_E_SINGULAR;
         fr->done = 1;
@@ -78,6 +107,7 @@ __device__ __forceinline__ void icp_solve_and_update(FrameResult* fr, const doub
     }
     if (sqrtf(n2) < threshold_delta) {  // icp_odometry.py:292-293: the last delta is not applied
         fr->done = 1;
+        PLS_SPLIT(8, n2);
         return;
     }
     float dT[16], Tn[16], prm[6];
@@ -86,21 +116,24 @@ __device__ __forceinline__ void icp_solve_and_update(FrameResult* fr, const doub
     from_pose(Tn, prm);          // icp_odometry.py:296
     build_pose(prm, fr->T);      // icp_odometry.py:297
     for (int i = 0; i < 6; ++i) fr->params[i] = prm[i];
+    PLS_SPLIT(8, prm[5] + fr->T[10]);
 }
 
-// Called by every block of a correspondence kernel (256 or 128 threads) after it stored its partial row: the block
+// Called by every block of a correspondence kernel (512, 256 or 128 threads) after it stored its partial row: the block
 // that arrives last (ticket in fr->pad) sums all rows in the fixed order and runs the solve -- one launch
 // and one dependent-launch gap less per ICP iteration than a separate step kernel.
 template <int THREADS = 256>
 __device__ __forceinline__ void icp_finish_in_last_block(FrameResult* fr, const double* __restrict__ partials,
-                                                         float threshold_delta) {
+                                                         float threshold_delta PLS_SPLIT_ARG) {
     __shared__ int s_last;
     __shared__ double s_sums[NACC];
+    if (threadIdx.x == 0) PLS_SPLIT(4);
     __threadfence();  // this block's partial row is visible before its ticket
     __syncthreads();
     if (threadIdx.x == 0) {
         const int ticket = atomicAdd(&fr->pad, 1);
         s_last = ticket == (int)gridDim.x - 1;
+        PLS_SPLIT(5, (double)ticket);
     }
     __syncthreads();
     if (!s_last) return;
@@ -109,8 +142,9 @@ __device__ __forceinline__ void icp_finish_in_last_block(FrameResult* fr, const 
     __syncthreads();
     if (threadIdx.x < NACC) fr->last_sums[threadIdx.x] = s_sums[threadIdx.x];
     if (threadIdx.x != 0) return;
+    PLS_SPLIT(6, s_sums[0] + s_sums[29]);
     fr->pad = 0;
-    icp_solve_and_update(fr, s_sums, threshold_delta);
+    icp_solve_and_update(fr, s_sums, threshold_delta PLS_SPLIT_PASS);
 }
 
 }  // namespace pls

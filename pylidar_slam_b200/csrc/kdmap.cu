@@ -248,6 +248,46 @@ enum { KDC_NN_CAND = 0, KDC_KNN_CAND = 1, KDC_NORMALS = 2 };
 // filled by the next -- so no list is ever reset by a separate launch
 enum { KDL_PENDING = 0, KDL_HARD_NN = 2, KDL_WORDS = 4 };
 
+#ifdef PLS_KD_SPLIT
+// Stamp records of the residual-and-solve phase (tools/kd_residual_split.py): one per block of the launch of ICP
+// iteration 0..KD_SPLIT_ITERS-1, and one for a launch that found ICP converged (a no-op).  Stamps: 0 start, 1 start of
+// the residual phase, 2 / 3 the block's last thread done with its loads / its accumulation, 4 block partial stored,
+// 5 ticket taken; last block only: 6 rows summed, 7 solve done, 8 pose written.
+constexpr int KD_SPLIT_ITERS = 8;
+constexpr int KD_SPLIT_BLOCKS = 8 * kNumSMs;
+constexpr int KD_SPLIT_WORDS = (KD_SPLIT_ITERS + 1) * KD_SPLIT_BLOCKS * 2 * KD_SPLIT_STAMPS;
+__device__ unsigned long long g_kd_split[KD_SPLIT_WORDS];
+__device__ unsigned long long g_kd_split_normals_end;  // the last warp of kd_normals_warp_kernel to finish
+
+__device__ __forceinline__ unsigned long long* kd_split_record(const FrameResult* fr) {
+    const int slot = fr->done ? KD_SPLIT_ITERS : fr->iters;
+    if ((!fr->done && slot >= KD_SPLIT_ITERS) || blockIdx.x >= KD_SPLIT_BLOCKS) return nullptr;
+    return g_kd_split + ((size_t)slot * KD_SPLIT_BLOCKS + blockIdx.x) * 2 * KD_SPLIT_STAMPS;
+}
+#define KD_SPLIT_BEGIN()                             \
+    unsigned long long* split = kd_split_record(fr); \
+    __shared__ unsigned long long s_split[2];        \
+    if (threadIdx.x == 0) {                          \
+        PLS_SPLIT(0);                                \
+        s_split[0] = s_split[1] = 0;                 \
+        unsigned sm;                                 \
+        asm volatile("mov.u32 %0, %%smid;" : "=r"(sm)); \
+        if (split) split[11] = sm + 1;               \
+    }
+#define KD_SPLIT_MAX(k, dep) atomicMax(&s_split[k], split_now(dep))
+#define KD_SPLIT_BLOCK_MAX()         \
+    if (threadIdx.x == 0 && split) { \
+        split[2] = s_split[0];       \
+        split[3] = s_split[1];       \
+    }
+#else
+#define KD_SPLIT_BEGIN()
+#define KD_SPLIT_MAX(k, dep) \
+    do {                     \
+    } while (0)
+#define KD_SPLIT_BLOCK_MAX()
+#endif
+
 // Appends this block's entries (collected in shared memory by any of its threads) to a global list: one atomic per block.
 __device__ __forceinline__ void block_flush_list(const int* s_list, int n, int* __restrict__ list, uint32_t* count, int* s_base) {
     if (n == 0) return;  // block-uniform
@@ -442,6 +482,9 @@ kd_normals_warp_kernel(KdIndex ix, int k_normals, const int* __restrict__ workli
         atomicAdd(counters + KDC_KNN_CAND, (unsigned long long)cand);
         atomicAdd(counters + KDC_NORMALS, (unsigned long long)done_here);
     }
+#ifdef PLS_KD_SPLIT
+    if (lane == 0) atomicMax(&g_kd_split_normals_end, split_now((double)done_here));
+#endif
 }
 
 constexpr int KD_RES_THREADS = 256;
@@ -450,10 +493,12 @@ __global__ void __launch_bounds__(KD_RES_THREADS)
 kd_residual_kernel(KdIndex ix, const float4* __restrict__ queries, const uint32_t* __restrict__ nq_dev, int64_t q_begin,
                    int64_t q_stride, FrameResult* fr, int scheme, float sigma,
                    const int* __restrict__ match, double* __restrict__ partials, float fuse_threshold) {
+    KD_SPLIT_BEGIN()
     if (fr->done) return;
     __shared__ float sT[12];
     if (threadIdx.x < 12) sT[threadIdx.x] = fr->T[threadIdx.x];
     __syncthreads();
+    if (threadIdx.x == 0) PLS_SPLIT(1);
     const int64_t nq = (int64_t)*nq_dev;
     double acc[NACC];
 #pragma unroll
@@ -474,11 +519,18 @@ kd_residual_kernel(KdIndex ix, const float4* __restrict__ queries, const uint32_
         float nn[3] = {nv.x, nv.y, nv.z};
         float J[6];
         const float r = p2plane_residual_jacobian_identity(p, q, nn, J);
+        KD_SPLIT_MAX(0, r);
         const float w = ls_weight<float>(scheme, sigma, r, p, q);
         accumulate_normal_equations<float>(acc, J, w, r * w, r);
     }
+    KD_SPLIT_MAX(1, acc[0] + acc[29]);
+    // The shuffle tree must start on a converged warp.  The grid's last block holds a warp whose lanes left the query
+    // loop at different iterations; without this it took the divergent-warp path of the 30 x 5 shuffles, 35 us on H100
+    // (profiles/h100_kd_residual_split_before.log) while every other block took 1.2 us -- and the solve waits for it.
+    __syncwarp();
     block_reduce_store<KD_RES_THREADS>(acc, partials + (size_t)blockIdx.x * NACC);
-    if (fuse_threshold >= 0.f) icp_finish_in_last_block(fr, partials, fuse_threshold);
+    KD_SPLIT_BLOCK_MAX()
+    if (fuse_threshold >= 0.f) icp_finish_in_last_block(fr, partials, fuse_threshold PLS_SPLIT_PASS);
 }
 
 // ICP iterations after a frame's first, in ONE launch.  Each block takes the queries kd_residual_kernel would give it
@@ -494,18 +546,26 @@ kd_residual_kernel(KdIndex ix, const float4* __restrict__ queries, const uint32_
 //      bits, and no block ever waits for another;
 //   3. once every round is searched, a thread per query: residual, Jacobian, weight, fp64 accumulation -- then the block
 //      partial and, fused, the solve in the last block.  The accumulators are not live during the searches.
-__global__ void __launch_bounds__(KD_THREADS)
+// A block has KD_REFINE_THREADS threads: the first KD_THREADS own the queries (steps 1 and 3, the block partial of
+// kd_residual_kernel's geometry), all of its warps share the searches of step 2.  A cfg2 block re-searches 13 queries
+// and computes 4 normals in the median, 30 and 13 at most (profiles/h100_kd_residual_split_after.log): with 8 warps
+// the slowest block's searches took 35 us, a chain of up to four searches per warp.
+constexpr int KD_REFINE_THREADS = 512;
+constexpr int KD_REFINE_WARPS = KD_REFINE_THREADS / 32;
+__global__ void __launch_bounds__(KD_REFINE_THREADS)
 kd_icp_refine_kernel(KdIndex ix, const float4* __restrict__ queries, const uint32_t* __restrict__ nq_dev, int64_t q_begin,
                      int64_t q_stride, FrameResult* fr, int scheme, float sigma, int k_normals, int* __restrict__ match,
                      float4* __restrict__ nn_state, double* __restrict__ partials, float fuse_threshold,
                      unsigned long long* __restrict__ counters) {
+    KD_SPLIT_BEGIN()
     if (fr->done) return;
     __shared__ float sT[12];
     __shared__ int s_hard[KD_THREADS];
     __shared__ int s_nh;
-    __shared__ unsigned long long s_stage[KD_WARPS][KNN_STAGE];
+    __shared__ unsigned long long s_stage[KD_REFINE_WARPS][KNN_STAGE];
     if (threadIdx.x < 12) sT[threadIdx.x] = fr->T[threadIdx.x];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const bool owner = threadIdx.x < KD_THREADS;  // warp-uniform: this thread has a query slot
     const int64_t nq = (int64_t)*nq_dev;
     const uint32_t valid = kd_normal_valid(ix.gen);
     int cand_nn = 0, cand_knn = 0, normals_here = 0;
@@ -514,7 +574,7 @@ kd_icp_refine_kernel(KdIndex ix, const float4* __restrict__ queries, const uint3
         if (threadIdx.x == 0) s_nh = 0;
         __syncthreads();
         const int64_t qi = q_begin + (round + threadIdx.x) * q_stride;
-        if (qi < nq) {
+        if (owner && qi < nq) {
             const float4 p0 = queries[qi];
             const float px = p0.x * sT[0] + p0.y * sT[1] + p0.z * sT[2] + sT[3];
             const float py = p0.x * sT[4] + p0.y * sT[5] + p0.z * sT[6] + sT[7];
@@ -531,9 +591,12 @@ kd_icp_refine_kernel(KdIndex ix, const float4* __restrict__ queries, const uint3
         }
         __syncthreads();
         const int nh = s_nh;
+#ifdef PLS_KD_SPLIT
+        if (threadIdx.x == 0 && split) split[9] += (unsigned long long)nh;  // not a time: the block's re-searches
+#endif
         if (warp < nh) {
             const KdGridLocal g = kd_load_grid(ix);
-            for (int e = warp; e < nh; e += KD_WARPS) {
+            for (int e = warp; e < nh; e += KD_REFINE_WARPS) {
                 const int64_t q = q_begin + (round + s_hard[e]) * q_stride;
                 const float4 p0 = queries[q];
                 const float px = p0.x * sT[0] + p0.y * sT[1] + p0.z * sT[2] + sT[3];
@@ -568,11 +631,15 @@ kd_icp_refine_kernel(KdIndex ix, const float4* __restrict__ queries, const uint3
         if (cand_knn) atomicAdd(counters + KDC_KNN_CAND, (unsigned long long)cand_knn);
         if (normals_here) atomicAdd(counters + KDC_NORMALS, (unsigned long long)normals_here);
     }
+#ifdef PLS_KD_SPLIT
+    if (lane == 0 && split && normals_here) atomicAdd(split + 10, (unsigned long long)normals_here);  // normals computed
+#endif
     // every match and normal of this block's queries is in place (the last round ended on a barrier)
+    if (threadIdx.x == 0) PLS_SPLIT(1);
     double acc[NACC];
 #pragma unroll
     for (int a = 0; a < NACC; ++a) acc[a] = 0.0;
-    for (int64_t s = (int64_t)blockIdx.x * KD_THREADS + threadIdx.x;; s += (int64_t)gridDim.x * KD_THREADS) {
+    for (int64_t s = (int64_t)blockIdx.x * KD_THREADS + threadIdx.x; owner; s += (int64_t)gridDim.x * KD_THREADS) {
         const int64_t qi = q_begin + s * q_stride;
         if (qi >= nq) break;
         const int pos = match[qi];
@@ -588,11 +655,18 @@ kd_icp_refine_kernel(KdIndex ix, const float4* __restrict__ queries, const uint3
         float nn[3] = {nv.x, nv.y, nv.z};
         float J[6];
         const float r = p2plane_residual_jacobian_identity(p, q, nn, J);
+        KD_SPLIT_MAX(0, r);
         const float w = ls_weight<float>(scheme, sigma, r, p, q);
         accumulate_normal_equations<float>(acc, J, w, r * w, r);
     }
-    block_reduce_store<KD_RES_THREADS>(acc, partials + (size_t)blockIdx.x * NACC);
-    if (fuse_threshold >= 0.f) icp_finish_in_last_block(fr, partials, fuse_threshold);
+    KD_SPLIT_MAX(1, acc[0] + acc[29]);
+    // The shuffle tree must start on a converged warp.  The grid's last block holds a warp whose lanes left the query
+    // loop at different iterations; without this it took the divergent-warp path of the 30 x 5 shuffles, 35 us on H100
+    // (profiles/h100_kd_residual_split_before.log) while every other block took 1.2 us -- and the solve waits for it.
+    __syncwarp();
+    block_reduce_store<KD_REFINE_THREADS, KD_WARPS>(acc, partials + (size_t)blockIdx.x * NACC);
+    KD_SPLIT_BLOCK_MAX()
+    if (fuse_threshold >= 0.f) icp_finish_in_last_block<KD_REFINE_THREADS>(fr, partials, fuse_threshold PLS_SPLIT_PASS);
 }
 
 // Fine-grained API: [n,3] rows -> float4 queries (no row is dropped: outputs stay aligned with the inputs)
@@ -956,7 +1030,7 @@ int kdmap_icp_iteration(pls_context* ctx, int64_t query_bound, int rank, int num
         PLS_CHECK_LAUNCH();
     } else {
         ProfileScope p11(ctx, 11, 0.0);
-        kd_icp_refine_kernel<<<blocks, KD_THREADS, 0, st>>>(ix, ctx->query_ptr, nq_dev, (int64_t)rank, (int64_t)num_ranks, fr,
+        kd_icp_refine_kernel<<<blocks, KD_REFINE_THREADS, 0, st>>>(ix, ctx->query_ptr, nq_dev, (int64_t)rank, (int64_t)num_ranks, fr,
                                                             ctx->cfg.scheme, ctx->cfg.sigma, ctx->cfg.num_neighbors_normals,
                                                             ctx->nn_prev.as<int>(), ctx->kd_nn_state.as<float4>(),
                                                             ctx->partials.as<double>(), fuse_threshold, kd_counters(ctx));
@@ -1130,5 +1204,23 @@ int pls_kdmap_last_correspondences(pls_context* ctx, int64_t n, int64_t* out_idx
     PLS_CUDA(cudaStreamSynchronize(st));
     PLS_API_END(ctx)
 }
+
+#ifdef PLS_KD_SPLIT
+// Development builds only: copies the stamp records (KD_SPLIT_WORDS words, then the normals kernel's end) to `out`
+// and clears them.  `words` must be KD_SPLIT_WORDS + 1.
+PLS_API int pls_debug_kd_split(pls_context* ctx, unsigned long long* out, int64_t words) {
+    PLS_API_BEGIN(ctx)
+    PLS_REQUIRE(out && words == (int64_t)KD_SPLIT_WORDS + 1, "pls_debug_kd_split: bad arguments");
+    sync_all(ctx);
+    PLS_CUDA(cudaMemcpyFromSymbol(out, g_kd_split, KD_SPLIT_WORDS * sizeof(unsigned long long)));
+    PLS_CUDA(cudaMemcpyFromSymbol(out + KD_SPLIT_WORDS, g_kd_split_normals_end, sizeof(unsigned long long)));
+    static const unsigned long long zero = 0;
+    void* p = nullptr;
+    PLS_CUDA(cudaGetSymbolAddress(&p, g_kd_split));
+    PLS_CUDA(cudaMemset(p, 0, KD_SPLIT_WORDS * sizeof(unsigned long long)));
+    PLS_CUDA(cudaMemcpyToSymbol(g_kd_split_normals_end, &zero, sizeof(zero)));
+    PLS_API_END(ctx)
+}
+#endif
 
 }  // extern "C"
