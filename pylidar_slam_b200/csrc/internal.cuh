@@ -380,8 +380,9 @@ int kdmap_icp_iteration(pls_context* ctx, int64_t query_bound, int rank, int num
 // pack [n,3] rows without NaN into float4 (stable); count -> *count_dev (u32)
 void pack_valid_rows(pls_context* ctx, const float* pts_dev, int64_t n, float4* out, uint32_t* count_dev);
 void pack_valid_rows_f64(pls_context* ctx, const double* pts_dev, int64_t n, float4* out, uint32_t* count_dev);
-// pack the non-null pixels (any channel != 0) of a [3,H,W] map into float4, row-major order
-void pack_nonnull_pixels(pls_context* ctx, const float* vmap_dev, int64_t hw, float4* out, uint32_t* count_dev);
+// pack the pixels of a [3,H,W] map with |p| > min_norm (NaN dropped) into float4, row-major order
+void pack_valid_pixels(pls_context* ctx, const float* vmap_dev, int64_t hw, float min_norm, float4* out,
+                       uint32_t* count_dev);
 // grid_sample.cu
 // compact = true sorts on 40-bit keys (5 radix passes instead of 8): exact whenever every hash lies in [-2^39, 2^39),
 // i.e. voxel coordinates up to ~3 000 000 in magnitude; otherwise the kernel stamps `gs_seq` into the device scalar

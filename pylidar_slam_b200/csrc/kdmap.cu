@@ -9,10 +9,8 @@
 //   radix sort (4 passes)   primitives.cu (stable: insertion order inside a cell)
 //   kd_finalize_kernel      sorted float4 copy + the hashed cell tables of all levels
 // Tables and cached normals carry the build's generation number: nothing is cleared between frames.
-// Search (local_map.py:372-422): whole warps per query, see kdmap_device.cuh.  A frame's first ICP iteration = three
-// launches (kd_nn_warp_kernel, kd_normals_warp_kernel, kd_residual_kernel which also runs the solve in its last block);
-// every later iteration = one (kd_icp_refine_kernel) or, on maps of KD_COLD_MAP_POINTS or more, four (verify, 1-NN of the
-// unproven queries, normals, residual).
+// Search (local_map.py:372-422): whole warps per query, see kdmap_device.cuh.  The kernels of one ICP iteration are
+// listed below, under "one ICP iteration on the kd map".
 #include <stdlib.h>
 
 #include "gn_device.cuh"
@@ -104,12 +102,12 @@ __global__ void kd_pack_rows_kernel(const T* __restrict__ pts, int64_t n, const 
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
         if (flags[i]) out[pos[i]] = make_float4((float)pts[3 * i], (float)pts[3 * i + 1], (float)pts[3 * i + 2], 0.f);
 }
-// vertex map [3,H,W] -> pixels with |p| > 0.01 and no NaN (local_map.py:320-328)
-__global__ void kd_valid_pixels_kernel(const float* __restrict__ vmap, int64_t hw, uint8_t* __restrict__ flags) {
+// vertex map [3,H,W] -> pixels with |p| > min_norm and no NaN
+__global__ void kd_valid_pixels_kernel(const float* __restrict__ vmap, int64_t hw, float min_norm,
+                                       uint8_t* __restrict__ flags) {
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < hw; i += (int64_t)gridDim.x * blockDim.x) {
         float x = vmap[i], y = vmap[hw + i], z = vmap[2 * hw + i];
-        float nrm = sqrtf(x * x + y * y + z * z);
-        flags[i] = (nrm > 0.01f) ? 1 : 0;  // NaN compares false
+        flags[i] = (sqrtf(x * x + y * y + z * z) > min_norm) ? 1 : 0;  // NaN compares false
     }
 }
 __global__ void kd_pack_pixels_kernel(const float* __restrict__ vmap, int64_t hw, const uint8_t* __restrict__ flags,
@@ -227,16 +225,12 @@ __global__ void kd_export_kernel(const float4* __restrict__ pts, int64_t n, floa
 }
 
 // ---- one ICP iteration on the kd map (icp_odometry.py:275-284 + alignment.py:91-127 at x0 = 0) -----------------------
-//   p = T p0; q = NN(p); n = normal(q); r = n.(p - q); J = [n, p x n]; w; reduce        -- three launches:
-//   kd_nn_verify_kernel     (iterations after a frame's first) a thread per query proves that its previous match is
-//                           still the nearest neighbour; the unproven ones are queued
-//   kd_nn_warp_kernel       transform, exact 1-NN -> match[qi] for every query (first iteration) or the queued ones: a
-//                           warp per query over the cell pyramid; the first to match a map point whose normal is not
-//                           cached claims it (CAS on the state word) and queues it (warp-aggregated appends)
-//   kd_normals_warp_kernel  exact (k+1)-NN of every queued map point, second moments, lane-parallel eigen-solves
-//   kd_residual_kernel      a thread per query: r, J, robust weight, the 30 fp64 accumulators -> block partials; the
-//                           last block sums them in fixed order and runs the solve / stop test / pose update
-// Below KD_COLD_MAP_POINTS, the iterations after a frame's first run all of that as ONE launch, kd_icp_refine_kernel.
+//   p = T p0; q = NN(p); n = normal(q); r = n.(p - q); J = [n, p x n]; w; reduce
+// A frame's first iteration is three launches: kd_nn_warp_kernel, kd_normals_warp_kernel and kd_residual_kernel, which
+// also runs the solve in its last block.  Every later iteration is one launch, kd_icp_refine_kernel, or, on maps of
+// KD_COLD_MAP_POINTS or more, four: kd_nn_verify_kernel and the same three on the queries it could not prove.
+// KD_THREADS is the block size of the kernels that own a thread per query, and the number of query slots of a
+// kd_icp_refine_kernel block: both striding and block partials follow from it.
 constexpr int KD_THREADS = 256;
 constexpr int KD_WARPS = KD_THREADS / 32;
 
@@ -280,12 +274,17 @@ __device__ __forceinline__ unsigned long long* kd_split_record(const FrameResult
         split[2] = s_split[0];       \
         split[3] = s_split[1];       \
     }
+// the record and the block's shared maxima, into the device helpers that stamp
+#define KD_SPLIT_ARG , unsigned long long* split, unsigned long long* s_split
+#define KD_SPLIT_PASS , split, s_split
 #else
 #define KD_SPLIT_BEGIN()
 #define KD_SPLIT_MAX(k, dep) \
     do {                     \
     } while (0)
 #define KD_SPLIT_BLOCK_MAX()
+#define KD_SPLIT_ARG
+#define KD_SPLIT_PASS
 #endif
 
 // Appends this block's entries (collected in shared memory by any of its threads) to a global list: one atomic per block.
@@ -304,11 +303,74 @@ __device__ __forceinline__ bool claim_normal(const KdIndex& ix, int pos) {
     return cur != valid && cur != claimed && atomicCAS(w, cur, claimed) == cur;
 }
 
-// 1-NN of ICP iterations after a frame's first: VERIFY instead of searching.  The full search stored, per query, where
-// the query stood (its transformed position) and a lower bound of the distance to every map point other than its match.
-// If the query has moved by eps since then and its match is now at distance d, every other point is still at least
-// (bound - eps) away, so d + eps < bound proves the match unchanged -- one point load and a dozen flops per query.
-// The few queries that cannot be proven are queued for the full search.
+// p = T p0, T the first three rows of a row-major 4x4 pose.
+__device__ __forceinline__ void transform_query(const float* T, const float4& p0, float* p) {
+    p[0] = p0.x * T[0] + p0.y * T[1] + p0.z * T[2] + T[3];
+    p[1] = p0.x * T[4] + p0.y * T[5] + p0.z * T[6] + T[7];
+    p[2] = p0.x * T[8] + p0.y * T[9] + p0.z * T[10] + T[11];
+}
+
+// 1-NN of ICP iterations after a frame's first: VERIFY instead of searching.  The full search stored in `state` where
+// the query stood (xyz, its transformed position) and in .w a lower bound of the squared distance to every map point
+// other than its match.  If the query, now at p, has moved by eps since then and its match `pos` is now at distance d,
+// every other point is still at least (bound - eps) away, so d + eps < bound proves the match unchanged -- one point
+// load and a dozen flops per query.  False when there is no match (pos < 0).
+__device__ __forceinline__ bool match_proven(const KdIndex& ix, const float* p, int pos, const float4& state) {
+    if (pos < 0) return false;
+    const float4 s = state;
+    const float d = sqrtf(dist2_point(p[0], p[1], p[2], __ldg(ix.sorted + pos)));
+    const float eps = sqrtf(dist2_point(p[0], p[1], p[2], s));
+    return (d + eps) * 1.00001f + 1e-6f < sqrtf(s.w);
+}
+
+// Second moments of map point c's k nearest OTHER map points, from its exact (k+1)-NN by the whole warp.
+__device__ __forceinline__ void warp_normal_moments(const KdIndex& ix, const KdGridLocal& g, const float4& c, int k, int lane,
+                                                    int* cand, unsigned long long* stage, float* cov) {
+    int ni;
+    const int found = warp_knn(ix, g, c.x, c.y, c.z, k + 1, lane, ni, cand, stage);
+    warp_second_moments(ix, c, k, found, ni, lane, cov);
+}
+
+// The normal of map point `pos` from its second moments, stored with `valid`, the state word kd_normal_valid(ix.gen).
+__device__ __forceinline__ void store_normal(const KdIndex& ix, int pos, const float* cov, uint32_t valid) {
+    float nn[3];
+    smallest_eigenvector(cov, nn);
+    __stcg(ix.normals + pos, make_float4(nn[0], nn[1], nn[2], __uint_as_float(valid)));
+}
+
+// A matched query's (p = T p0, match `pos`) share of the normal equations: residual, Jacobian, robust weight, fp64
+// accumulation.
+__device__ __forceinline__ void accumulate_match(double* acc, const KdIndex& ix, const float* p, int pos, int scheme,
+                                                 float sigma KD_SPLIT_ARG) {
+    const float4 qq = __ldg(ix.sorted + pos);
+    const float4 nv = __ldcg(ix.normals + pos);
+    float q[3] = {qq.x, qq.y, qq.z};
+    float nn[3] = {nv.x, nv.y, nv.z};
+    float J[6];
+    const float r = p2plane_residual_jacobian_identity(p, q, nn, J);
+    KD_SPLIT_MAX(0, r);
+    const float w = ls_weight<float>(scheme, sigma, r, p, q);
+    accumulate_normal_equations<float>(acc, J, w, r * w, r);
+}
+
+// The end of a residual phase, called by every thread of a THREADS-thread block whose first KD_WARPS warps hold
+// accumulators: the block partial row, then (fuse_threshold >= 0) the fixed-order sum and the solve in the grid's last
+// block.
+template <int THREADS>
+__device__ __forceinline__ void block_partial_and_finish(double* acc, FrameResult* fr, double* __restrict__ partials,
+                                                         float fuse_threshold KD_SPLIT_ARG) {
+    KD_SPLIT_MAX(1, acc[0] + acc[29]);
+    // The shuffle tree must start on a converged warp.  The grid's last block holds a warp whose lanes left the query
+    // loop at different iterations; without this it took the divergent-warp path of the 30 x 5 shuffles, 35 us on H100
+    // (profiles/h100_kd_residual_split_before.log) while every other block took 1.2 us -- and the solve waits for it.
+    __syncwarp();
+    block_reduce_store<THREADS, KD_WARPS>(acc, partials + (size_t)blockIdx.x * NACC);
+    KD_SPLIT_BLOCK_MAX()
+    if (fuse_threshold >= 0.f) icp_finish_in_last_block<THREADS>(fr, partials, fuse_threshold PLS_SPLIT_PASS);
+}
+
+// Iterations after a frame's first on maps of KD_COLD_MAP_POINTS or more: a thread per query keeps its previous match
+// if match_proven; the few others are queued for kd_nn_warp_kernel.
 __global__ void __launch_bounds__(KD_THREADS)
 kd_nn_verify_kernel(KdIndex ix, const float4* __restrict__ queries, const uint32_t* __restrict__ nq_dev, int64_t q_begin,
                     int64_t q_stride, const float* __restrict__ T, const int* __restrict__ done, const int* __restrict__ match,
@@ -327,19 +389,9 @@ kd_nn_verify_kernel(KdIndex ix, const float4* __restrict__ queries, const uint32
     const int64_t nq = (int64_t)*nq_dev;
     const int64_t qi = q_begin + ((int64_t)blockIdx.x * KD_THREADS + threadIdx.x) * q_stride;
     if (qi < nq) {
-        const float4 p0 = queries[qi];
-        const float px = p0.x * sT[0] + p0.y * sT[1] + p0.z * sT[2] + sT[3];
-        const float py = p0.x * sT[4] + p0.y * sT[5] + p0.z * sT[6] + sT[7];
-        const float pz = p0.x * sT[8] + p0.y * sT[9] + p0.z * sT[10] + sT[11];
-        const int pos = match[qi];
-        bool proven = false;
-        if (pos >= 0) {
-            const float4 s = nn_state[qi];
-            const float d = sqrtf(dist2_point(px, py, pz, __ldg(ix.sorted + pos)));
-            const float eps = sqrtf(dist2_point(px, py, pz, s));
-            proven = (d + eps) * 1.00001f + 1e-6f < sqrtf(s.w);
-        }
-        if (!proven) s_hard[atomicAdd(&s_nh, 1)] = (int)qi;
+        float p[3];
+        transform_query(sT, queries[qi], p);
+        if (!match_proven(ix, p, match[qi], nn_state[qi])) s_hard[atomicAdd(&s_nh, 1)] = (int)qi;
     }
     __syncthreads();
     block_flush_list(s_hard, s_nh, hard, lists + KDL_HARD_NN + parity, &s_base);
@@ -401,14 +453,13 @@ kd_nn_warp_kernel(KdIndex ix, const float4* __restrict__ queries, const uint32_t
             pn = queries[qn];
             if (hard) hn = match[qn];
         }
-        const float px = p0.x * t[0] + p0.y * t[1] + p0.z * t[2] + t[3];
-        const float py = p0.x * t[4] + p0.y * t[5] + p0.z * t[6] + t[7];
-        const float pz = p0.x * t[8] + p0.y * t[9] + p0.z * t[10] + t[11];
+        float p[3];
+        transform_query(t, p0, p);
         float second;
-        const int pos = warp_nearest(ix, g, px, py, pz, hint, lane, &cand, &second);
+        const int pos = warp_nearest(ix, g, p[0], p[1], p[2], hint, lane, &cand, &second);
         if (lane == 0) {
             match[qi] = pos;
-            if (nn_state) nn_state[qi] = make_float4(px, py, pz, second);
+            if (nn_state) nn_state[qi] = make_float4(p[0], p[1], p[2], second);
         }
         if (lane == held) my_pos = pos;
         if (++held == 32) flush_claims();
@@ -436,7 +487,7 @@ kd_normals_warp_kernel(KdIndex ix, int k_normals, const int* __restrict__ workli
     if (warp_global >= n) return;
     unsigned long long* stage = s_stage[threadIdx.x >> 5];
     const KdGridLocal g = kd_load_grid(ix);
-    const float valid = __uint_as_float(kd_normal_valid(ix.gen));
+    const uint32_t valid = kd_normal_valid(ix.gen);
     float mycov[6];
     int mypos = -1, held = 0, cand = 0, done_here = 0;
     int e = warp_global;
@@ -451,10 +502,8 @@ kd_normals_warp_kernel(KdIndex ix, int k_normals, const int* __restrict__ workli
             posn = worklist[en];
             cn = __ldg(ix.sorted + posn);
         }
-        int ni;
-        const int found = warp_knn(ix, g, c.x, c.y, c.z, k_normals + 1, lane, ni, &cand, stage);
         float cov[6];
-        warp_second_moments(ix, c, k_normals, found, ni, lane, cov);
+        warp_normal_moments(ix, g, c, k_normals, lane, &cand, stage, cov);
         if (lane == held) {
 #pragma unroll
             for (int a = 0; a < 6; ++a) mycov[a] = cov[a];
@@ -462,9 +511,7 @@ kd_normals_warp_kernel(KdIndex ix, int k_normals, const int* __restrict__ workli
         }
         ++done_here;
         if (++held == 32) {  // 32 moments collected: every lane solves its own
-            float nn[3];
-            smallest_eigenvector(mycov, nn);
-            __stcg(ix.normals + mypos, make_float4(nn[0], nn[1], nn[2], valid));
+            store_normal(ix, mypos, mycov, valid);
             held = 0;
             mypos = -1;
         }
@@ -473,11 +520,7 @@ kd_normals_warp_kernel(KdIndex ix, int k_normals, const int* __restrict__ workli
         pos = posn;
         c = cn;
     }
-    if (mypos >= 0) {
-        float nn[3];
-        smallest_eigenvector(mycov, nn);
-        __stcg(ix.normals + mypos, make_float4(nn[0], nn[1], nn[2], valid));
-    }
+    if (mypos >= 0) store_normal(ix, mypos, mycov, valid);
     if (counters && lane == 0) {
         atomicAdd(counters + KDC_KNN_CAND, (unsigned long long)cand);
         atomicAdd(counters + KDC_NORMALS, (unsigned long long)done_here);
@@ -487,9 +530,9 @@ kd_normals_warp_kernel(KdIndex ix, int k_normals, const int* __restrict__ workli
 #endif
 }
 
-constexpr int KD_RES_THREADS = 256;
-
-__global__ void __launch_bounds__(KD_RES_THREADS)
+// A thread per query: accumulate_match -> block partials; the last block sums them in fixed order and runs the solve,
+// stop test and pose update.
+__global__ void __launch_bounds__(KD_THREADS)
 kd_residual_kernel(KdIndex ix, const float4* __restrict__ queries, const uint32_t* __restrict__ nq_dev, int64_t q_begin,
                    int64_t q_stride, FrameResult* fr, int scheme, float sigma,
                    const int* __restrict__ match, double* __restrict__ partials, float fuse_threshold) {
@@ -506,46 +549,23 @@ kd_residual_kernel(KdIndex ix, const float4* __restrict__ queries, const uint32_
     for (int64_t s = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;; s += (int64_t)gridDim.x * blockDim.x) {
         const int64_t qi = q_begin + s * q_stride;
         if (qi >= nq) break;
-        const float4 p0 = queries[qi];
         float p[3];
-        p[0] = p0.x * sT[0] + p0.y * sT[1] + p0.z * sT[2] + sT[3];
-        p[1] = p0.x * sT[4] + p0.y * sT[5] + p0.z * sT[6] + sT[7];
-        p[2] = p0.x * sT[8] + p0.y * sT[9] + p0.z * sT[10] + sT[11];
+        transform_query(sT, queries[qi], p);
         const int pos = match[qi];
         if (pos < 0) continue;
-        const float4 qq = __ldg(ix.sorted + pos);
-        const float4 nv = __ldcg(ix.normals + pos);
-        float q[3] = {qq.x, qq.y, qq.z};
-        float nn[3] = {nv.x, nv.y, nv.z};
-        float J[6];
-        const float r = p2plane_residual_jacobian_identity(p, q, nn, J);
-        KD_SPLIT_MAX(0, r);
-        const float w = ls_weight<float>(scheme, sigma, r, p, q);
-        accumulate_normal_equations<float>(acc, J, w, r * w, r);
+        accumulate_match(acc, ix, p, pos, scheme, sigma KD_SPLIT_PASS);
     }
-    KD_SPLIT_MAX(1, acc[0] + acc[29]);
-    // The shuffle tree must start on a converged warp.  The grid's last block holds a warp whose lanes left the query
-    // loop at different iterations; without this it took the divergent-warp path of the 30 x 5 shuffles, 35 us on H100
-    // (profiles/h100_kd_residual_split_before.log) while every other block took 1.2 us -- and the solve waits for it.
-    __syncwarp();
-    block_reduce_store<KD_RES_THREADS>(acc, partials + (size_t)blockIdx.x * NACC);
-    KD_SPLIT_BLOCK_MAX()
-    if (fuse_threshold >= 0.f) icp_finish_in_last_block(fr, partials, fuse_threshold PLS_SPLIT_PASS);
+    block_partial_and_finish<KD_THREADS>(acc, fr, partials, fuse_threshold KD_SPLIT_PASS);
 }
 
 // ICP iterations after a frame's first, in ONE launch.  Each block takes the queries kd_residual_kernel would give it
 // (same grid, same striding, so the block partials are the same bits):
-//   1. per round of 256 of them, a thread per query VERIFIES instead of searching.  The full search stored, per query,
-//      where the query stood (its transformed position) and a lower bound of the distance to every map point other
-//      than its match.  If the query has moved by eps since then and its match is now at distance d, every other point
-//      is still at least (bound - eps) away, so d + eps < bound proves the match unchanged -- one point load and a
-//      dozen flops per query;
+//   1. per round of KD_THREADS of them, a thread per query keeps its previous match if match_proven;
 //   2. the block's warps re-search the round's unproven queries (warp_nearest, seeded with the previous match) and
-//      compute the normal of every new match that has none cached (warp_knn, second moments, eigen-solve).  Another
-//      block may compute the same normal at the same time: the computation is deterministic, so both store the same
-//      bits, and no block ever waits for another;
-//   3. once every round is searched, a thread per query: residual, Jacobian, weight, fp64 accumulation -- then the block
-//      partial and, fused, the solve in the last block.  The accumulators are not live during the searches.
+//      compute the normal of every new match that has none cached.  Another block may compute the same normal at the
+//      same time: the computation is deterministic, so both store the same bits, and no block ever waits for another;
+//   3. once every round is searched, a thread per query: accumulate_match, then the block partial and, fused, the
+//      solve in the last block.  The accumulators are not live during the searches.
 // A block has KD_REFINE_THREADS threads: the first KD_THREADS own the queries (steps 1 and 3, the block partial of
 // kd_residual_kernel's geometry), all of its warps share the searches of step 2.  A cfg2 block re-searches 13 queries
 // and computes 4 normals in the median, 30 and 13 at most (profiles/h100_kd_residual_split_after.log): with 8 warps
@@ -575,19 +595,9 @@ kd_icp_refine_kernel(KdIndex ix, const float4* __restrict__ queries, const uint3
         __syncthreads();
         const int64_t qi = q_begin + (round + threadIdx.x) * q_stride;
         if (owner && qi < nq) {
-            const float4 p0 = queries[qi];
-            const float px = p0.x * sT[0] + p0.y * sT[1] + p0.z * sT[2] + sT[3];
-            const float py = p0.x * sT[4] + p0.y * sT[5] + p0.z * sT[6] + sT[7];
-            const float pz = p0.x * sT[8] + p0.y * sT[9] + p0.z * sT[10] + sT[11];
-            const int pos = match[qi];
-            bool proven = false;
-            if (pos >= 0) {
-                const float4 s = nn_state[qi];
-                const float d = sqrtf(dist2_point(px, py, pz, __ldg(ix.sorted + pos)));
-                const float eps = sqrtf(dist2_point(px, py, pz, s));
-                proven = (d + eps) * 1.00001f + 1e-6f < sqrtf(s.w);
-            }
-            if (!proven) s_hard[atomicAdd(&s_nh, 1)] = threadIdx.x;
+            float p[3];
+            transform_query(sT, queries[qi], p);
+            if (!match_proven(ix, p, match[qi], nn_state[qi])) s_hard[atomicAdd(&s_nh, 1)] = threadIdx.x;
         }
         __syncthreads();
         const int nh = s_nh;
@@ -598,29 +608,20 @@ kd_icp_refine_kernel(KdIndex ix, const float4* __restrict__ queries, const uint3
             const KdGridLocal g = kd_load_grid(ix);
             for (int e = warp; e < nh; e += KD_REFINE_WARPS) {
                 const int64_t q = q_begin + (round + s_hard[e]) * q_stride;
-                const float4 p0 = queries[q];
-                const float px = p0.x * sT[0] + p0.y * sT[1] + p0.z * sT[2] + sT[3];
-                const float py = p0.x * sT[4] + p0.y * sT[5] + p0.z * sT[6] + sT[7];
-                const float pz = p0.x * sT[8] + p0.y * sT[9] + p0.z * sT[10] + sT[11];
+                float p[3];
+                transform_query(sT, queries[q], p);
                 float second;
-                const int pos = warp_nearest(ix, g, px, py, pz, match[q], lane, &cand_nn, &second);
+                const int pos = warp_nearest(ix, g, p[0], p[1], p[2], match[q], lane, &cand_nn, &second);
                 if (lane == 0) {
                     match[q] = pos;
-                    nn_state[q] = make_float4(px, py, pz, second);
+                    nn_state[q] = make_float4(p[0], p[1], p[2], second);
                 }
                 if (pos < 0) continue;
                 const uint32_t state = __shfl_sync(FULL, __ldcg(reinterpret_cast<const uint32_t*>(&ix.normals[pos].w)), 0);
                 if (state == valid) continue;
-                const float4 c = __ldg(ix.sorted + pos);
-                int ni;
-                const int found = warp_knn(ix, g, c.x, c.y, c.z, k_normals + 1, lane, ni, &cand_knn, s_stage[warp]);
                 float cov[6];
-                warp_second_moments(ix, c, k_normals, found, ni, lane, cov);
-                if (lane == 0) {
-                    float nn[3];
-                    smallest_eigenvector(cov, nn);
-                    __stcg(ix.normals + pos, make_float4(nn[0], nn[1], nn[2], __uint_as_float(valid)));
-                }
+                warp_normal_moments(ix, g, __ldg(ix.sorted + pos), k_normals, lane, &cand_knn, s_stage[warp], cov);
+                if (lane == 0) store_normal(ix, pos, cov, valid);
                 ++normals_here;
             }
         }
@@ -644,29 +645,11 @@ kd_icp_refine_kernel(KdIndex ix, const float4* __restrict__ queries, const uint3
         if (qi >= nq) break;
         const int pos = match[qi];
         if (pos < 0) continue;
-        const float4 p0 = queries[qi];
         float p[3];
-        p[0] = p0.x * sT[0] + p0.y * sT[1] + p0.z * sT[2] + sT[3];
-        p[1] = p0.x * sT[4] + p0.y * sT[5] + p0.z * sT[6] + sT[7];
-        p[2] = p0.x * sT[8] + p0.y * sT[9] + p0.z * sT[10] + sT[11];
-        const float4 qq = __ldg(ix.sorted + pos);
-        const float4 nv = __ldcg(ix.normals + pos);
-        float q[3] = {qq.x, qq.y, qq.z};
-        float nn[3] = {nv.x, nv.y, nv.z};
-        float J[6];
-        const float r = p2plane_residual_jacobian_identity(p, q, nn, J);
-        KD_SPLIT_MAX(0, r);
-        const float w = ls_weight<float>(scheme, sigma, r, p, q);
-        accumulate_normal_equations<float>(acc, J, w, r * w, r);
+        transform_query(sT, queries[qi], p);
+        accumulate_match(acc, ix, p, pos, scheme, sigma KD_SPLIT_PASS);
     }
-    KD_SPLIT_MAX(1, acc[0] + acc[29]);
-    // The shuffle tree must start on a converged warp.  The grid's last block holds a warp whose lanes left the query
-    // loop at different iterations; without this it took the divergent-warp path of the 30 x 5 shuffles, 35 us on H100
-    // (profiles/h100_kd_residual_split_before.log) while every other block took 1.2 us -- and the solve waits for it.
-    __syncwarp();
-    block_reduce_store<KD_REFINE_THREADS, KD_WARPS>(acc, partials + (size_t)blockIdx.x * NACC);
-    KD_SPLIT_BLOCK_MAX()
-    if (fuse_threshold >= 0.f) icp_finish_in_last_block<KD_REFINE_THREADS>(fr, partials, fuse_threshold PLS_SPLIT_PASS);
+    block_partial_and_finish<KD_REFINE_THREADS>(acc, fr, partials, fuse_threshold KD_SPLIT_PASS);
 }
 
 // Fine-grained API: [n,3] rows -> float4 queries (no row is dropped: outputs stay aligned with the inputs)
@@ -834,22 +817,13 @@ void pack_valid_rows_f64(pls_context* ctx, const double* pts_dev, int64_t n, flo
     pack_valid_rows_impl<double>(ctx, pts_dev, n, out, count_dev);
 }
 
-namespace {
-__global__ void nonnull_pixels_kernel(const float* __restrict__ vmap, int64_t hw, uint8_t* __restrict__ flags) {
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < hw; i += (int64_t)gridDim.x * blockDim.x) {
-        float x = vmap[i], y = vmap[hw + i], z = vmap[2 * hw + i];
-        // points[points.norm(dim=-1) > 0]  (icp_odometry.py:303-305)
-        flags[i] = (sqrtf(x * x + y * y + z * z) > 0.0f) ? 1 : 0;
-    }
-}
-}  // namespace
-
-void pack_nonnull_pixels(pls_context* ctx, const float* vmap_dev, int64_t hw, float4* out, uint32_t* count_dev) {
+void pack_valid_pixels(pls_context* ctx, const float* vmap_dev, int64_t hw, float min_norm, float4* out,
+                       uint32_t* count_dev) {
     cudaStream_t st = ctx->stream;
     ctx->tmp[1].reserve((size_t)hw, st);
     ctx->tmp[2].reserve((size_t)hw * sizeof(uint32_t), st);
     const int g = grid_for(hw, 256, 8 * kNumSMs);
-    nonnull_pixels_kernel<<<g, 256, 0, st>>>(vmap_dev, hw, ctx->tmp[1].as<uint8_t>());
+    kd_valid_pixels_kernel<<<g, 256, 0, st>>>(vmap_dev, hw, min_norm, ctx->tmp[1].as<uint8_t>());
     PLS_CHECK_LAUNCH();
     exclusive_scan_flags(ctx, ctx->tmp[1].as<uint8_t>(), hw, ctx->tmp[2].as<uint32_t>(), count_dev);
     kd_pack_pixels_kernel<<<g, 256, 0, st>>>(vmap_dev, hw, ctx->tmp[1].as<uint8_t>(), ctx->tmp[2].as<uint32_t>(), out);
@@ -919,15 +893,7 @@ void kdmap_update(pls_context* ctx, const float* rel_pose_host, const float* pts
         if (pts_dev) {
             pack_valid_rows(ctx, pts_dev, cap_new, ctx->tmp[4].as<float4>(), cnt);
         } else {
-            ctx->tmp[1].reserve((size_t)cap_new, st);
-            ctx->tmp[2].reserve((size_t)cap_new * sizeof(uint32_t), st);
-            const int g = grid_for(cap_new, 256, 8 * kNumSMs);
-            kd_valid_pixels_kernel<<<g, 256, 0, st>>>(vmap_dev, cap_new, ctx->tmp[1].as<uint8_t>());
-            PLS_CHECK_LAUNCH();
-            exclusive_scan_flags(ctx, ctx->tmp[1].as<uint8_t>(), cap_new, ctx->tmp[2].as<uint32_t>(), cnt);
-            kd_pack_pixels_kernel<<<g, 256, 0, st>>>(vmap_dev, cap_new, ctx->tmp[1].as<uint8_t>(),
-                                                      ctx->tmp[2].as<uint32_t>(), ctx->tmp[4].as<float4>());
-            PLS_CHECK_LAUNCH();
+            pack_valid_pixels(ctx, vmap_dev, cap_new, 0.01f, ctx->tmp[4].as<float4>(), cnt);  // local_map.py:320-328
         }
         if (known_count >= 0) {
             num_new = known_count;
@@ -954,6 +920,17 @@ static int resident_blocks(const void* kernel) {
 
 static unsigned long long* kd_counters(pls_context* ctx) {
     return reinterpret_cast<unsigned long long*>(scalar_u32(ctx, SC_KD_COUNTERS));
+}
+
+// What the last search was, for pls_kdmap_last_correspondences.  n: the query count of a fine-grained search (that of an
+// ICP iteration is in the FrameResult).
+static void record_search(KdMap& kd, bool icp, bool sharded, bool normals, int64_t n) {
+    kd.searched = true;
+    kd.searched_icp = icp;
+    kd.searched_sharded = sharded;
+    kd.searched_normals = normals;
+    kd.searched_gen = kd.gen;
+    kd.searched_n = n;
 }
 
 // The search of one ICP iteration (or of one fine-grained API call).  first: every query is searched; later iterations
@@ -1012,21 +989,16 @@ int kdmap_icp_iteration(pls_context* ctx, int64_t query_bound, int rank, int num
     // credited per executed iteration by the caller (the launch is a no-op once ICP converged)
     ProfileScope ps(ctx, 0, 0.0, false);
     const KdIndex ix = make_index(ctx);
-    const int blocks = grid_for(mine, KD_RES_THREADS, 8 * kNumSMs);
+    const int blocks = grid_for(mine, KD_THREADS, 8 * kNumSMs);
     ctx->partials.reserve((size_t)blocks * NACC * sizeof(double), st);
-    KdMap& kd = ctx->kd;
-    kd.searched = true;
-    kd.searched_icp = true;
-    kd.searched_sharded = num_ranks > 1;
-    kd.searched_normals = true;
-    kd.searched_gen = kd.gen;
+    record_search(ctx->kd, true, num_ranks > 1, true, 0);
     if (it == 0 || ctx->kd.indexed >= KD_COLD_MAP_POINTS) {
         launch_search(ctx, ix, ctx->query_ptr, nq_dev, mine, rank, num_ranks, fr->T, &fr->done, ctx->nn_prev.as<int>(), it == 0,
                       true, it & 1);
         ProfileScope p10(ctx, 10, 0.0);
-        kd_residual_kernel<<<blocks, KD_RES_THREADS, 0, st>>>(ix, ctx->query_ptr, nq_dev, (int64_t)rank, (int64_t)num_ranks, fr,
-                                                              ctx->cfg.scheme, ctx->cfg.sigma, ctx->nn_prev.as<int>(),
-                                                              ctx->partials.as<double>(), fuse_threshold);
+        kd_residual_kernel<<<blocks, KD_THREADS, 0, st>>>(ix, ctx->query_ptr, nq_dev, (int64_t)rank, (int64_t)num_ranks, fr,
+                                                          ctx->cfg.scheme, ctx->cfg.sigma, ctx->nn_prev.as<int>(),
+                                                          ctx->partials.as<double>(), fuse_threshold);
         PLS_CHECK_LAUNCH();
     } else {
         ProfileScope p11(ctx, 11, 0.0);
@@ -1134,13 +1106,7 @@ int pls_kdmap_nn_search(pls_context* ctx, const float* queries, int64_t n, float
     const KdIndex ix = make_index(ctx);
     launch_search(ctx, ix, ctx->queries.as<float4>(), nq, n, 0, 1, ctx->tmp[6].as<float>(), nullptr, ctx->nn_prev.as<int>(), true,
                   out_normals != nullptr, 0);
-    KdMap& kd = ctx->kd;
-    kd.searched = true;
-    kd.searched_icp = false;
-    kd.searched_sharded = false;
-    kd.searched_normals = out_normals != nullptr;
-    kd.searched_gen = kd.gen;
-    kd.searched_n = n;
+    record_search(ctx->kd, false, false, out_normals != nullptr, n);
     kd_search_export_kernel<<<grid_for(n, 256, 8 * kNumSMs), 256, 0, st>>>(ix, ctx->nn_prev.as<int>(), n, (float*)onb.dev,
                                                                             (float*)onr.dev, (long long*)oix.dev);
     PLS_CHECK_LAUNCH();

@@ -459,7 +459,8 @@ void process_frame_device(pls_context* ctx, const void* data_void, int layout, i
         scrub_vertex_map_kernel<<<grid_for(hw), 256, 0, st>>>(data_dev, hw, frame_vmap.as<float>());
         PLS_CHECK_LAUNCH();
         ctx->tmp[5].reserve((size_t)hw * sizeof(float4), st);
-        pack_nonnull_pixels(ctx, frame_vmap.as<float>(), hw, ctx->tmp[5].as<float4>(), count_slot(ctx, 1));
+        // points[points.norm(dim=-1) > 0]  (icp_odometry.py:303-305)
+        pack_valid_pixels(ctx, frame_vmap.as<float>(), hw, 0.f, ctx->tmp[5].as<float4>(), count_slot(ctx, 1));
         frame_pts.reserve(sizeof(float4) * 4, st);
         first_point_kernel<<<1, 32, 0, st>>>(ctx->tmp[5].as<float4>(), count_slot(ctx, 1), frame_pts.as<float4>(),
                                               count_slot(ctx, 2), fr);
@@ -549,7 +550,7 @@ void process_frame_device(pls_context* ctx, const void* data_void, int layout, i
         query_bound = n < hw ? n : hw;
     } else {
         ctx->queries.reserve((size_t)hw * sizeof(float4), st);
-        pack_nonnull_pixels(ctx, frame_vmap.as<float>(), hw, ctx->queries.as<float4>(), count_slot(ctx, 1));
+        pack_valid_pixels(ctx, frame_vmap.as<float>(), hw, 0.f, ctx->queries.as<float4>(), count_slot(ctx, 1));
         ctx->query_ptr = ctx->queries.as<float4>();
         query_bound = n < hw ? n : hw;
     }
