@@ -251,6 +251,24 @@ PLS_API int pls_process_frame_grid_sample(pls_context* ctx, const float* raw_poi
                                   int layout, const float* init_pose, float* out_pose,
                                   float* out_params, int* out_has_pose, double* out_info);
 
+/* Several independent sequences, one frame each, in one call (no reference counterpart: the reference's runner
+ * processes sequences one after another, odometry_runner.py:145-175).  ctxs [num] distinct kd-map contexts on one
+ * device; data / layouts / n / init_poses [num] as pls_process_frame (data[i] == NULL: sequence i skipped);
+ * voxel > 0 grid-samples every sequence first, as pls_process_frame_grid_sample; outputs [num,16] / [num,6] / [num] /
+ * [num,12] / [num], each nullable.  num <= PLS_MAX_SEQUENCES.
+ * Every context ends in the state its own pls_process_frame (pls_process_frame_grid_sample) call would have left, with
+ * the same outputs, bit for bit; a sequence may be on its first frame.  Each kernel of an ICP iteration is one launch for
+ * every sequence.  Contexts must have gn_max_iters == 1 and no communicator; otherwise PLS_E_INVALID before any work.
+ * Errors are per sequence: out_status[i] (PLS_E_SINGULAR, or an input pls_process_frame refuses, leaves sequence i as
+ * pls_process_frame leaves it after that error, the others complete), pls_last_error(ctxs[i]) its text; the call
+ * returns the first non-OK status in sequence order.  A failure of no one sequence (a CUDA error) ends the call: every
+ * sequence whose frame had not completed reports it, those that completed keep PLS_OK.  The profiling slots
+ * (pls_profile_*) are not credited by this call; PLS_BATCH_TRACE=<file> appends its per-phase times to <file>. */
+enum { PLS_MAX_SEQUENCES = 64 };
+PLS_API int pls_process_frames(pls_context* const* ctxs, int num, const void* const* data, const int* layouts,
+                               const int64_t* n, double voxel, const float* const* init_poses, float* out_poses,
+                               float* out_params, int* out_has_pose, double* out_info, int* out_status);
+
 /* ---- the rows either side of the path (SURVEY.md section 8f, ranks 1-2) -----------------------------------
  * Distortion.filter (slam/preprocessing.py:148-191): de-skew of a frame with the estimated relative motion.
  * xyz [n,3] float32|float64; timestamps [n] float32|float64 (alpha is formed in their dtype, like numpy does);

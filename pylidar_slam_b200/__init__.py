@@ -9,7 +9,7 @@ from .common import (Pose, SphericalProjector, compute_neighbors, compute_normal
                      grid_sample, voxel_hashing, voxel_normal_distribution, voxel_statistics, voxelise,
                      weighted_procrustes)
 from .odometry import (LOCAL_MAP, ODOMETRY, RIGID_ALIGNMENT, GaussNewtonPointToPlaneAlignment,  # noqa: F401
-                       GaussNewtonPointToPlaneConfig, GaussNewtonPointToPointAlignment, GNPointToPointConfig, ICPFrameToModel, ICPFrameToModelConfig, KdTreeLocalMap,
+                       GaussNewtonPointToPlaneConfig, GaussNewtonPointToPointAlignment, GNPointToPointConfig, ICPFrameToModel, ICPFrameToModelBatch, ICPFrameToModelConfig, KdTreeLocalMap,
                        KdTreeLocalMapConfig, LocalMap, OdometryAlgorithm, ProjectiveLocalMap,
                        ProjectiveLocalMapConfig)
 from .preprocessing import (FILTER, Distortion, DistortionConfig, GridSample, GridSampleConfig, Preprocessing,  # noqa: F401

@@ -18,6 +18,7 @@ SCHEMES = {"default": 0, "least_square": 1, "huber": 2, "exp": 3, "neighborhood"
 MAP_KDTREE, MAP_PROJECTIVE = 0, 1
 INPUT_NDARRAY, INPUT_TENSOR, INPUT_VERTEX_MAP, INPUT_NDARRAY_F64, INPUT_TENSOR_F64 = 0, 1, 2, 3, 4
 PTR_DEVICE, PTR_HOST = 0x100, 0x200  # residency hints OR-ed into a layout
+MAX_SEQUENCES = 64  # PLS_MAX_SEQUENCES: contexts one pls_process_frames call advances
 
 
 class PlsConfig(C.Structure):
@@ -76,6 +77,7 @@ _SIGNATURES = {
     "pls_register_frame": [_P, _P, _L, _P, _P, _P, _P, C.POINTER(_I)],
     "pls_process_frame": [_P, _P, _I, _L, _P, _P, _P, C.POINTER(_I), _P],
     "pls_process_frame_grid_sample": [_P, _P, _L, _D, _I, _P, _P, _P, C.POINTER(_I), _P],
+    "pls_process_frames": [_P, _I, _P, _P, _P, _D, _P, _P, _P, _P, _P, _P],
     "pls_comm_init": [_P, _I, _I, _P, C.c_char_p],
     "pls_comm_unique_id": [C.c_char_p, _P],
     "pls_comm_p2p_handle": [_P, _I, _P],
@@ -270,6 +272,15 @@ class Context:
         if _cuda_inputs:
             self._order_after_torch()
         return check(self.handle, getattr(self.lib, name)(self.handle, *args))
+
+    def check(self, status):
+        """Maps a status this context's last call returned onto the reference's error behaviour (see check())."""
+        return check(self.handle, status)
+
+    def process_frames(self, *args):
+        """pls_process_frames(*args); its first argument is the array of context handles, this context's among them.
+        Returns the status code unchecked: errors are per sequence."""
+        return self.lib.pls_process_frames(*args)
 
     def _order_after_torch(self):
         """CUDA tensors were addressed for this call: whatever PyTorch still has in flight on its current stream

@@ -327,12 +327,13 @@ int pls_destroy(pls_context* ctx) {
     for (auto& b : ctx->frame_vmap_buf) b.release();
     for (auto& b : ctx->frame_pts_buf) b.release();
     ctx->queries.release(); ctx->nn_prev.release();
-    ctx->partials.release(); ctx->gs_keys.release(); ctx->gs_vals.release(); ctx->gs_out_xyz.release();
+    ctx->partials.release(); ctx->batch_buf.release(); ctx->gs_keys.release(); ctx->gs_vals.release(); ctx->gs_out_xyz.release();
     ctx->gs_out_idx.release();
     for (auto& s : ctx->prof)
         for (auto e : s.pool) cudaEventDestroy(e);
     if (ctx->ev_map_done) cudaEventDestroy(ctx->ev_map_done);
     if (ctx->ev_inputs) cudaEventDestroy(ctx->ev_inputs);
+    if (ctx->ev_batch) cudaEventDestroy(ctx->ev_batch);
     ctx->gs_host_xyz.release(); ctx->gs_host_idx.release();
     if (ctx->stream_map) cudaStreamDestroy(ctx->stream_map);
     if (ctx->own_stream) cudaStreamDestroy(ctx->stream_main);

@@ -271,15 +271,24 @@ template void grid_sample_device<float>(pls_context*, const float*, int64_t, dou
 template void grid_sample_device<double>(pls_context*, const double*, int64_t, double, double*, long long*, bool, double*,
                                          long long*);
 
-uint32_t grid_sample_read_count(pls_context* ctx, bool* overflowed) {
+void grid_sample_count_to_host(pls_context* ctx) {
     // into the pinned block behind the host FrameResult: a pageable destination would make the copy synchronous
     // through the driver's own staging buffer
     uint32_t* words = reinterpret_cast<uint32_t*>(reinterpret_cast<char*>(ctx->pinned.p) + kScalarOffset);
     static_assert(SC_GS_COUNT == 0 && SC_GS_OVERFLOW == 7, "one 32-byte copy covers the count and the overflow stamp");
     PLS_CUDA(cudaMemcpyAsync(words, scalar_u32(ctx, SC_GS_COUNT), 8 * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
-    PLS_CUDA(cudaStreamSynchronize(ctx->stream));
+}
+
+uint32_t grid_sample_host_count(pls_context* ctx, bool* overflowed) {
+    const uint32_t* words = reinterpret_cast<const uint32_t*>(reinterpret_cast<const char*>(ctx->pinned.p) + kScalarOffset);
     *overflowed = ctx->gs_seq != 0 && words[SC_GS_OVERFLOW] == ctx->gs_seq;
     return words[SC_GS_COUNT];
+}
+
+uint32_t grid_sample_read_count(pls_context* ctx, bool* overflowed) {
+    grid_sample_count_to_host(ctx);
+    PLS_CUDA(cudaStreamSynchronize(ctx->stream));
+    return grid_sample_host_count(ctx, overflowed);
 }
 
 }  // namespace pls

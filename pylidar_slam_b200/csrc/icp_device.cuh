@@ -120,10 +120,10 @@ __device__ __forceinline__ void icp_solve_and_update(FrameResult* fr, const doub
 }
 
 // Called by every block of a correspondence kernel (512, 256 or 128 threads) after it stored its partial row: the block
-// that arrives last (ticket in fr->pad) sums all rows in the fixed order and runs the solve -- one launch
-// and one dependent-launch gap less per ICP iteration than a separate step kernel.
+// that arrives last of the num_blocks (ticket in fr->pad) sums all rows in the fixed order and runs the solve -- one
+// launch and one dependent-launch gap less per ICP iteration than a separate step kernel.
 template <int THREADS = 256>
-__device__ __forceinline__ void icp_finish_in_last_block(FrameResult* fr, const double* __restrict__ partials,
+__device__ __forceinline__ void icp_finish_in_last_block(FrameResult* fr, const double* __restrict__ partials, int num_blocks,
                                                          float threshold_delta PLS_SPLIT_ARG) {
     __shared__ int s_last;
     __shared__ double s_sums[NACC];
@@ -132,13 +132,13 @@ __device__ __forceinline__ void icp_finish_in_last_block(FrameResult* fr, const 
     __syncthreads();
     if (threadIdx.x == 0) {
         const int ticket = atomicAdd(&fr->pad, 1);
-        s_last = ticket == (int)gridDim.x - 1;
+        s_last = ticket == num_blocks - 1;
         PLS_SPLIT(5, (double)ticket);
     }
     __syncthreads();
     if (!s_last) return;
     __threadfence();
-    sum_partials_256<THREADS>(partials, (int)gridDim.x, s_sums);
+    sum_partials_256<THREADS>(partials, num_blocks, s_sums);
     __syncthreads();
     if (threadIdx.x < NACC) fr->last_sums[threadIdx.x] = s_sums[threadIdx.x];
     if (threadIdx.x != 0) return;

@@ -213,6 +213,8 @@ struct pls_context {
     pls::DBuf kd_worklist;              // map points whose normal the current iteration has to compute; queued queries
     pls::DBuf kd_nn_state;              // per query: position at its last full search + runner-up bound (float4)
     pls::DBuf partials;                 // [blocks][NACC] doubles
+    pls::DBuf batch_buf;                // pls_process_frames led by this context: sequence descriptors, then done flags
+    cudaEvent_t ev_batch = nullptr;     // pls_process_frames: this context's input stage, before the batched ICP
     pls::DBuf gs_keys, gs_vals, gs_out_xyz, gs_out_idx;
     uint32_t gs_seq = 0;                // stamp of the last compact-key grid sample (overflow detection)
     pls::HBuf gs_host_xyz, gs_host_idx; // pinned + mapped staging the grid sample's gather writes directly (host callers)
@@ -372,6 +374,14 @@ void kdmap_update(pls_context* ctx, const float* rel_pose_host, const float* pts
 // insertion of already packed float4 points (nullable) whose count the host knows
 void kdmap_update_packed(pls_context* ctx, const float* rel_pose_host, const float4* fresh_dev, int64_t num_new,
                          bool has_new);
+// pls_process_frames: the ICP of `num` sequences (distinct kd-map contexts, no communicator) in batched launches on st.
+// begin uploads their descriptors into lead->batch_buf and returns the launch widths in grid[3]; iterations enqueues
+// ICP iterations [first, last) of all of them; done reads every sequence's done flag with one copy and one sync.
+void kdmap_batch_begin(pls_context* lead, pls_context* const* ctxs, const int64_t* query_bounds, int num, cudaStream_t st,
+                       int* grid);
+void kdmap_batch_iterations(pls_context* lead, pls_context* const* ctxs, const int64_t* query_bounds, int num, cudaStream_t st,
+                            const int* grid, int first, int last);
+void kdmap_batch_done(pls_context* lead, int num, cudaStream_t st, int* out);
 // ICP iteration `it` of the frame over ctx->query_ptr; returns the number of partial rows written
 // it == 0: no previous matches; fuse_threshold >= 0: finish the iteration (sum + solve + pose update) in the last
 // block of the reduction kernel (*solved tells).
@@ -394,6 +404,10 @@ void grid_sample_device(pls_context* ctx, const T* xyz_dev, int64_t n, double vo
 // Reads SC_GS_COUNT (and the overflow stamp) back: one 32-byte copy + one stream sync.  Returns the sample count;
 // *overflowed tells whether the last compact grid sample has to be repeated with full keys.
 uint32_t grid_sample_read_count(pls_context* ctx, bool* overflowed);
+// The same in two halves, for callers that synchronise once for several contexts: the copy (enqueued on ctx->stream),
+// then, after the stream has been synchronised, the count and overflow test.
+void grid_sample_count_to_host(pls_context* ctx);
+uint32_t grid_sample_host_count(pls_context* ctx, bool* overflowed);
 // projmap.cu
 void projmap_reset(pls_context* ctx);
 // odometry.cu: would an ICP iteration over `work` items be split across the ranks (the rule of enqueue_icp_iterations)?

@@ -13,6 +13,8 @@
 // listed below, under "one ICP iteration on the kd map".
 #include <stdlib.h>
 
+#include <vector>
+
 #include "gn_device.cuh"
 #include "internal.cuh"
 #include "icp_device.cuh"
@@ -354,19 +356,19 @@ __device__ __forceinline__ void accumulate_match(double* acc, const KdIndex& ix,
 }
 
 // The end of a residual phase, called by every thread of a THREADS-thread block whose first KD_WARPS warps hold
-// accumulators: the block partial row, then (fuse_threshold >= 0) the fixed-order sum and the solve in the grid's last
-// block.
+// accumulators: the block partial row `block`, then (fuse_threshold >= 0) the fixed-order sum of the `grid` rows and the
+// solve in the last block to arrive.
 template <int THREADS>
 __device__ __forceinline__ void block_partial_and_finish(double* acc, FrameResult* fr, double* __restrict__ partials,
-                                                         float fuse_threshold KD_SPLIT_ARG) {
+                                                         float fuse_threshold, unsigned block, unsigned grid KD_SPLIT_ARG) {
     KD_SPLIT_MAX(1, acc[0] + acc[29]);
     // The shuffle tree must start on a converged warp.  The grid's last block holds a warp whose lanes left the query
     // loop at different iterations; without this it took the divergent-warp path of the 30 x 5 shuffles, 35 us on H100
     // (profiles/h100_kd_residual_split_before.log) while every other block took 1.2 us -- and the solve waits for it.
     __syncwarp();
-    block_reduce_store<THREADS, KD_WARPS>(acc, partials + (size_t)blockIdx.x * NACC);
+    block_reduce_store<THREADS, KD_WARPS>(acc, partials + (size_t)block * NACC);
     KD_SPLIT_BLOCK_MAX()
-    if (fuse_threshold >= 0.f) icp_finish_in_last_block<THREADS>(fr, partials, fuse_threshold PLS_SPLIT_PASS);
+    if (fuse_threshold >= 0.f) icp_finish_in_last_block<THREADS>(fr, partials, (int)grid, fuse_threshold PLS_SPLIT_PASS);
 }
 
 // Iterations after a frame's first on maps of KD_COLD_MAP_POINTS or more: a thread per query keeps its previous match
@@ -397,15 +399,23 @@ kd_nn_verify_kernel(KdIndex ix, const float4* __restrict__ queries, const uint32
     block_flush_list(s_hard, s_nh, hard, lists + KDL_HARD_NN + parity, &s_base);
 }
 
+// Each kernel of an ICP iteration below is one __device__ body, called by two entry points: the kernel of one sequence,
+// which passes blockIdx.x / gridDim.x and its arguments, and the *_batch_kernel of pls_process_frames, whose
+// blockIdx.y picks a sequence's descriptor and which passes that sequence's own block count.  A body reads no
+// blockIdx.x or gridDim.x itself, so a sequence's striding, block partials and solve ticket are those of its single path.
+
 // 1-NN, full search: a warp per query over the cell pyramid (warp_nearest).  hard == nullptr: every query of this
 // rank's shard (a frame's first iteration); else the queued ones, seeded with their previous match.  The first warp to
 // match a map point whose normal is not cached claims it (CAS on the state word) and queues it; claims are made by all
 // lanes at once after 32 queries.  Each query's position and runner-up bound are kept for the later iterations' checks.
-__global__ void __launch_bounds__(KD_THREADS)
-kd_nn_warp_kernel(KdIndex ix, const float4* __restrict__ queries, const uint32_t* __restrict__ nq_dev, int64_t q_begin,
-                  int64_t q_stride, const int* __restrict__ hard, uint32_t* lists, int parity, const float* __restrict__ T,
-                  const int* __restrict__ done, int* __restrict__ match, float4* __restrict__ nn_state, int want_normals,
-                  int* __restrict__ pending, unsigned long long* __restrict__ counters) {
+// Which warp searches which query does not change its result, so any block count gives the same bits.
+__device__ __forceinline__ void kd_nn_warp_body(const KdIndex& ix, const float4* __restrict__ queries,
+                                                const uint32_t* __restrict__ nq_dev, int64_t q_begin, int64_t q_stride,
+                                                const int* __restrict__ hard, uint32_t* lists, int parity,
+                                                const float* __restrict__ T, const int* __restrict__ done,
+                                                int* __restrict__ match, float4* __restrict__ nn_state, int want_normals,
+                                                int* __restrict__ pending, unsigned long long* __restrict__ counters,
+                                                unsigned block, unsigned grid) {
     if (done && *done) return;
     int n;
     if (hard) {
@@ -413,12 +423,12 @@ kd_nn_warp_kernel(KdIndex ix, const float4* __restrict__ queries, const uint32_t
     } else {
         const int64_t nq = (int64_t)*nq_dev;
         n = nq > q_begin ? (int)((nq - q_begin + q_stride - 1) / q_stride) : 0;
-        if (blockIdx.x == 0 && threadIdx.x == 0)  // first kernel of the iteration: recycle the other parity's lists
+        if (block == 0 && threadIdx.x == 0)  // first kernel of the iteration: recycle the other parity's lists
             for (int l = 0; l < KDL_WORDS; l += 2) lists[l + (parity ^ 1)] = 0;
     }
     const int lane = threadIdx.x & 31;
-    const int warp_global = blockIdx.x * KD_WARPS + (threadIdx.x >> 5);
-    const int total_warps = gridDim.x * KD_WARPS;
+    const int warp_global = block * KD_WARPS + (threadIdx.x >> 5);
+    const int total_warps = grid * KD_WARPS;
     if (warp_global >= n) return;
     float t[12];
 #pragma unroll
@@ -473,17 +483,26 @@ kd_nn_warp_kernel(KdIndex ix, const float4* __restrict__ queries, const uint32_t
     if (counters && lane == 0 && cand) atomicAdd(counters + KDC_NN_CAND, (unsigned long long)cand);
 }
 
+__global__ void __launch_bounds__(KD_THREADS)
+kd_nn_warp_kernel(KdIndex ix, const float4* __restrict__ queries, const uint32_t* __restrict__ nq_dev, int64_t q_begin,
+                  int64_t q_stride, const int* __restrict__ hard, uint32_t* lists, int parity, const float* __restrict__ T,
+                  const int* __restrict__ done, int* __restrict__ match, float4* __restrict__ nn_state, int want_normals,
+                  int* __restrict__ pending, unsigned long long* __restrict__ counters) {
+    kd_nn_warp_body(ix, queries, nq_dev, q_begin, q_stride, hard, lists, parity, T, done, match, nn_state, want_normals,
+                    pending, counters, blockIdx.x, gridDim.x);
+}
+
 // Normals: a warp per queued map point, exact (k+1)-NN over the cell pyramid (warp_knn), second moments; the
 // eigen-solves are deferred and run lane-parallel (each lane one point) so that no warp idles behind a serial solve.
-__global__ void __launch_bounds__(KD_THREADS)
-kd_normals_warp_kernel(KdIndex ix, int k_normals, const int* __restrict__ worklist, const uint32_t* __restrict__ wl_count,
-                       const int* __restrict__ done, unsigned long long* __restrict__ counters) {
+__device__ __forceinline__ void kd_normals_warp_body(const KdIndex& ix, int k_normals, const int* __restrict__ worklist,
+                                                     const uint32_t* __restrict__ wl_count, const int* __restrict__ done,
+                                                     unsigned long long* __restrict__ counters, unsigned block, unsigned grid) {
     if (done && *done) return;
     __shared__ unsigned long long s_stage[KD_WARPS][KNN_STAGE];
     const int n = (int)*wl_count;
     const int lane = threadIdx.x & 31;
-    const int warp_global = blockIdx.x * KD_WARPS + (threadIdx.x >> 5);
-    const int total_warps = gridDim.x * KD_WARPS;
+    const int warp_global = block * KD_WARPS + (threadIdx.x >> 5);
+    const int total_warps = grid * KD_WARPS;
     if (warp_global >= n) return;
     unsigned long long* stage = s_stage[threadIdx.x >> 5];
     const KdGridLocal g = kd_load_grid(ix);
@@ -530,13 +549,19 @@ kd_normals_warp_kernel(KdIndex ix, int k_normals, const int* __restrict__ workli
 #endif
 }
 
+__global__ void __launch_bounds__(KD_THREADS)
+kd_normals_warp_kernel(KdIndex ix, int k_normals, const int* __restrict__ worklist, const uint32_t* __restrict__ wl_count,
+                       const int* __restrict__ done, unsigned long long* __restrict__ counters) {
+    kd_normals_warp_body(ix, k_normals, worklist, wl_count, done, counters, blockIdx.x, gridDim.x);
+}
+
 // A thread per query: accumulate_match -> block partials; the last block sums them in fixed order and runs the solve,
 // stop test and pose update.
-__global__ void __launch_bounds__(KD_THREADS)
-kd_residual_kernel(KdIndex ix, const float4* __restrict__ queries, const uint32_t* __restrict__ nq_dev, int64_t q_begin,
-                   int64_t q_stride, FrameResult* fr, int scheme, float sigma,
-                   const int* __restrict__ match, double* __restrict__ partials, float fuse_threshold) {
-    KD_SPLIT_BEGIN()
+__device__ __forceinline__ void kd_residual_body(const KdIndex& ix, const float4* __restrict__ queries,
+                                                 const uint32_t* __restrict__ nq_dev, int64_t q_begin, int64_t q_stride,
+                                                 FrameResult* fr, int scheme, float sigma, const int* __restrict__ match,
+                                                 double* __restrict__ partials, float fuse_threshold, unsigned block,
+                                                 unsigned grid KD_SPLIT_ARG) {
     if (fr->done) return;
     __shared__ float sT[12];
     if (threadIdx.x < 12) sT[threadIdx.x] = fr->T[threadIdx.x];
@@ -546,7 +571,7 @@ kd_residual_kernel(KdIndex ix, const float4* __restrict__ queries, const uint32_
     double acc[NACC];
 #pragma unroll
     for (int a = 0; a < NACC; ++a) acc[a] = 0.0;
-    for (int64_t s = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;; s += (int64_t)gridDim.x * blockDim.x) {
+    for (int64_t s = (int64_t)block * blockDim.x + threadIdx.x;; s += (int64_t)grid * blockDim.x) {
         const int64_t qi = q_begin + s * q_stride;
         if (qi >= nq) break;
         float p[3];
@@ -555,7 +580,16 @@ kd_residual_kernel(KdIndex ix, const float4* __restrict__ queries, const uint32_
         if (pos < 0) continue;
         accumulate_match(acc, ix, p, pos, scheme, sigma KD_SPLIT_PASS);
     }
-    block_partial_and_finish<KD_THREADS>(acc, fr, partials, fuse_threshold KD_SPLIT_PASS);
+    block_partial_and_finish<KD_THREADS>(acc, fr, partials, fuse_threshold, block, grid KD_SPLIT_PASS);
+}
+
+__global__ void __launch_bounds__(KD_THREADS)
+kd_residual_kernel(KdIndex ix, const float4* __restrict__ queries, const uint32_t* __restrict__ nq_dev, int64_t q_begin,
+                   int64_t q_stride, FrameResult* fr, int scheme, float sigma,
+                   const int* __restrict__ match, double* __restrict__ partials, float fuse_threshold) {
+    KD_SPLIT_BEGIN()
+    kd_residual_body(ix, queries, nq_dev, q_begin, q_stride, fr, scheme, sigma, match, partials, fuse_threshold, blockIdx.x,
+                     gridDim.x KD_SPLIT_PASS);
 }
 
 // ICP iterations after a frame's first, in ONE launch.  Each block takes the queries kd_residual_kernel would give it
@@ -572,12 +606,13 @@ kd_residual_kernel(KdIndex ix, const float4* __restrict__ queries, const uint32_
 // the slowest block's searches took 35 us, a chain of up to four searches per warp.
 constexpr int KD_REFINE_THREADS = 512;
 constexpr int KD_REFINE_WARPS = KD_REFINE_THREADS / 32;
-__global__ void __launch_bounds__(KD_REFINE_THREADS)
-kd_icp_refine_kernel(KdIndex ix, const float4* __restrict__ queries, const uint32_t* __restrict__ nq_dev, int64_t q_begin,
-                     int64_t q_stride, FrameResult* fr, int scheme, float sigma, int k_normals, int* __restrict__ match,
-                     float4* __restrict__ nn_state, double* __restrict__ partials, float fuse_threshold,
-                     unsigned long long* __restrict__ counters) {
-    KD_SPLIT_BEGIN()
+__device__ __forceinline__ void kd_icp_refine_body(const KdIndex& ix, const float4* __restrict__ queries,
+                                                   const uint32_t* __restrict__ nq_dev, int64_t q_begin, int64_t q_stride,
+                                                   FrameResult* fr, int scheme, float sigma, int k_normals,
+                                                   int* __restrict__ match, float4* __restrict__ nn_state,
+                                                   double* __restrict__ partials, float fuse_threshold,
+                                                   unsigned long long* __restrict__ counters, unsigned block,
+                                                   unsigned grid KD_SPLIT_ARG) {
     if (fr->done) return;
     __shared__ float sT[12];
     __shared__ int s_hard[KD_THREADS];
@@ -589,7 +624,7 @@ kd_icp_refine_kernel(KdIndex ix, const float4* __restrict__ queries, const uint3
     const int64_t nq = (int64_t)*nq_dev;
     const uint32_t valid = kd_normal_valid(ix.gen);
     int cand_nn = 0, cand_knn = 0, normals_here = 0;
-    for (int64_t round = (int64_t)blockIdx.x * KD_THREADS;; round += (int64_t)gridDim.x * KD_THREADS) {
+    for (int64_t round = (int64_t)block * KD_THREADS;; round += (int64_t)grid * KD_THREADS) {
         if (q_begin + round * q_stride >= nq) break;  // block-uniform
         if (threadIdx.x == 0) s_nh = 0;
         __syncthreads();
@@ -640,7 +675,7 @@ kd_icp_refine_kernel(KdIndex ix, const float4* __restrict__ queries, const uint3
     double acc[NACC];
 #pragma unroll
     for (int a = 0; a < NACC; ++a) acc[a] = 0.0;
-    for (int64_t s = (int64_t)blockIdx.x * KD_THREADS + threadIdx.x; owner; s += (int64_t)gridDim.x * KD_THREADS) {
+    for (int64_t s = (int64_t)block * KD_THREADS + threadIdx.x; owner; s += (int64_t)grid * KD_THREADS) {
         const int64_t qi = q_begin + s * q_stride;
         if (qi >= nq) break;
         const int pos = match[qi];
@@ -649,7 +684,101 @@ kd_icp_refine_kernel(KdIndex ix, const float4* __restrict__ queries, const uint3
         transform_query(sT, queries[qi], p);
         accumulate_match(acc, ix, p, pos, scheme, sigma KD_SPLIT_PASS);
     }
-    block_partial_and_finish<KD_REFINE_THREADS>(acc, fr, partials, fuse_threshold KD_SPLIT_PASS);
+    block_partial_and_finish<KD_REFINE_THREADS>(acc, fr, partials, fuse_threshold, block, grid KD_SPLIT_PASS);
+}
+
+__global__ void __launch_bounds__(KD_REFINE_THREADS)
+kd_icp_refine_kernel(KdIndex ix, const float4* __restrict__ queries, const uint32_t* __restrict__ nq_dev, int64_t q_begin,
+                     int64_t q_stride, FrameResult* fr, int scheme, float sigma, int k_normals, int* __restrict__ match,
+                     float4* __restrict__ nn_state, double* __restrict__ partials, float fuse_threshold,
+                     unsigned long long* __restrict__ counters) {
+    KD_SPLIT_BEGIN()
+    kd_icp_refine_body(ix, queries, nq_dev, q_begin, q_stride, fr, scheme, sigma, k_normals, match, nn_state, partials,
+                       fuse_threshold, counters, blockIdx.x, gridDim.x KD_SPLIT_PASS);
+}
+
+// ---- several sequences per launch (pls_process_frames) --------------------------------------------------------------
+// What the kernels of one ICP iteration need of one sequence: the arguments its single path passes (every query is
+// the sequence's own: q_begin 0, stride 1), and its share of each launch.  Built on the host by kdmap_batch_begin and
+// uploaded once per call.
+struct KdSeq {
+    KdIndex ix;
+    const float4* queries;
+    const uint32_t* nq_dev;     // query count (FrameResult counts[1])
+    FrameResult* fr;            // pose, done flag, solve ticket
+    int* match;
+    float4* nn_state;
+    int* pending;               // normals work list
+    uint32_t* lists;            // work-list words (SC_KD_LISTS)
+    double* partials;
+    unsigned long long* counters;
+    int scheme;
+    float sigma;
+    int k_normals;
+    float fuse_threshold;
+    int max_iters;              // max_num_alignments: launches of later iterations leave the sequence alone
+    int blocks;                 // grid_for(query bound): the residual kernel's geometry on the single path
+    int refine_blocks;          // blocks, or 0 on a map of KD_COLD_MAP_POINTS or more (its own four launches)
+    int nn_blocks, kn_blocks;   // its share of the resident wave of the 1-NN / normals kernels
+};
+static_assert(sizeof(KdSeq) % sizeof(int) == 0, "KdSeq is copied in 4-byte words");
+
+// Sequence blockIdx.y's descriptor into shared memory, for every thread of the block.
+__device__ __forceinline__ void load_seq(const KdSeq* __restrict__ seqs, KdSeq& s) {
+    const int* src = reinterpret_cast<const int*>(seqs + blockIdx.y);
+    int* dst = reinterpret_cast<int*>(&s);
+    for (int i = threadIdx.x; i < (int)(sizeof(KdSeq) / sizeof(int)); i += blockDim.x) dst[i] = __ldg(src + i);
+    __syncthreads();
+}
+
+// The batched entry points do not stamp in -DPLS_KD_SPLIT builds.
+#ifdef PLS_KD_SPLIT
+#define KD_SPLIT_NONE()                     \
+    unsigned long long* split = nullptr;    \
+    __shared__ unsigned long long s_split[2];
+#else
+#define KD_SPLIT_NONE()
+#endif
+
+// A frame's first iteration: every query, parity 0.
+__global__ void __launch_bounds__(KD_THREADS) kd_nn_warp_batch_kernel(const KdSeq* __restrict__ seqs) {
+    __shared__ KdSeq s;
+    load_seq(seqs, s);
+    if ((int)blockIdx.x >= s.nn_blocks) return;
+    kd_nn_warp_body(s.ix, s.queries, s.nq_dev, 0, 1, nullptr, s.lists, 0, s.fr->T, &s.fr->done, s.match, s.nn_state, 1,
+                    s.pending, s.counters, blockIdx.x, s.nn_blocks);
+}
+
+__global__ void __launch_bounds__(KD_THREADS) kd_normals_warp_batch_kernel(const KdSeq* __restrict__ seqs) {
+    __shared__ KdSeq s;
+    load_seq(seqs, s);
+    if ((int)blockIdx.x >= s.kn_blocks) return;
+    kd_normals_warp_body(s.ix, s.k_normals, s.pending, s.lists + KDL_PENDING, &s.fr->done, s.counters, blockIdx.x,
+                         s.kn_blocks);
+}
+
+__global__ void __launch_bounds__(KD_THREADS) kd_residual_batch_kernel(const KdSeq* __restrict__ seqs) {
+    __shared__ KdSeq s;
+    load_seq(seqs, s);
+    if ((int)blockIdx.x >= s.blocks) return;
+    KD_SPLIT_NONE()
+    kd_residual_body(s.ix, s.queries, s.nq_dev, 0, 1, s.fr, s.scheme, s.sigma, s.match, s.partials, s.fuse_threshold,
+                     blockIdx.x, s.blocks KD_SPLIT_PASS);
+}
+
+// Iteration `it` (>= 1) of every sequence that has not reached its max_iters and whose map is below KD_COLD_MAP_POINTS.
+__global__ void __launch_bounds__(KD_REFINE_THREADS) kd_icp_refine_batch_kernel(const KdSeq* __restrict__ seqs, int it) {
+    __shared__ KdSeq s;
+    load_seq(seqs, s);
+    if ((int)blockIdx.x >= s.refine_blocks || it >= s.max_iters) return;
+    KD_SPLIT_NONE()
+    kd_icp_refine_body(s.ix, s.queries, s.nq_dev, 0, 1, s.fr, s.scheme, s.sigma, s.k_normals, s.match, s.nn_state,
+                       s.partials, s.fuse_threshold, s.counters, blockIdx.x, s.refine_blocks KD_SPLIT_PASS);
+}
+
+// The done flags of every sequence, for the host's extra-round check.
+__global__ void kd_batch_done_kernel(const KdSeq* __restrict__ seqs, int num, int* __restrict__ out) {
+    for (int i = threadIdx.x; i < num; i += blockDim.x) out[i] = seqs[i].fr->done;
 }
 
 // Fine-grained API: [n,3] rows -> float4 queries (no row is dropped: outputs stay aligned with the inputs)
@@ -1010,6 +1139,102 @@ int kdmap_icp_iteration(pls_context* ctx, int64_t query_bound, int rank, int num
     }
     *solved = fuse_threshold >= 0.f;
     return blocks;
+}
+
+// pls_process_frames: the descriptors of the sequences whose ICP runs in this call, into lead->batch_buf (uploaded on
+// st), and every buffer their iterations use reserved as their single path reserves it.
+// grid[3]: the launch widths, the largest residual / 1-NN / normals block count of a sequence.
+void kdmap_batch_begin(pls_context* lead, pls_context* const* ctxs, const int64_t* query_bounds, int num, cudaStream_t st,
+                       int* grid) {
+    static const int resident_nn = resident_blocks((const void*)kd_nn_warp_batch_kernel);
+    static const int resident_kn = resident_blocks((const void*)kd_normals_warp_batch_kernel);
+    const int share_nn = (resident_nn + num - 1) / num, share_kn = (resident_kn + num - 1) / num;
+    std::vector<KdSeq> seqs((size_t)num);
+    grid[0] = grid[1] = grid[2] = 1;
+    for (int i = 0; i < num; ++i) {
+        pls_context* ctx = ctxs[i];
+        PLS_REQUIRE(ctx->kd.valid, "kd map: search before any update");
+        const int64_t mine = query_bounds[i];
+        const size_t slots = (size_t)mine + 64;
+        const int blocks = grid_for(mine, KD_THREADS, 8 * kNumSMs);
+        ctx->nn_prev.reserve((size_t)mine * sizeof(int), ctx->stream);
+        ctx->partials.reserve((size_t)blocks * NACC * sizeof(double), ctx->stream);
+        ctx->kd_worklist.reserve(2 * slots * sizeof(int), ctx->stream);
+        ctx->kd_nn_state.reserve(slots * sizeof(float4), ctx->stream);
+        ctx->last_sharded = false;
+        record_search(ctx->kd, true, false, true, 0);
+        FrameResult* fr = frame_result_dev(ctx);
+        KdSeq& s = seqs[(size_t)i];
+        s.ix = make_index(ctx);
+        s.queries = ctx->query_ptr;
+        s.nq_dev = reinterpret_cast<const uint32_t*>(&fr->counts[1]);
+        s.fr = fr;
+        s.match = ctx->nn_prev.as<int>();
+        s.nn_state = ctx->kd_nn_state.as<float4>();
+        s.pending = ctx->kd_worklist.as<int>();
+        s.lists = scalar_u32(ctx, SC_KD_LISTS);
+        s.partials = ctx->partials.as<double>();
+        s.counters = kd_counters(ctx);
+        s.scheme = ctx->cfg.scheme;
+        s.sigma = ctx->cfg.sigma;
+        s.k_normals = ctx->cfg.num_neighbors_normals;
+        s.fuse_threshold = ctx->cfg.threshold_delta_pose;
+        s.max_iters = ctx->cfg.max_num_alignments;
+        s.blocks = blocks;
+        s.refine_blocks = ctx->kd.indexed >= KD_COLD_MAP_POINTS ? 0 : blocks;
+        const int wblocks = (int)((mine + KD_WARPS - 1) / KD_WARPS);
+        s.nn_blocks = wblocks < share_nn ? wblocks : share_nn;
+        s.kn_blocks = wblocks < share_kn ? wblocks : share_kn;
+        grid[0] = grid[0] > s.blocks ? grid[0] : s.blocks;
+        grid[1] = grid[1] > s.nn_blocks ? grid[1] : s.nn_blocks;
+        grid[2] = grid[2] > s.kn_blocks ? grid[2] : s.kn_blocks;
+    }
+    const size_t bytes = seqs.size() * sizeof(KdSeq);
+    lead->batch_buf.reserve(bytes + PLS_MAX_SEQUENCES * sizeof(int), st);
+    PLS_CUDA(cudaMemcpyAsync(lead->batch_buf.p, seqs.data(), bytes, cudaMemcpyHostToDevice, st));
+}
+
+// ICP iterations [first, last) of the sequences kdmap_batch_begin described, on st: one launch per kernel for all of
+// them; a sequence on a map of KD_COLD_MAP_POINTS or more runs its later iterations through its own four launches.
+void kdmap_batch_iterations(pls_context* lead, pls_context* const* ctxs, const int64_t* query_bounds, int num, cudaStream_t st,
+                            const int* grid, int first, int last) {
+    const KdSeq* seqs = lead->batch_buf.as<KdSeq>();
+    for (int it = first; it < last; ++it) {
+        if (it == 0) {
+            kd_nn_warp_batch_kernel<<<dim3(grid[1], num), KD_THREADS, 0, st>>>(seqs);
+            PLS_CHECK_LAUNCH();
+            kd_normals_warp_batch_kernel<<<dim3(grid[2], num), KD_THREADS, 0, st>>>(seqs);
+            PLS_CHECK_LAUNCH();
+            kd_residual_batch_kernel<<<dim3(grid[0], num), KD_THREADS, 0, st>>>(seqs);
+            PLS_CHECK_LAUNCH();
+            continue;
+        }
+        kd_icp_refine_batch_kernel<<<dim3(grid[0], num), KD_REFINE_THREADS, 0, st>>>(seqs, it);
+        PLS_CHECK_LAUNCH();
+        for (int i = 0; i < num; ++i) {
+            pls_context* ctx = ctxs[i];
+            if (ctx->kd.indexed < KD_COLD_MAP_POINTS || it >= ctx->cfg.max_num_alignments) continue;
+            cudaStream_t own = ctx->stream;
+            ctx->stream = st;
+            bool solved = false;
+            try {
+                kdmap_icp_iteration(ctx, query_bounds[i], 0, 1, it, ctx->cfg.threshold_delta_pose, &solved);
+            } catch (...) {
+                ctx->stream = own;
+                throw;
+            }
+            ctx->stream = own;
+        }
+    }
+}
+
+// The done flag of every sequence of the batch: one gather launch, one copy, one synchronisation.
+void kdmap_batch_done(pls_context* lead, int num, cudaStream_t st, int* out) {
+    int* dev = reinterpret_cast<int*>(lead->batch_buf.as<char>() + (size_t)num * sizeof(KdSeq));
+    kd_batch_done_kernel<<<1, 64, 0, st>>>(lead->batch_buf.as<KdSeq>(), num, dev);
+    PLS_CHECK_LAUNCH();
+    PLS_CUDA(cudaMemcpyAsync(out, dev, (size_t)num * sizeof(int), cudaMemcpyDeviceToHost, st));
+    PLS_CUDA(cudaStreamSynchronize(st));
 }
 
 }  // namespace pls

@@ -8,6 +8,8 @@
 #include <stdlib.h>
 
 #include <chrono>
+#include <utility>
+#include <vector>
 
 #include "internal.cuh"
 #include "icp_device.cuh"
@@ -312,23 +314,83 @@ struct HostTrace {
 };
 HostTrace g_trace;
 
-// The ICP loop (icp_odometry.py:248-299) over ctx->query_ptr / counts[1]: iterations are enqueued without
-// host syncs and turn into no-ops once the device-side `done` flag latches.  To avoid paying for
+// PLS_BATCH_TRACE=<file>: one JSON line per pls_process_frames call, appended to <file> -- CUDA-event times on the lead
+// stream of the input stage (call start until every sequence's input stage is done) and of the batched ICP (until the
+// FrameResults are copied back), the host time of the epilogue and of the whole call, and the extra ICP rounds.
+// A development aid for the per-phase split of a batched step (tools/multi_sequence_bench.py --phases).
+struct BatchTrace {
+    const char* path = nullptr;
+    cudaEvent_t ev[3] = {nullptr, nullptr, nullptr};
+    std::chrono::steady_clock::time_point t_call, t_epi;
+    int sequences = 0, icp_sequences = 0, extra_rounds = 0;
+    void begin(cudaStream_t st) {
+        path = getenv("PLS_BATCH_TRACE");
+        if (!path) return;
+        t_call = std::chrono::steady_clock::now();
+        for (auto& e : ev) PLS_CUDA(cudaEventCreate(&e));
+        PLS_CUDA(cudaEventRecord(ev[0], st));
+    }
+    void inputs_done(cudaStream_t st, int num, int icp) {
+        sequences = num;
+        icp_sequences = icp;
+        if (path) PLS_CUDA(cudaEventRecord(ev[1], st));
+    }
+    void icp_done(cudaStream_t st) {
+        if (path) PLS_CUDA(cudaEventRecord(ev[2], st));
+    }
+    void epilogue_begin() {
+        if (path) t_epi = std::chrono::steady_clock::now();
+    }
+    void end() {
+        if (!path) return;
+        const auto now = std::chrono::steady_clock::now();
+        float input_ms = 0.f, icp_ms = 0.f;
+        PLS_CUDA(cudaEventSynchronize(ev[1]));
+        PLS_CUDA(cudaEventElapsedTime(&input_ms, ev[0], ev[1]));
+        if (icp_sequences > 0) PLS_CUDA(cudaEventElapsedTime(&icp_ms, ev[1], ev[2]));
+        FILE* f = fopen(path, "a");
+        if (!f) return;
+        fprintf(f, "{\"sequences\": %d, \"icp_sequences\": %d, \"input_ms\": %.6f, \"icp_ms\": %.6f, \"epilogue_ms\": %.6f, "
+                   "\"call_ms\": %.6f, \"extra_rounds\": %d}\n",
+                sequences, icp_sequences, input_ms, icp_ms,
+                std::chrono::duration<double, std::milli>(now - t_epi).count(),
+                std::chrono::duration<double, std::milli>(now - t_call).count(), extra_rounds);
+        fclose(f);
+    }
+    ~BatchTrace() {
+        for (auto e : ev)
+            if (e) cudaEventDestroy(e);
+    }
+};
+
+// The start of a frame's ICP: the FrameResult at T0 (device, or null for the identity), the search counters cleared.
+void frame_begin(pls_context* ctx, const float* T0_dev) {
+    frame_begin_kernel<<<1, kMaxAlign, 0, ctx->stream>>>(frame_result_dev(ctx), T0_dev, ctx->cfg.max_num_alignments,
+                                                         scalar_u32(ctx, SC_KD_COUNTERS));
+    PLS_CHECK_LAUNCH();
+}
+
+// ICP iterations a frame enqueues before its first look at the done flag: the previous frame's count + 1.
+int upfront_iterations(const pls_context* ctx) {
+    const int max_it = ctx->cfg.max_num_alignments;
+    static const bool all_upfront = getenv("PLS_ICP_UPFRONT_ALL") != nullptr;
+    const int upfront = (ctx->last_icp_iters > 0 && !all_upfront) ? ctx->last_icp_iters + 1 : max_it;
+    return upfront > max_it ? max_it : upfront;
+}
+
+// The ICP loop (icp_odometry.py:248-299) over ctx->query_ptr / counts[1], after frame_begin: iterations are enqueued
+// without host syncs and turn into no-ops once the device-side `done` flag latches.  To avoid paying for
 // max_num_alignments launches when ICP converges in 2-3, only `previous frame's count + 1` iterations are
 // enqueued up front; the rare frame that needs more continues after the result fetch (same arithmetic,
 // one extra sync).  Returns the block count of the correspondence kernel.
-int run_icp(pls_context* ctx, const float* T0_dev, int64_t query_bound) {
+int run_icp(pls_context* ctx, int64_t query_bound) {
     cudaStream_t st = ctx->stream;
     FrameResult* fr = frame_result_dev(ctx);
-    frame_begin_kernel<<<1, kMaxAlign, 0, st>>>(fr, T0_dev, ctx->cfg.max_num_alignments, scalar_u32(ctx, SC_KD_COUNTERS));
-    PLS_CHECK_LAUNCH();
     if (query_bound < 1) query_bound = 1;
     ctx->pm.zbuf_clean = false;  // tmp[3] may have been used by the frame's own projection
     ctx->nn_prev.reserve((size_t)query_bound * sizeof(int), st);  // previous matches: ignored by iteration 0
     const int max_it = ctx->cfg.max_num_alignments;
-    static const bool all_upfront = getenv("PLS_ICP_UPFRONT_ALL") != nullptr;
-    int upfront = (ctx->last_icp_iters > 0 && !all_upfront) ? ctx->last_icp_iters + 1 : max_it;
-    if (upfront > max_it) upfront = max_it;
+    const int upfront = upfront_iterations(ctx);
     int blocks = enqueue_icp_iterations(ctx, query_bound, 0, upfront);
     int enq = upfront;
     g_trace.lap(0);
@@ -428,10 +490,27 @@ void flush_map_update(pls_context* ctx) {
 
 namespace {
 
-void process_frame_device(pls_context* ctx, const void* data_void, int layout, int64_t n, const float* init_pose,
-                          float* out_pose, float* out_params, int* out_has_pose, double* out_info) {
+// What a frame's input stage hands to its ICP and its epilogue.
+struct FrameIn {
+    int64_t pts_bound = 0;    // rows of the frame's own points, NaN rows included
+    int64_t query_bound = 0;  // bound of the query count
+    const float* T0_dev = nullptr;
+};
+
+// The caller's outputs of one frame, each nullable.
+struct FrameOut {
+    float* pose;
+    float* params;
+    int* has_pose;
+    double* info;
+};
+
+// The input stage of a frame (icp_odometry.py:319-358, 301-308): input selection, the map-update flush and
+// frame_begin_kernel, on ctx->stream.  A sequence's first frame only initialises the map (icp_odometry.py:171-181): that
+// is done here, outputs included, and false returned.
+bool frame_input(pls_context* ctx, const void* data_void, int layout, int64_t n, const float* init_pose, FrameIn& in,
+                 const FrameOut& out) {
     cudaStream_t st = ctx->stream;
-    g_trace.start();
     // float64 point layouts: same flow, the cloud is rounded to float32 for the queries / map insertion while the frame's
     // own vertex map is projected in float64 (icp_odometry.py:331-352)
     const bool is64 = layout == PLS_INPUT_NDARRAY_F64 || layout == PLS_INPUT_TENSOR_F64;
@@ -511,6 +590,7 @@ void process_frame_device(pls_context* ctx, const void* data_void, int layout, i
                                   frame_vmap.as<float>(), ctx->tmp[3].as<unsigned long long>());
         }
     }
+    in.pts_bound = pts_bound;
 
     float eye[16];
     for (int i = 0; i < 16; ++i) eye[i] = (i % 5 == 0) ? 1.f : 0.f;
@@ -522,17 +602,17 @@ void process_frame_device(pls_context* ctx, const void* data_void, int layout, i
         if (kd) kdmap_update(ctx, eye, nullptr, 0, frame_vmap.as<float>(), H, W, -1);
         else projmap_update(ctx, eye, frame_vmap.as<float>());
         ctx->frame_index = 1;
-        if (out_has_pose) *out_has_pose = 0;
-        if (out_pose) memcpy(out_pose, eye, sizeof(eye));
-        if (out_params) memset(out_params, 0, 6 * sizeof(float));
+        if (out.has_pose) *out.has_pose = 0;
+        if (out.pose) memcpy(out.pose, eye, sizeof(eye));
+        if (out.params) memset(out.params, 0, 6 * sizeof(float));
         fetch_result(ctx);
-        if (out_info) {
+        if (out.info) {
             FrameResult* h = frame_result_host(ctx);
-            for (int i = 0; i < 12; ++i) out_info[i] = 0.0;
-            out_info[3] = (double)ctx->kd.count;
-            out_info[5] = (double)(pts_bound - (int64_t)h->counts[2]);
+            for (int i = 0; i < 12; ++i) out.info[i] = 0.0;
+            out.info[3] = (double)ctx->kd.count;
+            out.info[5] = (double)(pts_bound - (int64_t)h->counts[2]);
         }
-        return;
+        return false;
     }
 
     // ---- sample_points (icp_odometry.py:301-308)
@@ -554,22 +634,26 @@ void process_frame_device(pls_context* ctx, const void* data_void, int layout, i
         ctx->query_ptr = ctx->queries.as<float4>();
         query_bound = n < hw ? n : hw;
     }
+    in.query_bound = query_bound;
 
     // ---- register_new_frame
-    const float* T0_dev = nullptr;
+    in.T0_dev = nullptr;
     if (init_pose) {
         ctx->tmp[6].reserve(16 * sizeof(float), st);
         PLS_CUDA(cudaMemcpyAsync(ctx->tmp[6].p, init_pose, 16 * sizeof(float), cudaMemcpyHostToDevice, st));
-        T0_dev = ctx->tmp[6].as<float>();
+        in.T0_dev = ctx->tmp[6].as<float>();
     }
     flush_map_update(ctx);  // (already enqueued by the grid-sample call of this frame, if there was one)
     map_stream_wait(ctx);   // the ICP below reads the local map the previous frame's update is still building
-    const int icp_blocks = run_icp(ctx, T0_dev, query_bound);
-    fetch_result(ctx);
-    g_trace.lap(1);
+    frame_begin(ctx, in.T0_dev);
+    return true;
+}
+
+// The epilogue of a frame whose ICP result is in the host FrameResult: status, key-frame decision, the deferred map
+// update, outputs.  Throws on a failed ICP, leaving the frame unadvanced and no map update pending.
+void frame_epilogue(pls_context* ctx, const FrameIn& in, const FrameOut& out, bool trace) {
     FrameResult* h = frame_result_host(ctx);
     ctx->last_icp_iters = h->iters;
-    credit_icp_profile(ctx, h, icp_blocks);
     raise_status(ctx, h->status);
 
     // ---- __update_map: decided now, enqueued (on the map stream, beside the NEXT frame's preprocessing) by the next call
@@ -581,23 +665,36 @@ void process_frame_device(pls_context* ctx, const void* data_void, int layout, i
     ctx->upd_count = (long long)h->counts[2];
     static const bool eager = getenv("PLS_MAP_UPDATE_EAGER") != nullptr;  // A/B: enqueue before returning, as before
     if (eager) flush_map_update(ctx);
-    g_trace.lap(2);
+    if (trace) g_trace.lap(2);
     ctx->frame_index += 1;
-    if (out_pose) memcpy(out_pose, h->T, 16 * sizeof(float));
-    if (out_params) memcpy(out_params, h->params, 6 * sizeof(float));
-    if (out_has_pose) *out_has_pose = 1;
-    if (out_info) {
-        out_info[0] = (double)h->iters;
-        out_info[1] = h->iters > 0 ? (double)h->losses[h->iters - 1] : 0.0;
-        out_info[2] = (double)h->counts[1];
-        out_info[3] = (double)ctx->kd.count;
-        out_info[4] = (double)h->counts[0];
-        out_info[5] = (double)(pts_bound - (int64_t)h->counts[2]);
-        out_info[6] = (double)h->status;
-        out_info[7] = insert ? 1.0 : 0.0;
-        out_info[8] = h->first_pt[0]; out_info[9] = h->first_pt[1]; out_info[10] = h->first_pt[2];
-        out_info[11] = ctx->last_sharded ? 1.0 : 0.0;  // the correspondences were split over the ranks
+    if (out.pose) memcpy(out.pose, h->T, 16 * sizeof(float));
+    if (out.params) memcpy(out.params, h->params, 6 * sizeof(float));
+    if (out.has_pose) *out.has_pose = 1;
+    if (out.info) {
+        out.info[0] = (double)h->iters;
+        out.info[1] = h->iters > 0 ? (double)h->losses[h->iters - 1] : 0.0;
+        out.info[2] = (double)h->counts[1];
+        out.info[3] = (double)ctx->kd.count;
+        out.info[4] = (double)h->counts[0];
+        out.info[5] = (double)(in.pts_bound - (int64_t)h->counts[2]);
+        out.info[6] = (double)h->status;
+        out.info[7] = insert ? 1.0 : 0.0;
+        out.info[8] = h->first_pt[0]; out.info[9] = h->first_pt[1]; out.info[10] = h->first_pt[2];
+        out.info[11] = ctx->last_sharded ? 1.0 : 0.0;  // the correspondences were split over the ranks
     }
+}
+
+void process_frame_device(pls_context* ctx, const void* data_void, int layout, int64_t n, const float* init_pose,
+                          float* out_pose, float* out_params, int* out_has_pose, double* out_info) {
+    g_trace.start();
+    const FrameOut out{out_pose, out_params, out_has_pose, out_info};
+    FrameIn in;
+    if (!frame_input(ctx, data_void, layout, n, init_pose, in, out)) return;
+    const int icp_blocks = run_icp(ctx, in.query_bound);
+    fetch_result(ctx);
+    g_trace.lap(1);
+    credit_icp_profile(ctx, frame_result_host(ctx), icp_blocks);
+    frame_epilogue(ctx, in, out, true);
     g_trace.lap(3);
     g_trace.end_frame();
 }
@@ -667,7 +764,8 @@ int pls_register_frame(pls_context* ctx, const float* points, int64_t n, const f
                                  is_device_ptr(T0) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st));
         T0_dev = ctx->tmp[6].as<float>();
     }
-    const int icp_blocks = run_icp(ctx, T0_dev, n);
+    frame_begin(ctx, T0_dev);
+    const int icp_blocks = run_icp(ctx, n);
     fetch_result(ctx);
     FrameResult* h = frame_result_host(ctx);
     credit_icp_profile(ctx, h, icp_blocks);
@@ -735,6 +833,226 @@ int pls_process_frame_grid_sample(pls_context* ctx, const float* raw_points, int
                          out_has_pose, out_info);
     if (out_info) out_info[4] = (double)S;
     PLS_API_END(ctx)
+}
+
+int pls_process_frames(pls_context* const* ctxs, int num, const void* const* data, const int* layouts, const int64_t* n,
+                       double voxel, const float* const* init_poses, float* out_poses, float* out_params, int* out_has_pose,
+                       double* out_info, int* out_status) {
+    // ---- every argument is checked before anything is enqueued: a refused call changes no context
+    const char* why = nullptr;
+    if (!ctxs || num < 0 || num > PLS_MAX_SEQUENCES) why = "pls_process_frames: need 0 <= num <= PLS_MAX_SEQUENCES contexts";
+    else if (num > 0 && (!data || !layouts || !n)) why = "pls_process_frames: data, layouts and n are required";
+    for (int i = 0; !why && i < num; ++i) {
+        const pls_context* c = ctxs[i];
+        if (!c) { why = "pls_process_frames: null context"; break; }
+        if (c->cfg.local_map_type != PLS_MAP_KDTREE) why = "pls_process_frames: batched sequences need a kd-tree local map";
+        else if (c->cfg.gn_max_iters != 1) why = "fused ICP path supports gauss_newton_config.max_iters == 1";
+        else if (c->comm) why = "pls_process_frames: a context with a multi-GPU communicator cannot be batched";
+        else if (c->cfg.device != ctxs[0]->cfg.device) why = "pls_process_frames: every context must be on one device";
+        for (int j = 0; !why && j < i; ++j)
+            if (ctxs[j] == c) why = "pls_process_frames: a context is listed twice";
+        if (why || !data[i]) continue;
+        const int lay = layouts[i] & ~(PLS_PTR_DEVICE | PLS_PTR_HOST);
+        if (lay < PLS_INPUT_NDARRAY || lay > PLS_INPUT_TENSOR_F64) why = "pls_process_frames: unknown layout";
+        else if (voxel > 0.0 && lay != PLS_INPUT_NDARRAY && lay != PLS_INPUT_TENSOR) why = "grid-sampled input is a point layout";
+        else if (lay != PLS_INPUT_VERTEX_MAP && n[i] <= 0) why = "process_frame: empty point cloud";
+    }
+    if (why) {
+        for (int i = 0; ctxs && i < num; ++i)
+            if (ctxs[i]) ctxs[i]->err = why;
+        return PLS_E_INVALID;
+    }
+    std::vector<int> active;
+    for (int i = 0; i < num; ++i)
+        if (data[i]) active.push_back(i);
+    for (int i = 0; i < num; ++i)
+        if (out_status) out_status[i] = PLS_OK;
+    if (active.empty()) return PLS_OK;
+
+    // profiling slots are not credited by a batched call
+    struct ProfileOff {
+        std::vector<std::pair<pls_context*, int>> off;
+        ~ProfileOff() {
+            for (auto& o : off) o.first->prof[o.second].enabled = true;
+        }
+    } prof_off;
+    for (int i : active)
+        for (int w = 0; w < kProfileSlots; ++w)
+            if (ctxs[i]->prof[w].enabled) {
+                ctxs[i]->prof[w].enabled = false;
+                prof_off.off.push_back({ctxs[i], w});
+            }
+
+    pls_context* lead = ctxs[active[0]];
+    int cur = active[0];  // the sequence a failure below belongs to
+    std::vector<int> status((size_t)num, PLS_OK);
+    std::vector<char> finished((size_t)num, 0);  // the sequence's frame is complete (or it was skipped)
+    for (int i = 0; i < num; ++i) finished[i] = data[i] == nullptr;
+    BatchTrace trace;
+    try {
+        PLS_CUDA(cudaSetDevice(lead->cfg.device));
+        const cudaStream_t st = lead->stream;
+        trace.begin(st);
+        auto order_before_lead = [&](pls_context* ctx) {  // ctx's work so far happens-before lead's next work
+            if (ctx == lead) return;
+            if (!ctx->ev_batch) PLS_CUDA(cudaEventCreateWithFlags(&ctx->ev_batch, cudaEventDisableTiming));
+            PLS_CUDA(cudaEventRecord(ctx->ev_batch, ctx->stream));
+            PLS_CUDA(cudaStreamWaitEvent(st, ctx->ev_batch, 0));
+        };
+        // ---- input stage, per sequence on its own stream: the pending map update, the input on the device and, with
+        // voxel > 0, the grid sample, whose counts are read back together
+        std::vector<const void*> dev((size_t)num, nullptr);
+        std::vector<int64_t> rows(n, n + num);
+        std::vector<int> lay((size_t)num);
+        for (int i : active) {
+            cur = i;
+            pls_context* ctx = ctxs[i];
+            flush_map_update(ctx);
+            const int hint = layouts[i] & (PLS_PTR_DEVICE | PLS_PTR_HOST);
+            lay[i] = layouts[i] & ~(PLS_PTR_DEVICE | PLS_PTR_HOST);
+            const bool is64 = lay[i] == PLS_INPUT_NDARRAY_F64 || lay[i] == PLS_INPUT_TENSOR_F64;
+            const size_t bytes = lay[i] == PLS_INPUT_VERTEX_MAP ? (size_t)3 * ctx->cfg.height * ctx->cfg.width * sizeof(float)
+                                                                : (size_t)n[i] * 3 * (is64 ? sizeof(double) : sizeof(float));
+            dev[i] = data[i];
+            if (hint == PLS_PTR_HOST) {
+                ctx->stage_in[0].reserve(bytes, ctx->stream);
+                PLS_CUDA(cudaMemcpyAsync(ctx->stage_in[0].p, data[i], bytes, cudaMemcpyHostToDevice, ctx->stream));
+                dev[i] = ctx->stage_in[0].p;
+            } else if (hint != PLS_PTR_DEVICE) {
+                dev[i] = to_device(ctx, data[i], bytes, ctx->stage_in[0]);
+            }
+            if (voxel > 0.0) {
+                ctx->gs_out_xyz.reserve((size_t)n[i] * 3 * sizeof(float), ctx->stream);
+                grid_sample_device<float>(ctx, (const float*)dev[i], n[i], voxel, ctx->gs_out_xyz.as<float>(), nullptr, true);
+                grid_sample_count_to_host(ctx);
+                order_before_lead(ctx);
+            }
+        }
+        if (voxel > 0.0) {
+            PLS_CUDA(cudaStreamSynchronize(st));
+            for (int i : active) {
+                cur = i;
+                pls_context* ctx = ctxs[i];
+                bool overflowed = false;
+                uint32_t S = grid_sample_host_count(ctx, &overflowed);
+                if (overflowed) {  // hashes beyond the 40-bit keys: once more on the raw 64-bit keys
+                    grid_sample_device<float>(ctx, (const float*)dev[i], n[i], voxel, ctx->gs_out_xyz.as<float>(), nullptr, false);
+                    S = grid_sample_read_count(ctx, &overflowed);
+                }
+                dev[i] = ctx->gs_out_xyz.p;
+                rows[i] = (int64_t)S;
+            }
+        }
+        std::vector<FrameIn> in((size_t)num);
+        std::vector<pls_context*> icp;
+        std::vector<int> icp_seq;
+        std::vector<int64_t> bounds;
+        auto outputs = [&](int i) {
+            return FrameOut{out_poses ? out_poses + 16 * i : nullptr, out_params ? out_params + 6 * i : nullptr,
+                            out_has_pose ? out_has_pose + i : nullptr, out_info ? out_info + 12 * i : nullptr};
+        };
+        for (int i : active) {
+            cur = i;
+            pls_context* ctx = ctxs[i];
+            bool runs_icp = false;
+            try {
+                runs_icp = frame_input(ctx, dev[i], lay[i], rows[i], init_poses ? init_poses[i] : nullptr, in[i], outputs(i));
+            } catch (const pls::Error& e) {
+                // an input the single path refuses (e.g. a grid sample of no point) is that sequence's error alone
+                if (e.code != PLS_E_INVALID) throw;
+                ctx->err = e.msg;
+                status[i] = e.code;
+                finished[i] = 1;
+                continue;
+            }
+            if (!runs_icp) {
+                if (voxel > 0.0 && out_info) out_info[12 * i + 4] = (double)rows[i];
+                finished[i] = 1;
+                continue;
+            }
+            ctx->pm.zbuf_clean = false;
+            icp.push_back(ctx);
+            icp_seq.push_back(i);
+            bounds.push_back(in[i].query_bound < 1 ? 1 : in[i].query_bound);
+            order_before_lead(ctx);
+        }
+        // ---- the ICP of every sequence on the lead's stream, each kernel one launch for all of them
+        const int m = (int)icp.size();
+        trace.inputs_done(st, (int)active.size(), m);
+        if (m > 0) {
+            cur = icp_seq[0];
+            int grid[3];
+            kdmap_batch_begin(lead, icp.data(), bounds.data(), m, st, grid);
+            int upfront = 0, max_it = 0;
+            for (pls_context* ctx : icp) {
+                const int u = upfront_iterations(ctx);
+                upfront = u > upfront ? u : upfront;
+                max_it = ctx->cfg.max_num_alignments > max_it ? ctx->cfg.max_num_alignments : max_it;
+            }
+            kdmap_batch_iterations(lead, icp.data(), bounds.data(), m, st, grid, 0, upfront);
+            int enq = upfront;
+            std::vector<int> done((size_t)m);
+            while (enq < max_it) {
+                // continue only for a sequence whose device has not latched `done` (the rare path, as on a single one)
+                kdmap_batch_done(lead, m, st, done.data());
+                bool more = false;
+                for (int j = 0; j < m; ++j) more = more || (!done[j] && enq < icp[j]->cfg.max_num_alignments);
+                if (!more) break;
+                const int k = (max_it - enq) < 4 ? (max_it - enq) : 4;
+                kdmap_batch_iterations(lead, icp.data(), bounds.data(), m, st, grid, enq, enq + k);
+                enq += k;
+                trace.extra_rounds += 1;
+            }
+            for (pls_context* ctx : icp)  // each FrameResult and the scalar slots behind it
+                PLS_CUDA(cudaMemcpyAsync(ctx->pinned.p, ctx->scalars.p, kScalarOffset + SC_NUM * sizeof(uint32_t),
+                                         cudaMemcpyDeviceToHost, st));
+            trace.icp_done(st);
+            PLS_CUDA(cudaStreamSynchronize(st));
+        }
+        trace.epilogue_begin();
+        // ---- epilogue, per sequence: a failed ICP is that sequence's error alone
+        for (int j = 0; j < m; ++j) {
+            const int i = icp_seq[j];
+            cur = i;
+            try {
+                frame_epilogue(icp[j], in[i], outputs(i), false);
+                if (voxel > 0.0 && out_info) out_info[12 * i + 4] = (double)rows[i];
+            } catch (const pls::Error& e) {
+                if (e.code != PLS_E_SINGULAR) throw;
+                icp[j]->err = e.msg;
+                status[i] = e.code;
+            }
+            finished[i] = 1;
+        }
+        trace.end();
+    } catch (...) {
+        // a failure no sequence can be blamed for alone (CUDA): every sequence whose frame did not complete reports it;
+        // those that completed (a frame 0, a refused input) keep their status
+        int code = PLS_E_INVALID;
+        std::string msg;
+        try {
+            throw;
+        } catch (const pls::Error& e) {
+            code = e.code;
+            msg = e.msg;
+        } catch (const std::exception& e) {
+            msg = e.what();
+        }
+        for (int i = 0; i < num; ++i) {
+            if (!finished[i]) {
+                status[i] = code;
+                ctxs[i]->err = msg;
+            }
+            if (out_status) out_status[i] = status[i];
+        }
+        return code;
+    }
+    int first_error = PLS_OK;
+    for (int i = 0; i < num; ++i) {
+        if (out_status) out_status[i] = status[i];
+        if (first_error == PLS_OK) first_error = status[i];
+    }
+    return first_error;
 }
 
 }  // extern "C"

@@ -643,15 +643,24 @@ class ICPFrameToModel(OdometryAlgorithm):
         self._iter += 1
 
     def do_process_next_frame(self, data_dict: dict):
+        if self._fine_grained:
+            self._check_data_key(data_dict)
+            return self._process_fine_grained(data_dict)
+        layout, data, n, address, init = self._frame_arguments(data_dict)
+        self.ctx.call("pls_process_frame", address, layout, n, _lib.ptr(init), *self._out_args)
+        self._frame_outputs(data_dict, layout, data)
+
+    def _check_data_key(self, data_dict: dict):
         assert_debug(self.config.data_key in data_dict,
                      f"Could not find the key `{self.config.data_key}` in the input dictionary.\n"
                      f"With keys : {data_dict.keys()}). Set the parameter `slam.odometry.data_key` to the desired key")
-        if self._fine_grained:
-            return self._process_fine_grained(data_dict)
+
+    def _frame_arguments(self, data_dict: dict):
+        """The C-ABI arguments of one frame: (layout, data, n, address, init pose).  Raises before anything runs."""
+        self._check_data_key(data_dict)
         layout, data, n = self._interpret(data_dict[self.config.data_key])
         init = data_dict.get("init_rpose", None)
         init = None if init is None else np.ascontiguousarray(np.asarray(init, dtype=np.float32).reshape(4, 4))
-        has_pose = self._has_pose
         address = _lib.ptr(data)
         if layout & _lib.PTR_HOST and n == _lib.Handoff.rows:
             # the array GridSample.filter handed out (possibly wrapped by ToTensor): its device-resident twin is used
@@ -659,13 +668,16 @@ class ICPFrameToModel(OdometryAlgorithm):
             twin = _lib.Handoff.match(address, n, bool((layout & 0xff) >= _lib.INPUT_NDARRAY_F64), int(self.ctx.cfg.device))
             if twin:
                 address, layout = twin, (layout & 0xff) | _lib.PTR_DEVICE
-        self.ctx.call("pls_process_frame", address, layout, n, _lib.ptr(init), *self._out_args)
+        return layout, data, n, address, init
+
+    def _frame_outputs(self, data_dict: dict, layout: int, data):
+        """Poses and data_dict entries of a frame whose results are in _pose_out, _params_out, _has_pose, last_info."""
         layout &= 0xff
         if int(self.last_info[6]) == _lib.PLS_W_TINY_RESIDUAL:   # GaussNewton.compute's warning (optimization.py:323-327)
             import logging
             logging.warning("The residual norm is lower than threshold 1e-7. "
                             "This would lead to invalid jacobian. We prefer Stopping ICP")
-        if not has_pose.value:
+        if not self._has_pose.value:
             eye = np.eye(4, dtype=np.float32).reshape(1, 4, 4)
             self.relative_poses.append(eye)
             self.absolute_poses.append(np.eye(4, dtype=np.float64))
@@ -703,6 +715,90 @@ class ICPFrameToModel(OdometryAlgorithm):
         self.ctx.call("pls_register_frame", _lib.ptr(pts), pts.shape[0], _lib.ptr(T0), _lib.ptr(T), _lib.ptr(params),
                       _lib.ptr(losses), C.byref(iters))
         return params, T, list(losses[:iters.value])
+
+
+class ICPFrameToModelBatch:
+    """Advances several independent ICPFrameToModel sequences by one frame each in ONE `pls_process_frames` call (no
+    reference counterpart: the reference's runner processes the sequences of a dataset one after another,
+    odometry_runner.py:145-175).  Every kernel of an ICP iteration is one launch for all of them, and every sequence
+    computes exactly what its own process_next_frame would: its poses, data_dict entries and local map.  Each odometry
+    keeps its own state, so process_next_frame and process_next_frames may be mixed on the same objects.
+
+        odos = [ICPFrameToModel(cfg, projector=proj) for _ in range(B)]
+        batch = ICPFrameToModelBatch(odos)
+        for o in odos: o.init()
+        batch.process_next_frames([dd0, dd1, None, dd3])   # None: no frame for that sequence this step
+
+    Supported: kd-tree local maps, gauss_newton_config.max_iters == 1, one CUDA device, at most 64 sequences."""
+
+    def __init__(self, odometries):
+        odos = list(odometries)
+        assert_debug(1 <= len(odos) <= _lib.MAX_SEQUENCES, f"between 1 and {_lib.MAX_SEQUENCES} odometries")
+        for o in odos:
+            assert_debug(isinstance(o, ICPFrameToModel), "ICPFrameToModelBatch batches ICPFrameToModel objects")
+            assert_debug(not o._fine_grained, "batched sequences need gauss_newton_config.max_iters == 1")
+            assert_debug(o.ctx.cfg.local_map_type == _lib.MAP_KDTREE, "batched sequences need a kd-tree local map")
+        assert_debug(len({id(o) for o in odos}) == len(odos), "an odometry is listed twice")
+        assert_debug(len({int(o.ctx.cfg.device) for o in odos}) == 1, "every odometry must run on one CUDA device")
+        self.odometries = odos
+        B = len(odos)
+        self._handles = (C.c_void_p * B)(*[o.ctx.handle.value for o in odos])
+        self._poses = np.zeros((B, 16), np.float32)
+        self._params = np.zeros((B, 6), np.float32)
+        self._has_pose = np.zeros(B, np.int32)
+        self._info = np.zeros((B, 12), np.float64)
+        self._status = np.zeros(B, np.int32)
+
+    def process_next_frames(self, data_dicts):
+        """data_dicts[i] is the next frame of sequence i, or None to leave it alone.  Each data_dict receives what
+        process_next_frame writes; a singular ICP raises RuntimeError after every other sequence's data_dict is filled."""
+        odos = self.odometries
+        B = len(odos)
+        assert_debug(len(data_dicts) == B, f"one data_dict (or None) per odometry: {B} expected")
+        beginning = time.time()
+        args = [None if dd is None else o._frame_arguments(dd) for o, dd in zip(odos, data_dicts)]
+        active = [i for i in range(B) if args[i] is not None]
+        if not active:
+            return
+        data = (C.c_void_p * B)(*[None if a is None else a[3] for a in args])
+        layouts = (C.c_int * B)(*[0 if a is None else a[0] for a in args])
+        n = (C.c_int64 * B)(*[0 if a is None else a[2] for a in args])
+        inits = (C.c_void_p * B)(*[None if a is None else _lib.ptr(a[4]) for a in args])
+        if _lib._cuda_inputs:   # CUDA tensors: their producers on PyTorch's current stream go first
+            devices = list(_lib._cuda_inputs)
+            _lib._cuda_inputs.clear()
+            for d in devices:
+                if d == int(odos[0].ctx.cfg.device):
+                    stream = torch.cuda.current_stream(d).cuda_stream
+                    for i in active:
+                        odos[i].ctx.call("pls_wait_stream", stream)
+                else:
+                    torch.cuda.current_stream(d).synchronize()
+        self._status[:] = _lib.PLS_OK
+        status = odos[active[0]].ctx.process_frames(self._handles, B, data, layouts, n, 0.0, inits, _lib.ptr(self._poses),
+                                                    _lib.ptr(self._params), _lib.ptr(self._has_pose),
+                                                    _lib.ptr(self._info), _lib.ptr(self._status))
+        # every sequence whose frame completed gets its outputs, also when another one failed
+        done = [i for i in active if self._status[i] == _lib.PLS_OK]
+        for i in done:
+            o = odos[i]
+            o._pose_out[:] = self._poses[i].reshape(4, 4)
+            o._params_out[:] = self._params[i]
+            o._has_pose.value = int(self._has_pose[i])
+            o.last_info[:] = self._info[i]
+            o._frame_outputs(data_dicts[i], args[i][0], args[i][1])
+        share = (time.time() - beginning) / len(active)
+        for i in done:
+            odos[i].elapsed.append(share)
+        failed = [i for i in active if self._status[i] not in (_lib.PLS_OK, _lib.PLS_E_SINGULAR)]
+        if failed or status not in (_lib.PLS_OK, _lib.PLS_E_SINGULAR):
+            bad = failed[0] if failed else active[0]
+            odos[bad].ctx.check(int(self._status[bad]) if failed else status)
+        singular = [i for i in active if self._status[i] == _lib.PLS_E_SINGULAR]
+        if singular:
+            import logging
+            logging.error("Invalid Jacobian in Gauss Newton minimization, the hessian is not invertible")
+            raise RuntimeError(f"Invalid Jacobian in Gauss Newton minimization (sequences {singular})")
 
 
 class ODOMETRY(ObjectLoaderEnum, Enum):
