@@ -34,7 +34,8 @@ __global__ void voxel_hash_kernel(const T* __restrict__ xyz, int64_t n, double v
         long long cx = __double2ll_rn(x / voxel);
         long long cy = __double2ll_rn(y / voxel_y);
         long long cz = __double2ll_rn(z / voxel_z);
-        long long h = HX * cx + HY * cy + HZ * cz;
+        // modulo 2^64 like numba's int64 arithmetic: signed overflow would be undefined behaviour
+        const long long h = (long long)((uint64_t)HX * (uint64_t)cx + (uint64_t)HY * (uint64_t)cy + (uint64_t)HZ * (uint64_t)cz);
         if (coords) {
             coords[3 * i] = cx;
             coords[3 * i + 1] = cy;

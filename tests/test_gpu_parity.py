@@ -291,10 +291,11 @@ def test_kd_local_map_golden(b200, golden_helpers):
     assert np.mean(dots > 1 - 1e-4) > 0.99
 
 
-@pytest.mark.parametrize("M,N", [(1, 7), (3, 50), (11, 100), (5000, 3000), (330000, 20000)])
+@pytest.mark.parametrize("M,N", [(1, 7), (3, 50), (11, 100), (2047, 3000), (2048, 3000), (2049, 3000), (5000, 3000),
+                                 (4 * 2048 + 1, 3000), (330000, 20000)])
 def test_kd_exact_nn_vs_bruteforce(b200, M, N):
     """Exactness independent of the oracle (the reference never tests KdTreeLocalMap): brute force,
-    ragged/tiny maps, heavy duplicates."""
+    ragged/tiny maps, heavy duplicates, maps on the edges of the index build's 2048-key sort tiles."""
     rng = np.random.RandomState(M)
     m = (rng.randn(M, 3) * np.array([40, 40, 3])).astype(np.float32)
     if M >= 5000:
