@@ -186,13 +186,12 @@ inline int grid_for(int64_t n, int threads = 256) {
 }  // namespace
 
 // Device-resident grid sample: xyz_dev [n,3] -> out_xyz_dev [<=n,3], out_idx_dev [<=n] (nullable);
-// the sample count lands in the device scalar SC_GS_COUNT.
+// the sample count lands in the device scalar SC_GS_COUNT.  compact: sort on GS_COMPACT_BITS-bit keys, stamping gs_seq
+// into SC_GS_OVERFLOW if a hash does not fit them.
 template <typename T>
 void grid_sample_device(pls_context* ctx, const T* xyz_dev, int64_t n, double voxel, T* out_xyz_dev,
                         long long* out_idx_dev, bool compact, T* host_xyz, long long* host_idx) {
     cudaStream_t st = ctx->stream;
-    static const bool full_keys = getenv("PLS_GS_FULLKEYS") != nullptr;  // A/B: always sort the raw 64-bit hashes
-    if (full_keys) compact = false;
     ProfileScope ps(ctx, 4, (double)n * 3 * sizeof(T));
     ctx->gs_keys.reserve((size_t)n * sizeof(uint64_t), st);
     ctx->gs_vals.reserve((size_t)n * sizeof(uint32_t), st);
@@ -267,10 +266,7 @@ void voxel_statistics_device(pls_context* ctx, const T* xyz_dev, int64_t n, doub
     PLS_CHECK_LAUNCH();
 }
 
-template void grid_sample_device<float>(pls_context*, const float*, int64_t, double, float*, long long*, bool, float*,
-                                        long long*);
-template void grid_sample_device<double>(pls_context*, const double*, int64_t, double, double*, long long*, bool, double*,
-                                         long long*);
+namespace {
 
 void grid_sample_count_to_host(pls_context* ctx) {
     // into the pinned block behind the host FrameResult: a pageable destination would make the copy synchronous
@@ -286,10 +282,31 @@ uint32_t grid_sample_host_count(pls_context* ctx, bool* overflowed) {
     return words[SC_GS_COUNT];
 }
 
-uint32_t grid_sample_read_count(pls_context* ctx, bool* overflowed) {
+void grid_sample_launch(pls_context* ctx, const GridSample& g, bool compact) {
+    if (!g.f64)
+        grid_sample_device<float>(ctx, (const float*)g.xyz, g.n, g.voxel, (float*)g.out_xyz, g.out_idx, compact,
+                                  (float*)g.host_xyz, g.host_idx);
+    else
+        grid_sample_device<double>(ctx, (const double*)g.xyz, g.n, g.voxel, (double*)g.out_xyz, g.out_idx, compact,
+                                   (double*)g.host_xyz, g.host_idx);
+}
+
+}  // namespace
+
+void grid_sample_enqueue(pls_context* ctx, const GridSample& g) {
+    grid_sample_launch(ctx, g, true);
+    grid_sample_count_to_host(ctx);
+}
+
+uint32_t grid_sample_finish(pls_context* ctx, const GridSample& g) {
+    bool overflowed = false;
+    const uint32_t count = grid_sample_host_count(ctx, &overflowed);
+    if (!overflowed) return count;
+    // hashes beyond 40 bits: once more on the raw 64-bit keys
+    grid_sample_launch(ctx, g, false);
     grid_sample_count_to_host(ctx);
     PLS_CUDA(cudaStreamSynchronize(ctx->stream));
-    return grid_sample_host_count(ctx, overflowed);
+    return grid_sample_host_count(ctx, &overflowed);
 }
 
 }  // namespace pls
@@ -334,19 +351,10 @@ int pls_grid_sample(pls_context* ctx, const void* xyz, int is_f64, int64_t n, do
     const void* d_xyz = to_device(ctx, xyz, (size_t)n * 3 * esz, ctx->stage_in[0]);
     OutArg ox = out_arg(ctx, out_xyz, (size_t)n * 3 * esz, ctx->stage_out[0]);
     OutArg oi = out_arg(ctx, out_idx, (size_t)n * sizeof(int64_t), ctx->stage_out[1]);
-    uint32_t count = 0;
-    for (int attempt = 0; attempt < 2; ++attempt) {
-        const bool compact = attempt == 0;
-        if (is_f64)
-            grid_sample_device<double>(ctx, (const double*)d_xyz, n, voxel, (double*)ox.dev, (long long*)oi.dev, compact,
-                                       nullptr, nullptr);
-        else
-            grid_sample_device<float>(ctx, (const float*)d_xyz, n, voxel, (float*)ox.dev, (long long*)oi.dev, compact,
-                                      nullptr, nullptr);
-        bool overflowed = false;
-        count = grid_sample_read_count(ctx, &overflowed);
-        if (!(compact && overflowed)) break;  // hashes beyond 40 bits: once more on the raw 64-bit keys
-    }
+    const GridSample g{d_xyz, is_f64 != 0, n, voxel, ox.dev, (long long*)oi.dev, nullptr, nullptr};
+    grid_sample_enqueue(ctx, g);
+    PLS_CUDA(cudaStreamSynchronize(ctx->stream));
+    const uint32_t count = grid_sample_finish(ctx, g);
     *out_count = count;
     finish_out(ctx, ox, (size_t)count * 3 * esz);
     finish_out(ctx, oi, (size_t)count * sizeof(int64_t));
@@ -380,21 +388,11 @@ int pls_grid_sample_staged(pls_context* ctx, const void* xyz, int is_f64, int64_
         map_xyz = ctx->gs_host_xyz.device_ptr();
         map_idx = ctx->gs_host_idx.device_ptr();
     }
-    uint32_t count = 0;
-    for (int attempt = 0; attempt < 2; ++attempt) {
-        const bool compact = attempt == 0;
-        if (is_f64)
-            grid_sample_device<double>(ctx, (const double*)d_xyz, n, voxel, dev_xyz.as<double>(), nullptr, compact,
-                                       (double*)map_xyz, (long long*)map_idx);
-        else
-            grid_sample_device<float>(ctx, (const float*)d_xyz, n, voxel, dev_xyz.as<float>(), nullptr, compact,
-                                      (float*)map_xyz, (long long*)map_idx);
-        flush_map_update(ctx);  // the last frame's local-map update is enqueued while the subsample runs
-        bool overflowed = false;
-        count = grid_sample_read_count(ctx, &overflowed);
-        if (!(compact && overflowed)) break;  // hashes beyond 40 bits: once more on the raw 64-bit keys
-    }
-    *out_count = count;
+    const GridSample g{d_xyz, is_f64 != 0, n, voxel, dev_xyz.p, nullptr, map_xyz, (long long*)map_idx};
+    grid_sample_enqueue(ctx, g);
+    flush_map_update(ctx);  // the last frame's local-map update is enqueued while the subsample runs
+    PLS_CUDA(cudaStreamSynchronize(ctx->stream));
+    *out_count = grid_sample_finish(ctx, g);
     *out_xyz_host = host_xyz;
     *out_idx_host = host_idx;
     if (out_xyz_dev) *out_xyz_dev = dev_xyz.p;

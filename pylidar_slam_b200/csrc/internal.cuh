@@ -394,20 +394,26 @@ void pack_valid_rows_f64(pls_context* ctx, const double* pts_dev, int64_t n, flo
 void pack_valid_pixels(pls_context* ctx, const float* vmap_dev, int64_t hw, float min_norm, float4* out,
                        uint32_t* count_dev);
 // grid_sample.cu
-// compact = true sorts on 40-bit keys (5 radix passes instead of 8): exact whenever every hash lies in [-2^39, 2^39),
-// i.e. voxel coordinates up to ~3 000 000 in magnitude; otherwise the kernel stamps `gs_seq` into the device scalar
-// SC_GS_OVERFLOW and the caller -- which reads the sample count back anyway -- repeats the call with compact = false
-// (grid_sample_overflowed() tells).
-template <typename T>
-void grid_sample_device(pls_context* ctx, const T* xyz_dev, int64_t n, double voxel, T* out_xyz_dev,
-                        long long* out_idx_dev, bool compact = true, T* host_xyz = nullptr, long long* host_idx = nullptr);
-// Reads SC_GS_COUNT (and the overflow stamp) back: one 32-byte copy + one stream sync.  Returns the sample count;
-// *overflowed tells whether the last compact grid sample has to be repeated with full keys.
-uint32_t grid_sample_read_count(pls_context* ctx, bool* overflowed);
-// The same in two halves, for callers that synchronise once for several contexts: the copy (enqueued on ctx->stream),
-// then, after the stream has been synchronised, the count and overflow test.
-void grid_sample_count_to_host(pls_context* ctx);
-uint32_t grid_sample_host_count(pls_context* ctx, bool* overflowed);
+// A grid sample whose sample count the host reads back: xyz [n,3] (float64 if f64, else float32) -> out_xyz [<=n,3] and
+// out_idx [<=n] (nullable) on the device; with host_xyz and host_idx (device aliases of mapped pinned memory) the
+// gather also writes a host copy.
+struct GridSample {
+    const void* xyz;
+    bool f64;
+    int64_t n;
+    double voxel;
+    void* out_xyz;
+    long long* out_idx;
+    void* host_xyz;
+    long long* host_idx;
+};
+// The sample runs in two halves on ctx->stream, so that a caller can synchronise once for several contexts.  enqueue
+// sorts on 40-bit keys (5 radix passes instead of 8), exact whenever every hash lies in [-2^39, 2^39), i.e. voxel
+// coordinates up to ~3 000 000 in magnitude, and copies the count and the overflow stamp to the host.  finish, once
+// ctx->stream has been synchronised, returns the count; if a hash overflowed the compact keys it first samples once more
+// on the raw 64-bit keys and reads that count (one more copy and stream synchronisation).
+void grid_sample_enqueue(pls_context* ctx, const GridSample& g);
+uint32_t grid_sample_finish(pls_context* ctx, const GridSample& g);
 // projmap.cu
 void projmap_reset(pls_context* ctx);
 // odometry.cu: would an ICP iteration over `work` items be split across the ranks (the rule of enqueue_icp_iterations)?

@@ -1062,24 +1062,46 @@ static void record_search(KdMap& kd, bool icp, bool sharded, bool normals, int64
     kd.searched_n = n;
 }
 
+// One sequence's kd search and ICP iteration over `query_bound` queries split over `num_ranks` shards: this shard's query
+// bound, its work-list slots and its block counts.
+struct KdPlan {
+    int64_t mine;  // queries of this shard
+    size_t slots;  // work-list slots of this shard
+    int blocks;    // residual and refine kernels
+    int wblocks;   // warp kernels (1-NN, normals), before the cap at a resident wave
+};
+
+// Reserves, on ctx->stream, what the plan's iterations use: nn_prev and kd_nn_state are indexed by query (not by shard
+// slot), kd_worklist holds two lists of the shard's slots, partials one row per residual block.
+static KdPlan plan_kd_iteration(pls_context* ctx, int64_t query_bound, int num_ranks) {
+    cudaStream_t st = ctx->stream;
+    KdPlan p;
+    p.mine = (query_bound + num_ranks - 1) / num_ranks;
+    p.slots = (size_t)p.mine + 64;
+    p.blocks = grid_for(p.mine, KD_THREADS, 8 * kNumSMs);
+    p.wblocks = (int)((p.mine + KD_WARPS - 1) / KD_WARPS);
+    ctx->nn_prev.reserve((size_t)query_bound * sizeof(int), st);  // previous matches: ignored by iteration 0
+    ctx->partials.reserve((size_t)p.blocks * NACC * sizeof(double), st);
+    ctx->kd_worklist.reserve(2 * p.slots * sizeof(int), st);
+    ctx->kd_nn_state.reserve(p.slots * (size_t)num_ranks * sizeof(float4), st);
+    return p;
+}
+
 // The search of one ICP iteration (or of one fine-grained API call).  first: every query is searched; later iterations
 // first verify the previous matches and search only the unproven ones.
-static void launch_search(pls_context* ctx, const KdIndex& ix, const float4* queries, const uint32_t* nq_dev, int64_t mine,
+static void launch_search(pls_context* ctx, const KdPlan& plan, const KdIndex& ix, const float4* queries, const uint32_t* nq_dev,
                           int rank, int num_ranks, const float* T, const int* done, int* match, bool first, bool normals,
                           int parity) {
     cudaStream_t st = ctx->stream;
-    const size_t slots = (size_t)mine + 64;
-    ctx->kd_worklist.reserve(2 * slots * sizeof(int), st);
-    ctx->kd_nn_state.reserve(slots * (size_t)num_ranks * sizeof(float4), st);  // indexed by query, not by shard slot
     int* pending = ctx->kd_worklist.as<int>();
-    int* hard_nn = pending + slots;
+    int* hard_nn = pending + plan.slots;
     float4* nn_state = ctx->kd_nn_state.as<float4>();
     uint32_t* lists = scalar_u32(ctx, SC_KD_LISTS);
     unsigned long long* counters = kd_counters(ctx);
-    const int tblocks = (int)((mine + KD_THREADS - 1) / KD_THREADS);
+    const int tblocks = (int)((plan.mine + KD_THREADS - 1) / KD_THREADS);
     static const int resident_nn = resident_blocks((const void*)kd_nn_warp_kernel);
     static const int resident_kn = resident_blocks((const void*)kd_normals_warp_kernel);
-    const int wblocks = (int)((mine + KD_WARPS - 1) / KD_WARPS);
+    const int wblocks = plan.wblocks;
     if (!first) {
         ProfileScope p6(ctx, 6, 0.0);
         kd_nn_verify_kernel<<<tblocks, KD_THREADS, 0, st>>>(ix, queries, nq_dev, (int64_t)rank, (int64_t)num_ranks, T, done, match,
@@ -1112,17 +1134,16 @@ int kdmap_icp_iteration(pls_context* ctx, int64_t query_bound, int rank, int num
                         bool* solved) {
     PLS_REQUIRE(ctx->kd.valid, "kd map: search before any update");
     cudaStream_t st = ctx->stream;
-    const int64_t mine = (query_bound + num_ranks - 1) / num_ranks;
     FrameResult* fr = frame_result_dev(ctx);
     const uint32_t* nq_dev = reinterpret_cast<const uint32_t*>(&fr->counts[1]);
     // credited per executed iteration by the caller (the launch is a no-op once ICP converged)
     ProfileScope ps(ctx, 0, 0.0, false);
     const KdIndex ix = make_index(ctx);
-    const int blocks = grid_for(mine, KD_THREADS, 8 * kNumSMs);
-    ctx->partials.reserve((size_t)blocks * NACC * sizeof(double), st);
+    const KdPlan plan = plan_kd_iteration(ctx, query_bound, num_ranks);
+    const int blocks = plan.blocks;
     record_search(ctx->kd, true, num_ranks > 1, true, 0);
     if (it == 0 || ctx->kd.indexed >= KD_COLD_MAP_POINTS) {
-        launch_search(ctx, ix, ctx->query_ptr, nq_dev, mine, rank, num_ranks, fr->T, &fr->done, ctx->nn_prev.as<int>(), it == 0,
+        launch_search(ctx, plan, ix, ctx->query_ptr, nq_dev, rank, num_ranks, fr->T, &fr->done, ctx->nn_prev.as<int>(), it == 0,
                       true, it & 1);
         ProfileScope p10(ctx, 10, 0.0);
         kd_residual_kernel<<<blocks, KD_THREADS, 0, st>>>(ix, ctx->query_ptr, nq_dev, (int64_t)rank, (int64_t)num_ranks, fr,
@@ -1154,13 +1175,7 @@ void kdmap_batch_begin(pls_context* lead, pls_context* const* ctxs, const int64_
     for (int i = 0; i < num; ++i) {
         pls_context* ctx = ctxs[i];
         PLS_REQUIRE(ctx->kd.valid, "kd map: search before any update");
-        const int64_t mine = query_bounds[i];
-        const size_t slots = (size_t)mine + 64;
-        const int blocks = grid_for(mine, KD_THREADS, 8 * kNumSMs);
-        ctx->nn_prev.reserve((size_t)mine * sizeof(int), ctx->stream);
-        ctx->partials.reserve((size_t)blocks * NACC * sizeof(double), ctx->stream);
-        ctx->kd_worklist.reserve(2 * slots * sizeof(int), ctx->stream);
-        ctx->kd_nn_state.reserve(slots * sizeof(float4), ctx->stream);
+        const KdPlan plan = plan_kd_iteration(ctx, query_bounds[i], 1);
         ctx->last_sharded = false;
         record_search(ctx->kd, true, false, true, 0);
         FrameResult* fr = frame_result_dev(ctx);
@@ -1180,11 +1195,10 @@ void kdmap_batch_begin(pls_context* lead, pls_context* const* ctxs, const int64_
         s.k_normals = ctx->cfg.num_neighbors_normals;
         s.fuse_threshold = ctx->cfg.threshold_delta_pose;
         s.max_iters = ctx->cfg.max_num_alignments;
-        s.blocks = blocks;
-        s.refine_blocks = ctx->kd.indexed >= KD_COLD_MAP_POINTS ? 0 : blocks;
-        const int wblocks = (int)((mine + KD_WARPS - 1) / KD_WARPS);
-        s.nn_blocks = wblocks < share_nn ? wblocks : share_nn;
-        s.kn_blocks = wblocks < share_kn ? wblocks : share_kn;
+        s.blocks = plan.blocks;
+        s.refine_blocks = ctx->kd.indexed >= KD_COLD_MAP_POINTS ? 0 : plan.blocks;
+        s.nn_blocks = plan.wblocks < share_nn ? plan.wblocks : share_nn;
+        s.kn_blocks = plan.wblocks < share_kn ? plan.wblocks : share_kn;
         grid[0] = grid[0] > s.blocks ? grid[0] : s.blocks;
         grid[1] = grid[1] > s.nn_blocks ? grid[1] : s.nn_blocks;
         grid[2] = grid[2] > s.kn_blocks ? grid[2] : s.kn_blocks;
@@ -1318,7 +1332,6 @@ int pls_kdmap_nn_search(pls_context* ctx, const float* queries, int64_t n, float
     // the same warp-cooperative kernels as the ICP loop, with an identity transform and no previous matches
     cudaStream_t st = ctx->stream;
     ctx->queries.reserve((size_t)n * sizeof(float4), st);
-    ctx->nn_prev.reserve((size_t)n * sizeof(int), st);
     ctx->tmp[6].reserve(16 * sizeof(float) + 16, st);
     static const float eye12[12] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0};
     PLS_CUDA(cudaMemcpyAsync(ctx->tmp[6].p, eye12, sizeof(eye12), cudaMemcpyHostToDevice, st));
@@ -1329,8 +1342,9 @@ int pls_kdmap_nn_search(pls_context* ctx, const float* queries, int64_t n, float
     kd_rows_to_float4_kernel<<<grid_for(n, 256, 8 * kNumSMs), 256, 0, st>>>(d, n, ctx->queries.as<float4>());
     PLS_CHECK_LAUNCH();
     const KdIndex ix = make_index(ctx);
-    launch_search(ctx, ix, ctx->queries.as<float4>(), nq, n, 0, 1, ctx->tmp[6].as<float>(), nullptr, ctx->nn_prev.as<int>(), true,
-                  out_normals != nullptr, 0);
+    const KdPlan plan = plan_kd_iteration(ctx, n, 1);
+    launch_search(ctx, plan, ix, ctx->queries.as<float4>(), nq, 0, 1, ctx->tmp[6].as<float>(), nullptr, ctx->nn_prev.as<int>(),
+                  true, out_normals != nullptr, 0);
     record_search(ctx->kd, false, false, out_normals != nullptr, n);
     kd_search_export_kernel<<<grid_for(n, 256, 8 * kNumSMs), 256, 0, st>>>(ix, ctx->nn_prev.as<int>(), n, (float*)onb.dev,
                                                                             (float*)onr.dev, (long long*)oix.dev);

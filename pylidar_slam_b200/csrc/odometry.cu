@@ -370,48 +370,68 @@ void frame_begin(pls_context* ctx, const float* T0_dev) {
     PLS_CHECK_LAUNCH();
 }
 
-// ICP iterations a frame enqueues before its first look at the done flag: the previous frame's count + 1.
-int upfront_iterations(const pls_context* ctx) {
-    const int max_it = ctx->cfg.max_num_alignments;
-    static const bool all_upfront = getenv("PLS_ICP_UPFRONT_ALL") != nullptr;
-    const int upfront = (ctx->last_icp_iters > 0 && !all_upfront) ? ctx->last_icp_iters + 1 : max_it;
-    return upfront > max_it ? max_it : upfront;
+// The ICP rounds (icp_odometry.py:248-299) of the frames of ctxs[0, num), after their frame_begin.  Iterations are
+// enqueued without host syncs and turn into no-ops once a frame's device-side `done` flag latches.  To avoid paying for
+// max_num_alignments launches when ICP converges in 2-3, only the previous frame's count + 1 are enqueued up front (the
+// most any of the frames asks for); while a frame has not latched `done` and may iterate further, up to 4 more follow
+// each host look at the flags (rare: one extra sync per round).
+// enqueue(first, last) enqueues iterations [first, last) of every frame; read_done(done) waits for the enqueued work and
+// stores each frame's done flag.  Returns the number of extra rounds.
+template <typename Enqueue, typename ReadDone>
+int icp_rounds(pls_context* const* ctxs, int num, Enqueue enqueue, ReadDone read_done) {
+    int upfront = 0, max_it = 0;
+    for (int j = 0; j < num; ++j) {
+        const int last = ctxs[j]->last_icp_iters, m = ctxs[j]->cfg.max_num_alignments;
+        const int u = last > 0 && last + 1 < m ? last + 1 : m;
+        upfront = u > upfront ? u : upfront;
+        max_it = m > max_it ? m : max_it;
+    }
+    enqueue(0, upfront);
+    int enq = upfront, extra = 0;
+    int done[PLS_MAX_SEQUENCES];
+    while (enq < max_it) {
+        read_done(done);
+        bool more = false;
+        for (int j = 0; j < num; ++j) more = more || (!done[j] && enq < ctxs[j]->cfg.max_num_alignments);
+        if (!more) break;
+        const int k = (max_it - enq) < 4 ? (max_it - enq) : 4;
+        enqueue(enq, enq + k);
+        enq += k;
+        extra += 1;
+    }
+    return extra;
 }
 
-// The ICP loop (icp_odometry.py:248-299) over ctx->query_ptr / counts[1], after frame_begin: iterations are enqueued
-// without host syncs and turn into no-ops once the device-side `done` flag latches.  To avoid paying for
-// max_num_alignments launches when ICP converges in 2-3, only `previous frame's count + 1` iterations are
-// enqueued up front; the rare frame that needs more continues after the result fetch (same arithmetic,
-// one extra sync).  Returns the block count of the correspondence kernel.
+// The ICP loop of one frame over ctx->query_ptr / counts[1], on ctx->stream.  Returns the block count of the
+// correspondence kernel.
 int run_icp(pls_context* ctx, int64_t query_bound) {
     cudaStream_t st = ctx->stream;
     FrameResult* fr = frame_result_dev(ctx);
     if (query_bound < 1) query_bound = 1;
     ctx->pm.zbuf_clean = false;  // tmp[3] may have been used by the frame's own projection
-    ctx->nn_prev.reserve((size_t)query_bound * sizeof(int), st);  // previous matches: ignored by iteration 0
-    const int max_it = ctx->cfg.max_num_alignments;
-    const int upfront = upfront_iterations(ctx);
-    int blocks = enqueue_icp_iterations(ctx, query_bound, 0, upfront);
-    int enq = upfront;
-    g_trace.lap(0);
-    while (enq < max_it) {
-        // continue only if the device has not latched `done` (checked on the host: rare path)
-        int flags[3];
+    int blocks = 0;
+    auto enqueue = [&](int first, int last) {
+        blocks = enqueue_icp_iterations(ctx, query_bound, first, last);
+        if (first == 0) g_trace.lap(0);
+    };
+    auto read_done = [&](int* done) {
+        int flags[3];  // iters, status, done
         PLS_CUDA(cudaMemcpyAsync(flags, &fr->iters, sizeof(flags), cudaMemcpyDeviceToHost, st));
         PLS_CUDA(cudaStreamSynchronize(st));
-        if (flags[2] /*done*/) break;
-        g_trace.extra_rounds += 1;
-        const int more = (max_it - enq) < 4 ? (max_it - enq) : 4;
-        blocks = enqueue_icp_iterations(ctx, query_bound, enq, enq + more);
-        enq += more;
-    }
+        done[0] = flags[2];
+    };
+    g_trace.extra_rounds += icp_rounds(&ctx, 1, enqueue, read_done);
     return blocks;
 }
 
-void fetch_result(pls_context* ctx) {
-    // the FrameResult and the u32 / u64 scalar slots behind it in one copy
+// The FrameResult and the u32 / u64 scalar slots behind it in one copy to the pinned host mirror, on st.
+void enqueue_result_copy(pls_context* ctx, cudaStream_t st) {
     PLS_CUDA(cudaMemcpyAsync(ctx->pinned.p, ctx->scalars.p, kScalarOffset + SC_NUM * sizeof(uint32_t), cudaMemcpyDeviceToHost,
-                             ctx->stream));
+                             st));
+}
+
+void fetch_result(pls_context* ctx) {
+    enqueue_result_copy(ctx, ctx->stream);
     PLS_CUDA(cudaStreamSynchronize(ctx->stream));
 }
 
@@ -503,7 +523,44 @@ struct FrameOut {
     float* params;
     int* has_pose;
     double* info;
+    int64_t samples;  // >= 0: the frame's rows are a grid sample of this many points, reported as info[4]
+    void put_samples() const {
+        if (info && samples >= 0) info[4] = (double)samples;
+    }
 };
+
+// Why ctx cannot run a frame of `layout` (without its residency hint) and n rows, grid-sampled at `voxel` if voxel > 0;
+// null if it can.  layout < 0: no frame this call (a skipped sequence of a batch), only the context is checked.
+const char* frame_refusal(const pls_context* ctx, int layout, int64_t n, double voxel) {
+    if (ctx->cfg.gn_max_iters != 1) return "fused ICP path supports gauss_newton_config.max_iters == 1";
+    if (layout < 0) return nullptr;
+    if (layout < PLS_INPUT_NDARRAY || layout > PLS_INPUT_TENSOR_F64) return "process_frame: unknown layout";
+    if (voxel > 0.0 && layout != PLS_INPUT_NDARRAY && layout != PLS_INPUT_TENSOR) return "grid-sampled input is a point layout";
+    if (layout != PLS_INPUT_VERTEX_MAP && n <= 0) return "process_frame: empty point cloud";
+    return nullptr;
+}
+
+// A frame's input on the device.  *layout may carry a residency hint in its high bits: the caller knows where `data`
+// lives (a device-resident grid-sample result handed over by pls_grid_sample_staged, a CUDA tensor, a numpy array) and
+// saves the classification; host data is copied through ctx->stage_in[0].  Leaves the bare layout in *layout.
+const void* stage_frame_input(pls_context* ctx, const void* data, int* layout, int64_t n) {
+    const int hint = *layout & (PLS_PTR_DEVICE | PLS_PTR_HOST);
+    *layout &= ~(PLS_PTR_DEVICE | PLS_PTR_HOST);
+    const bool is64 = *layout == PLS_INPUT_NDARRAY_F64 || *layout == PLS_INPUT_TENSOR_F64;
+    const size_t bytes = *layout == PLS_INPUT_VERTEX_MAP ? (size_t)3 * ctx->cfg.height * ctx->cfg.width * sizeof(float)
+                                                         : (size_t)n * 3 * (is64 ? sizeof(double) : sizeof(float));
+    if (hint == PLS_PTR_DEVICE) return data;
+    if (hint != PLS_PTR_HOST) return to_device(ctx, data, bytes, ctx->stage_in[0]);
+    ctx->stage_in[0].reserve(bytes, ctx->stream);
+    PLS_CUDA(cudaMemcpyAsync(ctx->stage_in[0].p, data, bytes, cudaMemcpyHostToDevice, ctx->stream));
+    return ctx->stage_in[0].p;
+}
+
+// The grid sample of a frame's raw float32 rows into ctx->gs_out_xyz, which then holds the frame's input.
+GridSample frame_grid_sample(pls_context* ctx, const void* raw, int64_t n, double voxel) {
+    ctx->gs_out_xyz.reserve((size_t)n * 3 * sizeof(float), ctx->stream);
+    return GridSample{raw, false, n, voxel, ctx->gs_out_xyz.p, nullptr, nullptr, nullptr};
+}
 
 // The input stage of a frame (icp_odometry.py:319-358, 301-308): input selection, the map-update flush and
 // frame_begin_kernel, on ctx->stream.  A sequence's first frame only initialises the map (icp_odometry.py:171-181): that
@@ -612,6 +669,7 @@ bool frame_input(pls_context* ctx, const void* data_void, int layout, int64_t n,
             out.info[3] = (double)ctx->kd.count;
             out.info[5] = (double)(pts_bound - (int64_t)h->counts[2]);
         }
+        out.put_samples();
         return false;
     }
 
@@ -663,8 +721,6 @@ void frame_epilogue(pls_context* ctx, const FrameIn& in, const FrameOut& out, bo
     memcpy(ctx->upd_T, h->T, sizeof(ctx->upd_T));
     ctx->upd_slot = ctx->frame_slot;
     ctx->upd_count = (long long)h->counts[2];
-    static const bool eager = getenv("PLS_MAP_UPDATE_EAGER") != nullptr;  // A/B: enqueue before returning, as before
-    if (eager) flush_map_update(ctx);
     if (trace) g_trace.lap(2);
     ctx->frame_index += 1;
     if (out.pose) memcpy(out.pose, h->T, 16 * sizeof(float));
@@ -682,12 +738,12 @@ void frame_epilogue(pls_context* ctx, const FrameIn& in, const FrameOut& out, bo
         out.info[8] = h->first_pt[0]; out.info[9] = h->first_pt[1]; out.info[10] = h->first_pt[2];
         out.info[11] = ctx->last_sharded ? 1.0 : 0.0;  // the correspondences were split over the ranks
     }
+    out.put_samples();
 }
 
 void process_frame_device(pls_context* ctx, const void* data_void, int layout, int64_t n, const float* init_pose,
-                          float* out_pose, float* out_params, int* out_has_pose, double* out_info) {
+                          const FrameOut& out) {
     g_trace.start();
-    const FrameOut out{out_pose, out_params, out_has_pose, out_info};
     FrameIn in;
     if (!frame_input(ctx, data_void, layout, n, init_pose, in, out)) return;
     const int icp_blocks = run_icp(ctx, in.query_bound);
@@ -786,26 +842,10 @@ int pls_process_frame(pls_context* ctx, const void* data, int layout, int64_t n,
                       float* out_pose, float* out_params, int* out_has_pose, double* out_info) {
     PLS_API_BEGIN(ctx)  // (enqueues the last frame's map update first, unless this frame's grid-sample call already did)
     PLS_REQUIRE(data, "pls_process_frame: null data");
-    // optional residency hint in the high bits: the caller knows where `data` lives (a device-resident grid-sample
-    // result handed over by pls_grid_sample_staged, a CUDA tensor, a numpy array) and saves the classification
-    const int hint = layout & (PLS_PTR_DEVICE | PLS_PTR_HOST);
-    layout &= ~(PLS_PTR_DEVICE | PLS_PTR_HOST);
-    PLS_REQUIRE(layout >= PLS_INPUT_NDARRAY && layout <= PLS_INPUT_TENSOR_F64, "pls_process_frame: unknown layout");
-    PLS_REQUIRE(ctx->cfg.gn_max_iters == 1, "fused ICP path supports gauss_newton_config.max_iters == 1");
-    const bool is64 = layout == PLS_INPUT_NDARRAY_F64 || layout == PLS_INPUT_TENSOR_F64;
-    const size_t bytes = layout == PLS_INPUT_VERTEX_MAP ? (size_t)3 * ctx->cfg.height * ctx->cfg.width * sizeof(float)
-                                                        : (size_t)n * 3 * (is64 ? sizeof(double) : sizeof(float));
-    const void* d = data;
-    if (hint != PLS_PTR_DEVICE) {
-        if (hint == PLS_PTR_HOST) {
-            ctx->stage_in[0].reserve(bytes, ctx->stream);
-            PLS_CUDA(cudaMemcpyAsync(ctx->stage_in[0].p, data, bytes, cudaMemcpyHostToDevice, ctx->stream));
-            d = ctx->stage_in[0].p;
-        } else {
-            d = to_device(ctx, data, bytes, ctx->stage_in[0]);
-        }
-    }
-    process_frame_device(ctx, d, layout, n, init_pose, out_pose, out_params, out_has_pose, out_info);
+    if (const char* why = frame_refusal(ctx, layout & ~(PLS_PTR_DEVICE | PLS_PTR_HOST), n, 0.0))
+        throw pls::Error{PLS_E_INVALID, why};
+    const void* d = stage_frame_input(ctx, data, &layout, n);
+    process_frame_device(ctx, d, layout, n, init_pose, FrameOut{out_pose, out_params, out_has_pose, out_info, -1});
     PLS_API_END(ctx)
 }
 
@@ -816,22 +856,14 @@ int pls_process_frame_grid_sample(pls_context* ctx, const float* raw_points, int
     // otherwise wait for an index build that started a subsample's worth of launches later)
     PLS_API_BEGIN(ctx)
     PLS_REQUIRE(raw_points && n > 0 && voxel > 0.0, "pls_process_frame_grid_sample: bad arguments");
-    PLS_REQUIRE(layout == PLS_INPUT_NDARRAY || layout == PLS_INPUT_TENSOR, "grid-sampled input is a point layout");
-    PLS_REQUIRE(ctx->cfg.gn_max_iters == 1, "fused ICP path supports gauss_newton_config.max_iters == 1");
-    const float* d = (const float*)to_device(ctx, raw_points, (size_t)n * 3 * sizeof(float), ctx->stage_in[0]);
-    ctx->gs_out_xyz.reserve((size_t)n * 3 * sizeof(float), ctx->stream);
-    // the sample count is needed on the host to size the point-layout frame: one small sync (it also carries the
-    // overflow stamp of the 40-bit sort keys; a frame whose hashes exceed them is re-sampled on the raw keys)
-    uint32_t S = 0;
-    for (int attempt = 0; attempt < 2; ++attempt) {
-        grid_sample_device<float>(ctx, d, n, voxel, ctx->gs_out_xyz.as<float>(), nullptr, attempt == 0);
-        bool overflowed = false;
-        S = grid_sample_read_count(ctx, &overflowed);
-        if (!(attempt == 0 && overflowed)) break;
-    }
-    process_frame_device(ctx, ctx->gs_out_xyz.as<float>(), layout, (int64_t)S, init_pose, out_pose, out_params,
-                         out_has_pose, out_info);
-    if (out_info) out_info[4] = (double)S;
+    if (const char* why = frame_refusal(ctx, layout, n, voxel)) throw pls::Error{PLS_E_INVALID, why};
+    const void* d = to_device(ctx, raw_points, (size_t)n * 3 * sizeof(float), ctx->stage_in[0]);
+    // the sample count is needed on the host to size the point-layout frame: one small sync
+    const GridSample g = frame_grid_sample(ctx, d, n, voxel);
+    grid_sample_enqueue(ctx, g);
+    PLS_CUDA(cudaStreamSynchronize(ctx->stream));
+    const int64_t S = grid_sample_finish(ctx, g);
+    process_frame_device(ctx, ctx->gs_out_xyz.p, layout, S, init_pose, FrameOut{out_pose, out_params, out_has_pose, out_info, S});
     PLS_API_END(ctx)
 }
 
@@ -846,16 +878,11 @@ int pls_process_frames(pls_context* const* ctxs, int num, const void* const* dat
         const pls_context* c = ctxs[i];
         if (!c) { why = "pls_process_frames: null context"; break; }
         if (c->cfg.local_map_type != PLS_MAP_KDTREE) why = "pls_process_frames: batched sequences need a kd-tree local map";
-        else if (c->cfg.gn_max_iters != 1) why = "fused ICP path supports gauss_newton_config.max_iters == 1";
         else if (c->comm) why = "pls_process_frames: a context with a multi-GPU communicator cannot be batched";
         else if (c->cfg.device != ctxs[0]->cfg.device) why = "pls_process_frames: every context must be on one device";
         for (int j = 0; !why && j < i; ++j)
             if (ctxs[j] == c) why = "pls_process_frames: a context is listed twice";
-        if (why || !data[i]) continue;
-        const int lay = layouts[i] & ~(PLS_PTR_DEVICE | PLS_PTR_HOST);
-        if (lay < PLS_INPUT_NDARRAY || lay > PLS_INPUT_TENSOR_F64) why = "pls_process_frames: unknown layout";
-        else if (voxel > 0.0 && lay != PLS_INPUT_NDARRAY && lay != PLS_INPUT_TENSOR) why = "grid-sampled input is a point layout";
-        else if (lay != PLS_INPUT_VERTEX_MAP && n[i] <= 0) why = "process_frame: empty point cloud";
+        if (!why) why = frame_refusal(c, data[i] ? layouts[i] & ~(PLS_PTR_DEVICE | PLS_PTR_HOST) : -1, n[i], voxel);
     }
     if (why) {
         for (int i = 0; ctxs && i < num; ++i)
@@ -903,28 +930,16 @@ int pls_process_frames(pls_context* const* ctxs, int num, const void* const* dat
         // voxel > 0, the grid sample, whose counts are read back together
         std::vector<const void*> dev((size_t)num, nullptr);
         std::vector<int64_t> rows(n, n + num);
-        std::vector<int> lay((size_t)num);
+        std::vector<int> lay(layouts, layouts + num);
+        std::vector<GridSample> gs((size_t)num);
         for (int i : active) {
             cur = i;
             pls_context* ctx = ctxs[i];
             flush_map_update(ctx);
-            const int hint = layouts[i] & (PLS_PTR_DEVICE | PLS_PTR_HOST);
-            lay[i] = layouts[i] & ~(PLS_PTR_DEVICE | PLS_PTR_HOST);
-            const bool is64 = lay[i] == PLS_INPUT_NDARRAY_F64 || lay[i] == PLS_INPUT_TENSOR_F64;
-            const size_t bytes = lay[i] == PLS_INPUT_VERTEX_MAP ? (size_t)3 * ctx->cfg.height * ctx->cfg.width * sizeof(float)
-                                                                : (size_t)n[i] * 3 * (is64 ? sizeof(double) : sizeof(float));
-            dev[i] = data[i];
-            if (hint == PLS_PTR_HOST) {
-                ctx->stage_in[0].reserve(bytes, ctx->stream);
-                PLS_CUDA(cudaMemcpyAsync(ctx->stage_in[0].p, data[i], bytes, cudaMemcpyHostToDevice, ctx->stream));
-                dev[i] = ctx->stage_in[0].p;
-            } else if (hint != PLS_PTR_DEVICE) {
-                dev[i] = to_device(ctx, data[i], bytes, ctx->stage_in[0]);
-            }
+            dev[i] = stage_frame_input(ctx, data[i], &lay[i], n[i]);
             if (voxel > 0.0) {
-                ctx->gs_out_xyz.reserve((size_t)n[i] * 3 * sizeof(float), ctx->stream);
-                grid_sample_device<float>(ctx, (const float*)dev[i], n[i], voxel, ctx->gs_out_xyz.as<float>(), nullptr, true);
-                grid_sample_count_to_host(ctx);
+                gs[i] = frame_grid_sample(ctx, dev[i], n[i], voxel);
+                grid_sample_enqueue(ctx, gs[i]);
                 order_before_lead(ctx);
             }
         }
@@ -932,15 +947,8 @@ int pls_process_frames(pls_context* const* ctxs, int num, const void* const* dat
             PLS_CUDA(cudaStreamSynchronize(st));
             for (int i : active) {
                 cur = i;
-                pls_context* ctx = ctxs[i];
-                bool overflowed = false;
-                uint32_t S = grid_sample_host_count(ctx, &overflowed);
-                if (overflowed) {  // hashes beyond the 40-bit keys: once more on the raw 64-bit keys
-                    grid_sample_device<float>(ctx, (const float*)dev[i], n[i], voxel, ctx->gs_out_xyz.as<float>(), nullptr, false);
-                    S = grid_sample_read_count(ctx, &overflowed);
-                }
-                dev[i] = ctx->gs_out_xyz.p;
-                rows[i] = (int64_t)S;
+                rows[i] = grid_sample_finish(ctxs[i], gs[i]);
+                dev[i] = ctxs[i]->gs_out_xyz.p;
             }
         }
         std::vector<FrameIn> in((size_t)num);
@@ -949,7 +957,8 @@ int pls_process_frames(pls_context* const* ctxs, int num, const void* const* dat
         std::vector<int64_t> bounds;
         auto outputs = [&](int i) {
             return FrameOut{out_poses ? out_poses + 16 * i : nullptr, out_params ? out_params + 6 * i : nullptr,
-                            out_has_pose ? out_has_pose + i : nullptr, out_info ? out_info + 12 * i : nullptr};
+                            out_has_pose ? out_has_pose + i : nullptr, out_info ? out_info + 12 * i : nullptr,
+                            voxel > 0.0 ? rows[i] : -1};
         };
         for (int i : active) {
             cur = i;
@@ -966,7 +975,6 @@ int pls_process_frames(pls_context* const* ctxs, int num, const void* const* dat
                 continue;
             }
             if (!runs_icp) {
-                if (voxel > 0.0 && out_info) out_info[12 * i + 4] = (double)rows[i];
                 finished[i] = 1;
                 continue;
             }
@@ -983,29 +991,12 @@ int pls_process_frames(pls_context* const* ctxs, int num, const void* const* dat
             cur = icp_seq[0];
             int grid[3];
             kdmap_batch_begin(lead, icp.data(), bounds.data(), m, st, grid);
-            int upfront = 0, max_it = 0;
-            for (pls_context* ctx : icp) {
-                const int u = upfront_iterations(ctx);
-                upfront = u > upfront ? u : upfront;
-                max_it = ctx->cfg.max_num_alignments > max_it ? ctx->cfg.max_num_alignments : max_it;
-            }
-            kdmap_batch_iterations(lead, icp.data(), bounds.data(), m, st, grid, 0, upfront);
-            int enq = upfront;
-            std::vector<int> done((size_t)m);
-            while (enq < max_it) {
-                // continue only for a sequence whose device has not latched `done` (the rare path, as on a single one)
-                kdmap_batch_done(lead, m, st, done.data());
-                bool more = false;
-                for (int j = 0; j < m; ++j) more = more || (!done[j] && enq < icp[j]->cfg.max_num_alignments);
-                if (!more) break;
-                const int k = (max_it - enq) < 4 ? (max_it - enq) : 4;
-                kdmap_batch_iterations(lead, icp.data(), bounds.data(), m, st, grid, enq, enq + k);
-                enq += k;
-                trace.extra_rounds += 1;
-            }
-            for (pls_context* ctx : icp)  // each FrameResult and the scalar slots behind it
-                PLS_CUDA(cudaMemcpyAsync(ctx->pinned.p, ctx->scalars.p, kScalarOffset + SC_NUM * sizeof(uint32_t),
-                                         cudaMemcpyDeviceToHost, st));
+            auto enqueue = [&](int first, int last) {
+                kdmap_batch_iterations(lead, icp.data(), bounds.data(), m, st, grid, first, last);
+            };
+            auto read_done = [&](int* done) { kdmap_batch_done(lead, m, st, done); };
+            trace.extra_rounds += icp_rounds(icp.data(), m, enqueue, read_done);
+            for (pls_context* ctx : icp) enqueue_result_copy(ctx, st);
             trace.icp_done(st);
             PLS_CUDA(cudaStreamSynchronize(st));
         }
@@ -1016,7 +1007,6 @@ int pls_process_frames(pls_context* const* ctxs, int num, const void* const* dat
             cur = i;
             try {
                 frame_epilogue(icp[j], in[i], outputs(i), false);
-                if (voxel > 0.0 && out_info) out_info[12 * i + 4] = (double)rows[i];
             } catch (const pls::Error& e) {
                 if (e.code != PLS_E_SINGULAR) throw;
                 icp[j]->err = e.msg;

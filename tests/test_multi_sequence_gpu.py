@@ -132,6 +132,7 @@ class Pair:
         lib = self.lib
         inits = inits or [self.prev[i] for i in range(self.B)]
         rc, status, outs = batch(lib, self.bat, frames, self.voxel, inits)
+        self.outs = outs
         first_bad = next((int(s) for s in status if s != lib.PLS_OK), lib.PLS_OK)
         assert rc == first_bad, (tag, rc, status)
         for i, f in enumerate(frames):
@@ -179,6 +180,29 @@ def test_grid_sampled_sequences(lib):
     pair = Pair(lib, 5, voxel=VOXEL)
     for k in range(30):
         pair.step([Frame(lib, kinds[i], scan(200 * i + k)) for i in range(5)], tag=k)
+    pair.finish()
+
+
+def test_grid_sampled_sequence_beyond_the_compact_sort_keys(lib):
+    """Sequence 2's scans are shifted by 5e5 m: its voxel hashes exceed the 40-bit sort keys, and the batched call samples
+    it once more on the raw 64-bit keys, as pls_process_frame_grid_sample does.  Its frame 0 lies outside the vertical
+    field of view, so its kd map is filled from that scan before the ICP frames."""
+    from oracle import icp_oracle as orc
+    import pylidar_slam_b200 as b200
+    pair = Pair(lib, 3, voxel=VOXEL)
+    eye = np.eye(4, dtype=np.float32)
+    for k in range(6):
+        far = np.ascontiguousarray(scan(400 + k) + np.float32(5.0e5))
+        assert np.abs(orc.voxel_hashes(orc.voxel_coords(far, VOXEL))).max() >= 2 ** 39
+        pair.step([Frame(lib, "tensor", scan(k)), Frame(lib, "ndarray", scan(200 + k)), Frame(lib, "ndarray", far)], tag=k)
+        if pair.statuses[2][-1] == lib.PLS_OK:
+            assert int(pair.outs[2]["info"][4]) == orc.grid_sample(far, VOXEL)[1].shape[0], k
+        if k == 0:
+            fill = np.ascontiguousarray(b200.grid_sample(far, VOXEL)[0])
+            for c in (pair.bat[2], pair.ind[2]):
+                c.call("pls_kdmap_update_points", lib.ptr(eye), lib.ptr(fill), fill.shape[0])
+    assert pair.statuses[2][0] == lib.PLS_OK and pair.iters[2][0] == 0, pair.statuses[2]
+    assert sum(it > 0 for it in pair.iters[2][1:]) >= 2, (pair.iters[2], pair.statuses[2])
     pair.finish()
 
 
