@@ -268,6 +268,12 @@ enum { PLS_MAX_SEQUENCES = 64 };
 PLS_API int pls_process_frames(pls_context* const* ctxs, int num, const void* const* data, const int* layouts,
                                const int64_t* n, double voxel, const float* const* init_poses, float* out_poses,
                                float* out_params, int* out_has_pose, double* out_info, int* out_status);
+/* Test / debug aid: out_sums [30] = the accumulators of the last executed ICP iteration of the last frame of
+ * pls_register_frame, pls_process_frame(_grid_sample) or pls_process_frames on this context, for either map type (the
+ * order of pls_kdmap_last_correspondences: 21 JtJ upper, 6 Jtr, sum (w r)^2, sum r^2, count); *out_iters (nullable) =
+ * that frame's executed iterations.  Reads the host copy of the frame's result: no kernel, no synchronisation, a
+ * pending map update is not flushed.  PLS_E_STATE before the context's first ICP frame. */
+PLS_API int pls_last_icp_sums(pls_context* ctx, double* out_sums, int* out_iters);
 
 /* ---- the rows either side of the path (SURVEY.md section 8f, ranks 1-2) -----------------------------------
  * Distortion.filter (slam/preprocessing.py:148-191): de-skew of a frame with the estimated relative motion.

@@ -78,6 +78,7 @@ _SIGNATURES = {
     "pls_process_frame": [_P, _P, _I, _L, _P, _P, _P, C.POINTER(_I), _P],
     "pls_process_frame_grid_sample": [_P, _P, _L, _D, _I, _P, _P, _P, C.POINTER(_I), _P],
     "pls_process_frames": [_P, _I, _P, _P, _P, _D, _P, _P, _P, _P, _P, _P],
+    "pls_last_icp_sums": [_P, _P, C.POINTER(_I)],
     "pls_comm_init": [_P, _I, _I, _P, C.c_char_p],
     "pls_comm_unique_id": [C.c_char_p, _P],
     "pls_comm_p2p_handle": [_P, _I, _P],

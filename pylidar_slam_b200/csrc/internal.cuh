@@ -195,6 +195,7 @@ struct pls_context {
     pls::ProjMap pm;
     int frame_index = 0;
     int last_icp_iters = 0;             // iterations the previous frame's ICP executed (sizes the up-front enqueue)
+    bool icp_result = false;            // the host FrameResult holds an ICP frame's result (pls_last_icp_sums)
     bool last_sharded = false;          // the last ICP actually split its correspondences over the ranks
     int sample_pointcloud = 0;          // _sample_pointcloud
     float delta_since_update[16];       // _delta_since_map_update

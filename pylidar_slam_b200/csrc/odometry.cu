@@ -748,6 +748,7 @@ void process_frame_device(pls_context* ctx, const void* data_void, int layout, i
     if (!frame_input(ctx, data_void, layout, n, init_pose, in, out)) return;
     const int icp_blocks = run_icp(ctx, in.query_bound);
     fetch_result(ctx);
+    ctx->icp_result = true;
     g_trace.lap(1);
     credit_icp_profile(ctx, frame_result_host(ctx), icp_blocks);
     frame_epilogue(ctx, in, out, true);
@@ -823,6 +824,7 @@ int pls_register_frame(pls_context* ctx, const float* points, int64_t n, const f
     frame_begin(ctx, T0_dev);
     const int icp_blocks = run_icp(ctx, n);
     fetch_result(ctx);
+    ctx->icp_result = true;
     FrameResult* h = frame_result_host(ctx);
     credit_icp_profile(ctx, h, icp_blocks);
     auto put = [&](void* dst, const void* src, size_t bytes) {
@@ -864,6 +866,18 @@ int pls_process_frame_grid_sample(pls_context* ctx, const float* raw_points, int
     PLS_CUDA(cudaStreamSynchronize(ctx->stream));
     const int64_t S = grid_sample_finish(ctx, g);
     process_frame_device(ctx, ctx->gs_out_xyz.p, layout, S, init_pose, FrameOut{out_pose, out_params, out_has_pose, out_info, S});
+    PLS_API_END(ctx)
+}
+
+// A read-only look at the host copy of the last ICP frame's result.  PLS_API_BEGIN_FRAME: a pending map update stays
+// pending.
+int pls_last_icp_sums(pls_context* ctx, double* out_sums, int* out_iters) {
+    PLS_API_BEGIN_FRAME(ctx)
+    PLS_REQUIRE(out_sums, "pls_last_icp_sums: null output");
+    if (!ctx->icp_result) throw pls::Error{PLS_E_STATE, "pls_last_icp_sums: no ICP frame has run on this context"};
+    const FrameResult* h = frame_result_host(ctx);
+    memcpy(out_sums, h->last_sums, NACC * sizeof(double));
+    if (out_iters) *out_iters = h->iters;
     PLS_API_END(ctx)
 }
 
@@ -999,6 +1013,7 @@ int pls_process_frames(pls_context* const* ctxs, int num, const void* const* dat
             for (pls_context* ctx : icp) enqueue_result_copy(ctx, st);
             trace.icp_done(st);
             PLS_CUDA(cudaStreamSynchronize(st));
+            for (pls_context* ctx : icp) ctx->icp_result = true;
         }
         trace.epilogue_begin();
         // ---- epilogue, per sequence: a failed ICP is that sequence's error alone
