@@ -252,8 +252,10 @@ PLS_API int pls_process_frame_grid_sample(pls_context* ctx, const float* raw_poi
                                   float* out_params, int* out_has_pose, double* out_info);
 
 /* Several independent sequences, one frame each, in one call (no reference counterpart: the reference's runner
- * processes sequences one after another, odometry_runner.py:145-175).  ctxs [num] distinct kd-map contexts on one
- * device; data / layouts / n / init_poses [num] as pls_process_frame (data[i] == NULL: sequence i skipped);
+ * processes sequences one after another, odometry_runner.py:145-175).  ctxs [num] distinct contexts on one device,
+ * all with kd-tree local maps or all with projective ones (a mixed call is refused); their other settings (frame size,
+ * local_map_size, scheme, ...) may differ.  data / layouts / n / init_poses [num] as pls_process_frame (data[i] == NULL:
+ * sequence i skipped);
  * voxel > 0 grid-samples every sequence first, as pls_process_frame_grid_sample; outputs [num,16] / [num,6] / [num] /
  * [num,12] / [num], each nullable.  num <= PLS_MAX_SEQUENCES.
  * Every context ends in the state its own pls_process_frame (pls_process_frame_grid_sample) call would have left, with

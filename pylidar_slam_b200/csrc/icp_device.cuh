@@ -119,6 +119,23 @@ __device__ __forceinline__ void icp_solve_and_update(FrameResult* fr, const doub
     PLS_SPLIT(8, prm[5] + fr->T[10]);
 }
 
+// K7: normal-equation solve + ICP bookkeeping of one frame, by one 256-thread block: icp_step_kernel (odometry.cu) and,
+// one block per sequence, icp_step_batch_kernel (projmap.cu).  num_blocks == 0: `reduced` holds the (all-reduced) sums.
+__device__ __forceinline__ void icp_step_body(FrameResult* fr, const double* __restrict__ partials, int num_blocks,
+                                              const double* __restrict__ reduced, float threshold_delta) {
+    if (fr->done) return;
+    __shared__ double sums[NACC];
+    if (num_blocks > 0) {
+        sum_partials_256(partials, num_blocks, sums);
+    } else if (threadIdx.x < NACC) {
+        sums[threadIdx.x] = reduced[threadIdx.x];
+    }
+    __syncthreads();
+    if (threadIdx.x < NACC) fr->last_sums[threadIdx.x] = sums[threadIdx.x];
+    if (threadIdx.x != 0) return;
+    icp_solve_and_update(fr, sums, threshold_delta);
+}
+
 // Called by every block of a correspondence kernel (512, 256 or 128 threads) after it stored its partial row: the block
 // that arrives last of the num_blocks (ticket in fr->pad) sums all rows in the fixed order and runs the solve -- one
 // launch and one dependent-launch gap less per ICP iteration than a separate step kernel.

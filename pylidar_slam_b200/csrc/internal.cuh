@@ -417,6 +417,14 @@ void grid_sample_enqueue(pls_context* ctx, const GridSample& g);
 uint32_t grid_sample_finish(pls_context* ctx, const GridSample& g);
 // projmap.cu
 void projmap_reset(pls_context* ctx);
+// pls_process_frames on projective maps, the counterparts of kdmap_batch_*: begin uploads the descriptors into
+// lead->batch_buf and returns the launch widths and the TMA kernel's dynamic shared memory in grid[4]; iterations
+// enqueues ICP iterations [first, last) of all of them, solve included; done reads every sequence's done flag.
+void projmap_batch_begin(pls_context* lead, pls_context* const* ctxs, const int64_t* query_bounds, int num, cudaStream_t st,
+                         int* grid);
+void projmap_batch_iterations(pls_context* lead, pls_context* const* ctxs, const int64_t* query_bounds, int num, cudaStream_t st,
+                              const int* grid, int first, int last);
+void projmap_batch_done(pls_context* lead, int num, cudaStream_t st, int* out);
 // odometry.cu: would an ICP iteration over `work` items be split across the ranks (the rule of enqueue_icp_iterations)?
 bool icp_shards(pls_context* ctx, int64_t work);
 // comm.cu

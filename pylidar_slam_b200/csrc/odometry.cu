@@ -68,17 +68,7 @@ __global__ void __launch_bounds__(256) reduce_partials_kernel(const FrameResult*
 // K7: normal-equation solve + ICP bookkeeping (256 threads).  num_blocks == 0: `reduced` holds the (all-reduced) sums.
 __global__ void __launch_bounds__(256) icp_step_kernel(FrameResult* fr, const double* __restrict__ partials,
                                                        int num_blocks, const double* __restrict__ reduced, float threshold_delta) {
-    if (fr->done) return;
-    __shared__ double sums[NACC];
-    if (num_blocks > 0) {
-        sum_partials_256(partials, num_blocks, sums);
-    } else if (threadIdx.x < NACC) {
-        sums[threadIdx.x] = reduced[threadIdx.x];
-    }
-    __syncthreads();
-    if (threadIdx.x < NACC) fr->last_sums[threadIdx.x] = sums[threadIdx.x];
-    if (threadIdx.x != 0) return;
-    icp_solve_and_update(fr, sums, threshold_delta);
+    icp_step_body(fr, partials, num_blocks, reduced, threshold_delta);
 }
 
 // K9 fused: block-partial sum + ONE-SHOT all-reduce over NVLink peer memory + solve, in one kernel.
@@ -891,7 +881,8 @@ int pls_process_frames(pls_context* const* ctxs, int num, const void* const* dat
     for (int i = 0; !why && i < num; ++i) {
         const pls_context* c = ctxs[i];
         if (!c) { why = "pls_process_frames: null context"; break; }
-        if (c->cfg.local_map_type != PLS_MAP_KDTREE) why = "pls_process_frames: batched sequences need a kd-tree local map";
+        if (c->cfg.local_map_type != ctxs[0]->cfg.local_map_type)
+            why = "pls_process_frames: batched sequences share one local map type: all kd-tree or all projective";
         else if (c->comm) why = "pls_process_frames: a context with a multi-GPU communicator cannot be batched";
         else if (c->cfg.device != ctxs[0]->cfg.device) why = "pls_process_frames: every context must be on one device";
         for (int j = 0; !why && j < i; ++j)
@@ -1003,12 +994,18 @@ int pls_process_frames(pls_context* const* ctxs, int num, const void* const* dat
         trace.inputs_done(st, (int)active.size(), m);
         if (m > 0) {
             cur = icp_seq[0];
-            int grid[3];
-            kdmap_batch_begin(lead, icp.data(), bounds.data(), m, st, grid);
+            int grid[4];
+            const bool kd = lead->cfg.local_map_type == PLS_MAP_KDTREE;
+            if (kd) kdmap_batch_begin(lead, icp.data(), bounds.data(), m, st, grid);
+            else projmap_batch_begin(lead, icp.data(), bounds.data(), m, st, grid);
             auto enqueue = [&](int first, int last) {
-                kdmap_batch_iterations(lead, icp.data(), bounds.data(), m, st, grid, first, last);
+                if (kd) kdmap_batch_iterations(lead, icp.data(), bounds.data(), m, st, grid, first, last);
+                else projmap_batch_iterations(lead, icp.data(), bounds.data(), m, st, grid, first, last);
             };
-            auto read_done = [&](int* done) { kdmap_batch_done(lead, m, st, done); };
+            auto read_done = [&](int* done) {
+                if (kd) kdmap_batch_done(lead, m, st, done);
+                else projmap_batch_done(lead, m, st, done);
+            };
             trace.extra_rounds += icp_rounds(icp.data(), m, enqueue, read_done);
             for (pls_context* ctx : icp) enqueue_result_copy(ctx, st);
             trace.icp_done(st);

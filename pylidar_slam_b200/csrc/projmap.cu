@@ -16,6 +16,7 @@
 #include <stdlib.h>
 
 #include "gn_device.cuh"
+#include "icp_device.cuh"
 #include "internal.cuh"
 #include "pose_device.cuh"
 #include "projection_device.cuh"
@@ -192,14 +193,19 @@ __device__ __forceinline__ void load_T(const float* __restrict__ T, float* sT) {
     __syncthreads();
 }
 
-__global__ void query_zbuf_kernel(const float4* __restrict__ queries, const uint32_t* __restrict__ nq_dev, int64_t nq_host,
-                                  const float* __restrict__ T, const int* __restrict__ done, ProjConst pc, int pix_lo,
-                                  int pix_hi, unsigned long long* __restrict__ zbuf) {
+// The kernels of an ICP iteration below are __device__ bodies with two entry points each: the kernel of one sequence,
+// which passes blockIdx.x / gridDim.x and its arguments, and the *_batch_kernel of pls_process_frames, whose blockIdx.y
+// picks a sequence's descriptor (ProjSeq) and which passes that sequence's own block count.  A body reads no blockIdx.x
+// or gridDim.x itself, so a sequence's striding, tile assignment and partial rows are those of its single path.
+__device__ __forceinline__ void query_zbuf_body(const float4* __restrict__ queries, const uint32_t* __restrict__ nq_dev,
+                                                int64_t nq_host, const float* __restrict__ T, const int* __restrict__ done,
+                                                ProjConst pc, int pix_lo, int pix_hi, unsigned long long* __restrict__ zbuf,
+                                                unsigned block, unsigned grid) {
     if (done && *done) return;
     __shared__ float sT[12];
     if (T) load_T(T, sT);
     const int64_t nq = nq_dev ? (int64_t)*nq_dev : nq_host;
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < nq; i += (int64_t)gridDim.x * blockDim.x) {
+    for (int64_t i = (int64_t)block * blockDim.x + threadIdx.x; i < nq; i += (int64_t)grid * blockDim.x) {
         const float4 p0 = queries[i];
         float p[3] = {p0.x, p0.y, p0.z};
         if (T) {
@@ -216,14 +222,20 @@ __global__ void query_zbuf_kernel(const float4* __restrict__ queries, const uint
     }
 }
 
+__global__ void query_zbuf_kernel(const float4* __restrict__ queries, const uint32_t* __restrict__ nq_dev, int64_t nq_host,
+                                  const float* __restrict__ T, const int* __restrict__ done, ProjConst pc, int pix_lo,
+                                  int pix_hi, unsigned long long* __restrict__ zbuf) {
+    query_zbuf_body(queries, nq_dev, nq_host, T, done, pc, pix_lo, pix_hi, zbuf, blockIdx.x, gridDim.x);
+}
+
 // z-buffer winners -> the target vertex map of this iteration, float4 (p transformed, valid flag) per pixel
-__global__ void query_resolve_kernel(unsigned long long* __restrict__ zbuf, const float4* __restrict__ queries,
-                                     const float* __restrict__ T, const int* __restrict__ done, int64_t pix_lo,
-                                     int64_t pix_hi, float4* __restrict__ tgt) {
+__device__ __forceinline__ void query_resolve_body(unsigned long long* __restrict__ zbuf, const float4* __restrict__ queries,
+                                                   const float* __restrict__ T, const int* __restrict__ done, int64_t pix_lo,
+                                                   int64_t pix_hi, float4* __restrict__ tgt, unsigned block, unsigned grid) {
     if (done && *done) return;
     __shared__ float sT[12];
     load_T(T, sT);
-    for (int64_t pix = pix_lo + (int64_t)blockIdx.x * blockDim.x + threadIdx.x; pix < pix_hi; pix += (int64_t)gridDim.x * blockDim.x) {
+    for (int64_t pix = pix_lo + (int64_t)block * blockDim.x + threadIdx.x; pix < pix_hi; pix += (int64_t)grid * blockDim.x) {
         const unsigned long long key = zbuf[pix];
         zbuf[pix] = ~0ull;  // leave the z-buffer cleared for the next iteration (no separate memset)
         float4 o = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -236,6 +248,12 @@ __global__ void query_resolve_kernel(unsigned long long* __restrict__ zbuf, cons
         }
         tgt[pix] = o;
     }
+}
+
+__global__ void query_resolve_kernel(unsigned long long* __restrict__ zbuf, const float4* __restrict__ queries,
+                                     const float* __restrict__ T, const int* __restrict__ done, int64_t pix_lo,
+                                     int64_t pix_hi, float4* __restrict__ tgt) {
+    query_resolve_body(zbuf, queries, T, done, pix_lo, pix_hi, tgt, blockIdx.x, gridDim.x);
 }
 
 // Arg-min over distances WITHOUT the square roots in the common case.  The reference takes the arg-min over
@@ -374,11 +392,11 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
         : "memory");
 }
 
-__global__ void __launch_bounds__(PT_TILE)
-proj_icp_tma_kernel(const float* __restrict__ model_v, const float4* __restrict__ model_n, int K, int kcap,
-                    const float4* __restrict__ tgt, const FrameResult* __restrict__ fr, int64_t tile_begin, int64_t tile_end, int scheme, float sigma,
-                    int stages, int ktma, int64_t resident_end, unsigned long long policy_resident,
-                    unsigned long long policy_stream, double* __restrict__ partials) {
+__device__ __forceinline__ void
+proj_icp_tma_body(const float* __restrict__ model_v, const float4* __restrict__ model_n, int K, int kcap,
+                  const float4* __restrict__ tgt, const FrameResult* __restrict__ fr, int64_t tile_begin, int64_t tile_end, int scheme, float sigma,
+                  int stages, int ktma, int64_t resident_end, unsigned long long policy_resident,
+                  unsigned long long policy_stream, double* __restrict__ partials, unsigned block, unsigned grid) {
     if (fr->done) return;
     extern __shared__ __align__(128) unsigned char smem_raw[];
     __shared__ __align__(8) uint64_t full_bar[PT_STAGES];
@@ -396,8 +414,8 @@ proj_icp_tma_kernel(const float* __restrict__ model_v, const float4* __restrict_
     }
     __syncthreads();
 
-    const int64_t first_tile = tile_begin + blockIdx.x;
-    const int64_t stride = gridDim.x;
+    const int64_t first_tile = tile_begin + block;
+    const int64_t stride = grid;
     auto issue = [&](int64_t tile, int s) {  // thread 0 only
         mbar_arrive_expect_tx(&full_bar[s], stage_bytes);
         // the tile's K*3 candidate rows are contiguous in the tile-interleaved layout: one bulk copy; a second
@@ -531,9 +549,89 @@ proj_icp_tma_kernel(const float* __restrict__ model_v, const float4* __restrict_
     double acc64[NACC];
 #pragma unroll
     for (int a = 0; a < NACC; ++a) acc64[a] = (double)acc[a];
-    block_reduce_store<PT_TILE>(acc64, partials + (size_t)blockIdx.x * NACC);
+    block_reduce_store<PT_TILE>(acc64, partials + (size_t)block * NACC);
     // (the solve stays in icp_step_kernel: finishing the iteration in the CTA that arrives last, as kd_residual_kernel
     // does, was slower here)
+}
+
+__global__ void __launch_bounds__(PT_TILE)
+proj_icp_tma_kernel(const float* __restrict__ model_v, const float4* __restrict__ model_n, int K, int kcap,
+                    const float4* __restrict__ tgt, const FrameResult* __restrict__ fr, int64_t tile_begin, int64_t tile_end, int scheme, float sigma,
+                    int stages, int ktma, int64_t resident_end, unsigned long long policy_resident,
+                    unsigned long long policy_stream, double* __restrict__ partials) {
+    proj_icp_tma_body(model_v, model_n, K, kcap, tgt, fr, tile_begin, tile_end, scheme, sigma, stages, ktma, resident_end,
+                      policy_resident, policy_stream, partials, blockIdx.x, gridDim.x);
+}
+
+// ---- several sequences per launch (pls_process_frames) --------------------------------------------------------------
+// What the kernels of one ICP iteration need of one sequence: the arguments its single path passes (one rank: every
+// tile and every pixel), and its share of each launch.  Built on the host by projmap_batch_begin and uploaded once per
+// call.  A sequence that cannot take the TMA path has no blocks in the first three kernels: its correspondences run
+// through its own launches (proj_icp_iter_kernel), and only the step kernel is shared.
+struct ProjSeq {
+    const float* model_v;
+    const float4* model_n;
+    const float4* queries;
+    const uint32_t* nq_dev;     // query count (FrameResult counts[1])
+    FrameResult* fr;            // pose, done flag
+    unsigned long long* zbuf;   // the query z-buffer (tmp[3]), all-empty between iterations
+    float4* tgt;                // the target vertex map of the iteration (tmp[7])
+    double* partials;           // step_blocks rows
+    ProjConst pc;
+    int K, kcap, ktma, stages;
+    int scheme;
+    float sigma;
+    float threshold_delta;
+    int64_t tiles;              // hw / 128: the tile range [0, tiles)
+    int64_t resident_end;       // tiles below it are read evict-last
+    int zbuf_blocks, resolve_blocks, tma_blocks;  // the single path's geometry of each kernel (0: not launched)
+    int step_blocks;            // partial rows the step sums: the TMA kernel's or proj_icp_iter_kernel's blocks
+    int max_iters;              // max_num_alignments: launches of later iterations leave the sequence alone
+};
+static_assert(sizeof(ProjSeq) % sizeof(int) == 0, "ProjSeq is copied in 4-byte words");
+
+// Sequence blockIdx.y's descriptor into shared memory, for every thread of the block.
+__device__ __forceinline__ void load_seq(const ProjSeq* __restrict__ seqs, ProjSeq& s) {
+    const int* src = reinterpret_cast<const int*>(seqs + blockIdx.y);
+    int* dst = reinterpret_cast<int*>(&s);
+    for (int i = threadIdx.x; i < (int)(sizeof(ProjSeq) / sizeof(int)); i += blockDim.x) dst[i] = __ldg(src + i);
+    __syncthreads();
+}
+
+__global__ void query_zbuf_batch_kernel(const ProjSeq* __restrict__ seqs, int it) {
+    __shared__ ProjSeq s;
+    load_seq(seqs, s);
+    if ((int)blockIdx.x >= s.zbuf_blocks || it >= s.max_iters) return;
+    query_zbuf_body(s.queries, s.nq_dev, 0, s.fr->T, &s.fr->done, s.pc, 0, (int)(s.tiles * PT_TILE), s.zbuf, blockIdx.x,
+                    s.zbuf_blocks);
+}
+
+__global__ void query_resolve_batch_kernel(const ProjSeq* __restrict__ seqs, int it) {
+    __shared__ ProjSeq s;
+    load_seq(seqs, s);
+    if ((int)blockIdx.x >= s.resolve_blocks || it >= s.max_iters) return;
+    query_resolve_body(s.zbuf, s.queries, s.fr->T, &s.fr->done, 0, s.tiles * PT_TILE, s.tgt, blockIdx.x, s.resolve_blocks);
+}
+
+__global__ void __launch_bounds__(PT_TILE) proj_icp_tma_batch_kernel(const ProjSeq* __restrict__ seqs, int it) {
+    __shared__ ProjSeq s;
+    load_seq(seqs, s);
+    if ((int)blockIdx.x >= s.tma_blocks || it >= s.max_iters) return;
+    proj_icp_tma_body(s.model_v, s.model_n, s.K, s.kcap, s.tgt, s.fr, 0, s.tiles, s.scheme, s.sigma, s.stages, s.ktma,
+                      s.resident_end, L2_EVICT_LAST, L2_EVICT_FIRST, s.partials, blockIdx.x, s.tma_blocks);
+}
+
+// One block per sequence: the fixed-order sum of its own partial rows, the guards, the solve and the done latch.
+__global__ void __launch_bounds__(256) icp_step_batch_kernel(const ProjSeq* __restrict__ seqs, int it) {
+    __shared__ ProjSeq s;
+    load_seq(seqs, s);
+    if (it >= s.max_iters) return;
+    icp_step_body(s.fr, s.partials, s.step_blocks, nullptr, s.threshold_delta);
+}
+
+// The done flags of every sequence, for the host's extra-round check.
+__global__ void proj_batch_done_kernel(const ProjSeq* __restrict__ seqs, int num, int* __restrict__ out) {
+    for (int i = threadIdx.x; i < num; i += blockDim.x) out[i] = seqs[i].fr->done;
 }
 
 // per-pixel association for the fine-grained API: flag + (q, n, p)
@@ -738,6 +836,73 @@ void projmap_update(pls_context* ctx, const float* rel_pose_host, const float* v
     rebuild_model(ctx);
 }
 
+namespace {
+
+// The launch geometry of one ICP iteration of ctx on rank `rank` of `num_ranks`, shared by projmap_icp_iteration and
+// projmap_batch_begin.
+struct ProjPlan {
+    bool use_tma;
+    int ktma, stages;
+    size_t smem;                  // the TMA kernel's dynamic shared memory
+    int64_t tile_begin, tile_end; // the rank's tiles (TMA path)
+    int64_t need_lo, need_hi;     // the pixels the rank reduces
+    int blocks;                   // partial rows: the TMA kernel's CTAs, or proj_icp_iter_kernel's blocks
+};
+
+// PLS_PROJ_RESIDENT_MB into *mb if it is set; returns whether it is.
+bool resident_mb_env(int* mb) {
+    static const char* e = getenv("PLS_PROJ_RESIDENT_MB");
+    static const int v = e ? atoi(e) : 0;
+    if (e) *mb = v;
+    return e != nullptr;
+}
+
+ProjPlan plan_proj_iteration(const pls_context* ctx, int rank, int num_ranks) {
+    const int64_t hw = (int64_t)ctx->cfg.height * ctx->cfg.width;
+    const int K = ctx->pm.K;
+    ProjPlan p;
+    // split of the K candidates between the TMA path and the direct-load path (at most 10 direct)
+    static const int kdirect_env = getenv("PLS_PROJ_KDIRECT") ? atoi(getenv("PLS_PROJ_KDIRECT")) : 4;
+    int kdirect = kdirect_env < 0 ? 0 : (kdirect_env > 10 ? 10 : kdirect_env);
+    if (kdirect > K - 1) kdirect = K > 1 ? K - 1 : 0;
+    p.ktma = K - kdirect;
+    const size_t stage_bytes = (size_t)(p.ktma * 3 + 4) * PT_TILE * sizeof(float);
+    static const bool no_tma = getenv("PLS_PROJ_NO_TMA") != nullptr;
+    static const int stages = getenv("PLS_PROJ_STAGES") ? atoi(getenv("PLS_PROJ_STAGES")) : 2;
+    p.stages = stages;
+    p.use_tma = !no_tma && hw % PT_TILE == 0 && stages >= 1 && stages <= PT_STAGES && stage_bytes * stages <= 200 * 1024;
+    p.smem = stage_bytes * stages;
+    // the pixels this rank reduces: whole 128-pixel tiles on the TMA path.  Only they take part in the z-buffer of the
+    // transformed queries and in the target map, and only they need the model (a sharded rank builds just its share)
+    const int64_t tiles = hw / PT_TILE;
+    p.tile_begin = tiles * rank / num_ranks;
+    p.tile_end = tiles * (rank + 1) / num_ranks;
+    p.need_lo = p.use_tma ? p.tile_begin * PT_TILE : hw * rank / num_ranks;
+    p.need_hi = p.use_tma ? p.tile_end * PT_TILE : hw * (rank + 1) / num_ranks;
+    if (p.use_tma) {
+        // TMA-staged persistent kernel over 128-pixel tiles; ranks take contiguous tile ranges
+        int per_sm = (int)((220 * 1024) / (p.smem + 2048));
+        per_sm = per_sm < 1 ? 1 : (per_sm > 8 ? 8 : per_sm);
+        // equal tile counts per CTA: ceil(tiles / ceil(tiles / max_ctas)) persistent CTAs
+        const int64_t my_tiles = p.tile_end - p.tile_begin;
+        const int64_t max_ctas = (int64_t)per_sm * kNumSMs;
+        const int64_t per_cta = (my_tiles + max_ctas - 1) / max_ctas;
+        p.blocks = (int)((my_tiles + (per_cta > 0 ? per_cta : 1) - 1) / (per_cta > 0 ? per_cta : 1));
+        if (p.blocks < 1) p.blocks = 1;
+    } else {
+        p.blocks = grid_for(p.need_hi - p.need_lo, PJ_THREADS, 4 * kNumSMs);
+    }
+    return p;
+}
+
+// The end of the tiles [tile_begin, ...) read evict-last: the first `budget` bytes of the model, a tile at a time.
+int64_t resident_end_tile(const pls_context* ctx, int64_t tile_begin, int64_t budget) {
+    const int64_t tile_bytes = (int64_t)ctx->cfg.local_map_size * 3 * PT_TILE * sizeof(float);
+    return tile_begin + budget / tile_bytes;
+}
+
+}  // namespace
+
 // one ICP iteration on the projective map; pixels [rank*hw/R, (rank+1)*hw/R) are reduced by this rank
 int projmap_icp_iteration(pls_context* ctx, int64_t query_bound, int rank, int num_ranks) {
     ProjMap& pm = ctx->pm;
@@ -753,43 +918,21 @@ int projmap_icp_iteration(pls_context* ctx, int64_t query_bound, int rank, int n
     pm.zbuf_clean = false;
     ProjConst pc = make_proj_const(H, W, ctx->cfg.up_fov_deg, ctx->cfg.down_fov_deg);
     const int K = pm.K;
-    // split of the K candidates between the TMA path and the direct-load path (at most 10 direct)
-    static const int kdirect_env = getenv("PLS_PROJ_KDIRECT") ? atoi(getenv("PLS_PROJ_KDIRECT")) : 4;
-    int kdirect = kdirect_env < 0 ? 0 : (kdirect_env > 10 ? 10 : kdirect_env);
-    if (kdirect > K - 1) kdirect = K > 1 ? K - 1 : 0;
-    const int ktma = K - kdirect;
-    const size_t stage_bytes = (size_t)(ktma * 3 + 4) * PT_TILE * sizeof(float);
-    static const bool no_tma = getenv("PLS_PROJ_NO_TMA") != nullptr;
-    static const int stages = getenv("PLS_PROJ_STAGES") ? atoi(getenv("PLS_PROJ_STAGES")) : 2;
-    const bool use_tma = !no_tma && hw % PT_TILE == 0 && stages >= 1 && stages <= PT_STAGES && stage_bytes * stages <= 200 * 1024;
-    // the pixels this rank reduces: whole 128-pixel tiles on the TMA path.  Only they take part in the z-buffer of the
-    // transformed queries and in the target map, and only they need the model (a sharded rank builds just its share)
-    const int64_t tiles = hw / PT_TILE;
-    const int64_t tile_begin = tiles * rank / num_ranks, tile_end = tiles * (rank + 1) / num_ranks;
-    const int64_t need_lo = use_tma ? tile_begin * PT_TILE : hw * rank / num_ranks;
-    const int64_t need_hi = use_tma ? tile_end * PT_TILE : hw * (rank + 1) / num_ranks;
+    const ProjPlan plan = plan_proj_iteration(ctx, rank, num_ranks);
+    const bool use_tma = plan.use_tma;
+    const int64_t tile_begin = plan.tile_begin, tile_end = plan.tile_end;
+    const int64_t need_lo = plan.need_lo, need_hi = plan.need_hi;
     if (need_lo < pm.built_lo || need_hi > pm.built_hi) rebuild_model(ctx, true);  // (the split rule changed since the update)
     query_zbuf_kernel<<<grid_for(query_bound, 256), 256, 0, st>>>(
         ctx->query_ptr, reinterpret_cast<const uint32_t*>(&fr->counts[1]), 0, fr->T, &fr->done, pc,
         use_tma ? (int)need_lo : 0, use_tma ? (int)need_hi : (int)hw, zbuf);
     PLS_CHECK_LAUNCH();
-    int blocks;
+    const int blocks = plan.blocks;
     if (use_tma) {
-        // TMA-staged persistent kernel over 128-pixel tiles; ranks take contiguous tile ranges
-        const size_t smem = stage_bytes * stages;
         static bool attr_set = false;
         if (!attr_set) {
             PLS_CUDA(cudaFuncSetAttribute(proj_icp_tma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
             attr_set = true;
-        }
-        int per_sm = (int)((220 * 1024) / (smem + 2048));
-        per_sm = per_sm < 1 ? 1 : (per_sm > 8 ? 8 : per_sm);
-        {   // equal tile counts per CTA: ceil(tiles / ceil(tiles / max_ctas)) persistent CTAs
-            const int64_t my_tiles = tile_end - tile_begin;
-            const int64_t max_ctas = (int64_t)per_sm * kNumSMs;
-            const int64_t per_cta = (my_tiles + max_ctas - 1) / max_ctas;
-            blocks = (int)((my_tiles + (per_cta > 0 ? per_cta : 1) - 1) / (per_cta > 0 ? per_cta : 1));
-            if (blocks < 1) blocks = 1;
         }
         ctx->partials.reserve((size_t)blocks * NACC * sizeof(double), st);
         ctx->tmp[7].reserve((size_t)hw * sizeof(float4), st);
@@ -798,22 +941,22 @@ int projmap_icp_iteration(pls_context* ctx, int64_t query_bound, int rank, int n
         PLS_CHECK_LAUNCH();
         // how much of this rank's share of the model asks to stay in the 50 MB L2 between iterations (swept on H100:
         // 16 MB is best for cfg3 and within 2 us of no hint for cfg5; 32 MB and more lose on both, profiles/README.md)
-        static const int resident_mb = getenv("PLS_PROJ_RESIDENT_MB") ? atoi(getenv("PLS_PROJ_RESIDENT_MB")) : 16;
-        const int64_t tile_bytes = (int64_t)ctx->cfg.local_map_size * 3 * PT_TILE * sizeof(float);
-        const int64_t resident_end = tile_begin + ((int64_t)resident_mb << 20) / tile_bytes;
+        int resident_mb = 16;
+        resident_mb_env(&resident_mb);
+        const int64_t resident_end = resident_end_tile(ctx, tile_begin, (int64_t)resident_mb << 20);
         // (a persisting access-policy window on the stream -- a set-aside part of L2 -- was tried instead of the
         // per-instruction priorities and was slower)
         ProfileScope ps(ctx, 1, 0.0, false);
-        proj_icp_tma_kernel<<<blocks, PT_TILE, smem, st>>>(pm.model_v.as<float>(), pm.model_n.as<float4>(), K,
-                                                           ctx->cfg.local_map_size, ctx->tmp[7].as<float4>(), fr, tile_begin,
-                                                           tile_end, ctx->cfg.scheme, ctx->cfg.sigma, stages, ktma, resident_end,
-                                                           L2_EVICT_LAST, L2_EVICT_FIRST, ctx->partials.as<double>());
+        proj_icp_tma_kernel<<<blocks, PT_TILE, plan.smem, st>>>(pm.model_v.as<float>(), pm.model_n.as<float4>(), K,
+                                                                ctx->cfg.local_map_size, ctx->tmp[7].as<float4>(), fr, tile_begin,
+                                                                tile_end, ctx->cfg.scheme, ctx->cfg.sigma, plan.stages, plan.ktma,
+                                                                resident_end, L2_EVICT_LAST, L2_EVICT_FIRST,
+                                                                ctx->partials.as<double>());
         PLS_CHECK_LAUNCH();
         pm.zbuf_clean = true;
         return blocks;
     }
-    const int64_t pix_begin = hw * rank / num_ranks, pix_end = hw * (rank + 1) / num_ranks;
-    blocks = grid_for(pix_end - pix_begin, PJ_THREADS, 4 * kNumSMs);
+    const int64_t pix_begin = need_lo, pix_end = need_hi;
     ctx->partials.reserve((size_t)blocks * NACC * sizeof(double), st);
     {
         ProfileScope ps(ctx, 1, 0.0, false);
@@ -824,6 +967,138 @@ int projmap_icp_iteration(pls_context* ctx, int64_t query_bound, int rank, int n
         PLS_CHECK_LAUNCH();
     }
     return blocks;
+}
+
+// pls_process_frames: the descriptors of the projective sequences whose ICP runs in this call, into lead->batch_buf
+// (uploaded on st) with their done flags and then the TMA sequences' partial rows behind them, one range per sequence,
+// and every buffer their iterations use reserved as their single path reserves it.
+// grid[4]: the launch widths (the largest query z-buffer / resolve / TMA block count of a sequence) and the TMA
+// kernel's dynamic shared memory (the largest of a sequence; 0: no sequence takes the TMA path).
+void projmap_batch_begin(pls_context* lead, pls_context* const* ctxs, const int64_t* query_bounds, int num, cudaStream_t st,
+                         int* grid) {
+    std::vector<ProjSeq> seqs((size_t)num);
+    std::vector<ProjPlan> plans((size_t)num);
+    int tma_seqs = 0;
+    size_t rows = 0;
+    for (int i = 0; i < num; ++i) {
+        PLS_REQUIRE(ctxs[i]->pm.valid, "projective map: search before any update");
+        plans[(size_t)i] = plan_proj_iteration(ctxs[i], 0, 1);
+        if (plans[(size_t)i].use_tma) {
+            tma_seqs += 1;
+            rows += (size_t)plans[(size_t)i].blocks;
+        }
+    }
+    // The L2 budget for evict-last reads: the single path's 16 MB, split evenly across the TMA sequences (measured on
+    // H100 against 16 MB for each of them, DESIGN section 11).  PLS_PROJ_RESIDENT_MB is each sequence's own budget.
+    int mb = 16;
+    const int64_t budget = resident_mb_env(&mb) ? (int64_t)mb << 20 : ((int64_t)16 << 20) / (tma_seqs > 0 ? tma_seqs : 1);
+    const size_t head = (num * sizeof(ProjSeq) + PLS_MAX_SEQUENCES * sizeof(int) + 255) / 256 * 256;
+    lead->batch_buf.reserve(head + rows * NACC * sizeof(double), st);
+    double* part = reinterpret_cast<double*>(lead->batch_buf.as<char>() + head);
+    grid[0] = grid[1] = grid[2] = 1;
+    grid[3] = 0;
+    for (int i = 0; i < num; ++i) {
+        pls_context* ctx = ctxs[i];
+        const ProjPlan& plan = plans[(size_t)i];
+        const int64_t hw = (int64_t)ctx->cfg.height * ctx->cfg.width;
+        FrameResult* fr = frame_result_dev(ctx);
+        ctx->last_sharded = false;
+        ctx->tmp[3].reserve((size_t)hw * sizeof(unsigned long long), st);
+        ProjSeq& s = seqs[(size_t)i];
+        s.model_v = ctx->pm.model_v.as<float>();
+        s.model_n = ctx->pm.model_n.as<float4>();
+        s.queries = ctx->query_ptr;
+        s.nq_dev = reinterpret_cast<const uint32_t*>(&fr->counts[1]);
+        s.fr = fr;
+        s.zbuf = ctx->tmp[3].as<unsigned long long>();
+        s.pc = make_proj_const(ctx->cfg.height, ctx->cfg.width, ctx->cfg.up_fov_deg, ctx->cfg.down_fov_deg);
+        s.K = ctx->pm.K;
+        s.kcap = ctx->cfg.local_map_size;
+        s.ktma = plan.ktma;
+        s.stages = plan.stages;
+        s.scheme = ctx->cfg.scheme;
+        s.sigma = ctx->cfg.sigma;
+        s.threshold_delta = ctx->cfg.threshold_delta_pose;
+        s.tiles = hw / PT_TILE;
+        s.resident_end = resident_end_tile(ctx, 0, budget);
+        s.step_blocks = plan.blocks;
+        s.max_iters = ctx->cfg.max_num_alignments;
+        if (plan.use_tma) {
+            ctx->tmp[7].reserve((size_t)hw * sizeof(float4), st);
+            s.tgt = ctx->tmp[7].as<float4>();
+            s.partials = part;
+            part += (size_t)plan.blocks * NACC;
+            s.zbuf_blocks = grid_for(query_bounds[i], 256);
+            s.resolve_blocks = grid_for(hw, 256);
+            s.tma_blocks = plan.blocks;
+            grid[0] = grid[0] > s.zbuf_blocks ? grid[0] : s.zbuf_blocks;
+            grid[1] = grid[1] > s.resolve_blocks ? grid[1] : s.resolve_blocks;
+            grid[2] = grid[2] > s.tma_blocks ? grid[2] : s.tma_blocks;
+            grid[3] = grid[3] > (int)plan.smem ? grid[3] : (int)plan.smem;
+        } else {
+            // its own launches write ctx->partials (projmap_icp_iteration reserves the same size: no reallocation)
+            ctx->partials.reserve((size_t)plan.blocks * NACC * sizeof(double), st);
+            s.tgt = nullptr;
+            s.partials = ctx->partials.as<double>();
+            s.zbuf_blocks = s.resolve_blocks = s.tma_blocks = 0;
+        }
+    }
+    PLS_CUDA(cudaMemcpyAsync(lead->batch_buf.p, seqs.data(), seqs.size() * sizeof(ProjSeq), cudaMemcpyHostToDevice, st));
+}
+
+// ICP iterations [first, last) of the sequences projmap_batch_begin described, on st: one launch per kernel for all of
+// them.  A sequence off the TMA path runs its correspondences through its own launches; the step kernel serves all.
+void projmap_batch_iterations(pls_context* lead, pls_context* const* ctxs, const int64_t* query_bounds, int num, cudaStream_t st,
+                              const int* grid, int first, int last) {
+    const ProjSeq* seqs = lead->batch_buf.as<ProjSeq>();
+    static bool attr_set = false;
+    if (!attr_set) {
+        PLS_CUDA(cudaFuncSetAttribute(proj_icp_tma_batch_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+        attr_set = true;
+    }
+    for (int it = first; it < last; ++it) {
+        for (int i = 0; i < num; ++i) {
+            pls_context* ctx = ctxs[i];
+            if (it >= ctx->cfg.max_num_alignments) continue;
+            if (plan_proj_iteration(ctx, 0, 1).use_tma) {
+                // the first iteration clears the query z-buffer (the frame's own projection used it); the resolve kernel
+                // leaves it clear for the next
+                if (it == 0)
+                    PLS_CUDA(cudaMemsetAsync(ctx->tmp[3].p, 0xff,
+                                             (size_t)ctx->cfg.height * ctx->cfg.width * sizeof(unsigned long long), st));
+                ctx->pm.zbuf_clean = true;
+                continue;
+            }
+            cudaStream_t own = ctx->stream;
+            ctx->stream = st;
+            try {
+                projmap_icp_iteration(ctx, query_bounds[i], 0, 1);
+            } catch (...) {
+                ctx->stream = own;
+                throw;
+            }
+            ctx->stream = own;
+        }
+        if (grid[3] > 0) {
+            query_zbuf_batch_kernel<<<dim3(grid[0], num), 256, 0, st>>>(seqs, it);
+            PLS_CHECK_LAUNCH();
+            query_resolve_batch_kernel<<<dim3(grid[1], num), 256, 0, st>>>(seqs, it);
+            PLS_CHECK_LAUNCH();
+            proj_icp_tma_batch_kernel<<<dim3(grid[2], num), PT_TILE, (size_t)grid[3], st>>>(seqs, it);
+            PLS_CHECK_LAUNCH();
+        }
+        icp_step_batch_kernel<<<dim3(1, num), 256, 0, st>>>(seqs, it);
+        PLS_CHECK_LAUNCH();
+    }
+}
+
+// The done flag of every sequence of the batch: one gather launch, one copy, one synchronisation.
+void projmap_batch_done(pls_context* lead, int num, cudaStream_t st, int* out) {
+    int* dev = reinterpret_cast<int*>(lead->batch_buf.as<char>() + (size_t)num * sizeof(ProjSeq));
+    proj_batch_done_kernel<<<1, 64, 0, st>>>(lead->batch_buf.as<ProjSeq>(), num, dev);
+    PLS_CHECK_LAUNCH();
+    PLS_CUDA(cudaMemcpyAsync(out, dev, (size_t)num * sizeof(int), cudaMemcpyDeviceToHost, st));
+    PLS_CUDA(cudaStreamSynchronize(st));
 }
 
 }  // namespace pls

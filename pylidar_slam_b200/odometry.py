@@ -729,7 +729,9 @@ class ICPFrameToModelBatch:
         for o in odos: o.init()
         batch.process_next_frames([dd0, dd1, None, dd3])   # None: no frame for that sequence this step
 
-    Supported: kd-tree local maps, gauss_newton_config.max_iters == 1, one CUDA device, at most 64 sequences."""
+    Supported: kd-tree or projective local maps (one type per batch; the sequences may differ in every other setting,
+    frame size and local_map_size included), gauss_newton_config.max_iters == 1, one CUDA device, at most 64
+    sequences."""
 
     def __init__(self, odometries):
         odos = list(odometries)
@@ -737,7 +739,8 @@ class ICPFrameToModelBatch:
         for o in odos:
             assert_debug(isinstance(o, ICPFrameToModel), "ICPFrameToModelBatch batches ICPFrameToModel objects")
             assert_debug(not o._fine_grained, "batched sequences need gauss_newton_config.max_iters == 1")
-            assert_debug(o.ctx.cfg.local_map_type == _lib.MAP_KDTREE, "batched sequences need a kd-tree local map")
+            assert_debug(o.ctx.cfg.local_map_type == odos[0].ctx.cfg.local_map_type,
+                         "batched sequences share one local map type: all kd-tree or all projective")
         assert_debug(len({id(o) for o in odos}) == len(odos), "an odometry is listed twice")
         assert_debug(len({int(o.ctx.cfg.device) for o in odos}) == 1, "every odometry must run on one CUDA device")
         self.odometries = odos
