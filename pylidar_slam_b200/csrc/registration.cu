@@ -10,9 +10,9 @@
 //   procrustes_moments_kernel : sum w, sum w p_t, sum w p_r  -> one float64 partial row per block
 //   procrustes_cross_kernel   : every block folds the moment partials in its prologue, then accumulates the 9
 //                               entries of C in float64 (warp shuffle + shared-memory block reduction)
-//   procrustes_solve_kernel   : one warp sums the C partials in fixed order; thread 0 runs a cyclic-Jacobi
-//                               eigen-decomposition of C^T C (float64), u_i = C v_i / sigma_i for the two largest
-//                               singular values, and closes the frame with u_3 = det(V) u_1 x u_2 -- identical to
+//   procrustes_solve_kernel   : one warp sums the C partials in fixed order; thread 0 runs a one-sided cyclic-Jacobi
+//                               SVD of C itself (float64; C^T C would square its condition number), takes u_1, u_2
+//                               of the two largest singular values, and closes the frame with u_3 = det(V) u_1 x u_2 -- identical to
 //                               U diag(1, 1, +-1) V^T whenever the SVD is unique, and well defined for planar clouds
 //                               (sigma_3 = 0) where LAPACK's u_3 is arbitrary up to the same sign rule.
 //

@@ -6,50 +6,54 @@
 
 namespace pls {
 
-// Cyclic Jacobi on a symmetric 3x3 (float64): A = V diag(d) V^T, columns of V orthonormal.
-__host__ __device__ inline void jacobi3(double A[3][3], double V[3][3], double d[3]) {
+// One-sided (Hestenes) cyclic Jacobi SVD of a 3x3 (float64): plane rotations J of column pairs make the columns of
+// B = C V mutually orthogonal, so B = U diag(s) with s[k] = |B e_k| and the columns of V orthonormal.  Working on C
+// itself rather than on C^T C keeps the small singular directions accurate to eps / (relative gap): squaring C squares
+// its condition number, and the eigen-decomposition of C^T C loses the rotation about the long axis of an elongated
+// cloud once sigma_2 / sigma_1 falls below ~1e-3.
+__host__ __device__ inline void svd3_one_sided(const double C[3][3], double B[3][3], double V[3][3], double s[3]) {
     for (int i = 0; i < 3; ++i)
-        for (int j = 0; j < 3; ++j) V[i][j] = (i == j) ? 1.0 : 0.0;
+        for (int j = 0; j < 3; ++j) {
+            B[i][j] = C[i][j];
+            V[i][j] = (i == j) ? 1.0 : 0.0;
+        }
     for (int sweep = 0; sweep < 32; ++sweep) {
-        const double off = fabs(A[0][1]) + fabs(A[0][2]) + fabs(A[1][2]);
-        const double diag = fabs(A[0][0]) + fabs(A[1][1]) + fabs(A[2][2]);
-        if (off <= 1e-300 || off <= 1e-17 * diag) break;
+        bool rotated = false;
         for (int p = 0; p < 2; ++p)
             for (int q = p + 1; q < 3; ++q) {
-                if (A[p][q] == 0.0) continue;
-                const double theta = (A[q][q] - A[p][p]) / (2.0 * A[p][q]);
-                const double t = (theta >= 0.0 ? 1.0 : -1.0) / (fabs(theta) + sqrt(theta * theta + 1.0));
-                const double c = 1.0 / sqrt(t * t + 1.0), s = t * c;
-                for (int k = 0; k < 3; ++k) {  // A <- A J
-                    const double akp = A[k][p], akq = A[k][q];
-                    A[k][p] = c * akp - s * akq;
-                    A[k][q] = s * akp + c * akq;
-                }
-                for (int k = 0; k < 3; ++k) {  // A <- J^T A
-                    const double apk = A[p][k], aqk = A[q][k];
-                    A[p][k] = c * apk - s * aqk;
-                    A[q][k] = s * apk + c * aqk;
-                }
+                double alpha = 0.0, beta = 0.0, gamma = 0.0;
                 for (int k = 0; k < 3; ++k) {
+                    alpha += B[k][p] * B[k][p];
+                    beta += B[k][q] * B[k][q];
+                    gamma += B[k][p] * B[k][q];
+                }
+                if (!(fabs(gamma) > 1e-17 * sqrt(alpha * beta))) continue;  // orthogonal to working precision (or zero)
+                rotated = true;
+                const double zeta = (beta - alpha) / (2.0 * gamma);
+                const double t = (zeta >= 0.0 ? 1.0 : -1.0) / (fabs(zeta) + sqrt(zeta * zeta + 1.0));
+                const double c = 1.0 / sqrt(t * t + 1.0), sn = t * c;
+                for (int k = 0; k < 3; ++k) {
+                    const double bkp = B[k][p], bkq = B[k][q];
+                    B[k][p] = c * bkp - sn * bkq;
+                    B[k][q] = sn * bkp + c * bkq;
                     const double vkp = V[k][p], vkq = V[k][q];
-                    V[k][p] = c * vkp - s * vkq;
-                    V[k][q] = s * vkp + c * vkq;
+                    V[k][p] = c * vkp - sn * vkq;
+                    V[k][q] = sn * vkp + c * vkq;
                 }
             }
+        if (!rotated) break;
     }
-    for (int i = 0; i < 3; ++i) d[i] = A[i][i];
+    for (int k = 0; k < 3; ++k) s[k] = sqrt(B[0][k] * B[0][k] + B[1][k] * B[1][k] + B[2][k] * B[2][k]);
 }
 
 // R = U diag(1, 1, sign(det U det V)) V^T of the cross-covariance C (row-major, reference rows x target columns),
 // t = mu_r - R mu_t; mu = (mu_t, mu_r).  Registration.py:48-73.
 __host__ __device__ inline void kabsch_from_cross(const double* C9, const double* mu, double* out_T /*[16]*/) {
-    double Cm[3][3], A[3][3], V[3][3], d[3];
+    double Cm[3][3], B[3][3], V[3][3], d[3];
     for (int i = 0; i < 3; ++i)
         for (int j = 0; j < 3; ++j) Cm[i][j] = C9[3 * i + j];
-    for (int i = 0; i < 3; ++i)
-        for (int j = 0; j < 3; ++j) A[i][j] = Cm[0][i] * Cm[0][j] + Cm[1][i] * Cm[1][j] + Cm[2][i] * Cm[2][j];  // C^T C
-    jacobi3(A, V, d);
-    // order the eigenpairs by descending eigenvalue (LAPACK's singular-value order)
+    svd3_one_sided(Cm, B, V, d);
+    // order the singular triplets by descending singular value (LAPACK's order)
     int o[3] = {0, 1, 2};
     for (int i = 0; i < 2; ++i)
         for (int j = i + 1; j < 3; ++j)
@@ -58,8 +62,8 @@ __host__ __device__ inline void kabsch_from_cross(const double* C9, const double
     for (int k = 0; k < 3; ++k)
         for (int i = 0; i < 3; ++i) v[k][i] = V[i][o[k]];
     for (int k = 0; k < 2; ++k) {
-        for (int i = 0; i < 3; ++i) u[k][i] = Cm[i][0] * v[k][0] + Cm[i][1] * v[k][1] + Cm[i][2] * v[k][2];
-        if (k == 1) {  // Gram-Schmidt against u_0: C v_1 is orthogonal to it only up to rounding
+        for (int i = 0; i < 3; ++i) u[k][i] = B[i][o[k]];  // = sigma_k u_k
+        if (k == 1) {  // Gram-Schmidt against u_0: the columns of B are orthogonal only up to rounding
             const double dp = u[1][0] * u[0][0] + u[1][1] * u[0][1] + u[1][2] * u[0][2];
             for (int i = 0; i < 3; ++i) u[1][i] -= dp * u[0][i];
         }
