@@ -276,12 +276,6 @@ void grid_sample_count_to_host(pls_context* ctx) {
     PLS_CUDA(cudaMemcpyAsync(words, scalar_u32(ctx, SC_GS_COUNT), 8 * sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
 }
 
-uint32_t grid_sample_host_count(pls_context* ctx, bool* overflowed) {
-    const uint32_t* words = reinterpret_cast<const uint32_t*>(reinterpret_cast<const char*>(ctx->pinned.p) + kScalarOffset);
-    *overflowed = ctx->gs_seq != 0 && words[SC_GS_OVERFLOW] == ctx->gs_seq;
-    return words[SC_GS_COUNT];
-}
-
 void grid_sample_launch(pls_context* ctx, const GridSample& g, bool compact) {
     if (!g.f64)
         grid_sample_device<float>(ctx, (const float*)g.xyz, g.n, g.voxel, (float*)g.out_xyz, g.out_idx, compact,
@@ -293,9 +287,15 @@ void grid_sample_launch(pls_context* ctx, const GridSample& g, bool compact) {
 
 }  // namespace
 
-void grid_sample_enqueue(pls_context* ctx, const GridSample& g) {
+void grid_sample_enqueue(pls_context* ctx, const GridSample& g, bool count_to_host) {
     grid_sample_launch(ctx, g, true);
-    grid_sample_count_to_host(ctx);
+    if (count_to_host) grid_sample_count_to_host(ctx);
+}
+
+uint32_t grid_sample_host_count(pls_context* ctx, bool* overflowed) {
+    const uint32_t* words = reinterpret_cast<const uint32_t*>(reinterpret_cast<const char*>(ctx->pinned.p) + kScalarOffset);
+    *overflowed = ctx->gs_seq != 0 && words[SC_GS_OVERFLOW] == ctx->gs_seq;
+    return words[SC_GS_COUNT];
 }
 
 uint32_t grid_sample_finish(pls_context* ctx, const GridSample& g) {

@@ -42,6 +42,29 @@ extern long long g_kernel_launches;
         PLS_CUDA(cudaGetLastError()); \
     } while (0)
 
+// A launch of a kernel on a dependent chain, with programmatic stream serialisation: the kernel may be launched while
+// its predecessor in the stream is still finishing, which hides the launch latency between the two.  Every kernel
+// launched this way calls pls_grid_dependency_wait() before its first global memory access; the wait returns once the
+// predecessor grid has completed and its writes are visible, and is a no-op in a plain launch.
+#ifdef __CUDACC__
+__device__ __forceinline__ void pls_grid_dependency_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+#endif
+template <typename... KArgs, typename... Args>
+void launch_dependent(void (*kernel)(KArgs...), dim3 grid, dim3 block, cudaStream_t st, Args&&... args) {
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = grid;
+    cfg.blockDim = block;
+    cfg.dynamicSmemBytes = 0;
+    cfg.stream = st;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    PLS_CUDA(cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...));
+    PLS_CHECK_LAUNCH();
+}
+
 #define PLS_REQUIRE(cond, text)                                   \
     do {                                                          \
         if (!(cond)) throw pls::Error{PLS_E_INVALID, (text)};     \
@@ -385,9 +408,11 @@ void kdmap_batch_iterations(pls_context* lead, pls_context* const* ctxs, const i
 void kdmap_batch_done(pls_context* lead, int num, cudaStream_t st, int* out);
 // ICP iteration `it` of the frame over ctx->query_ptr; returns the number of partial rows written
 // it == 0: no previous matches; fuse_threshold >= 0: finish the iteration (sum + solve + pose update) in the last
-// block of the reduction kernel (*solved tells).
-int kdmap_icp_iteration(pls_context* ctx, int64_t query_bound, int rank, int num_ranks, int it, float fuse_threshold,
-                        bool* solved);
+// block of the reduction kernel (*solved tells).  bound_dev (nullable, unsharded frames only): a device-side count that
+// tightens query_bound; the kernels then use the block count of min(query_bound, *bound_dev) queries, and the returned
+// count is the launched one, that of query_bound.
+int kdmap_icp_iteration(pls_context* ctx, int64_t query_bound, const uint32_t* bound_dev, int rank, int num_ranks, int it,
+                        float fuse_threshold, bool* solved);
 // pack [n,3] rows without NaN into float4 (stable); count -> *count_dev (u32)
 void pack_valid_rows(pls_context* ctx, const float* pts_dev, int64_t n, float4* out, uint32_t* count_dev);
 void pack_valid_rows_f64(pls_context* ctx, const double* pts_dev, int64_t n, float4* out, uint32_t* count_dev);
@@ -413,8 +438,12 @@ struct GridSample {
 // coordinates up to ~3 000 000 in magnitude, and copies the count and the overflow stamp to the host.  finish, once
 // ctx->stream has been synchronised, returns the count; if a hash overflowed the compact keys it first samples once more
 // on the raw 64-bit keys and reads that count (one more copy and stream synchronisation).
-void grid_sample_enqueue(pls_context* ctx, const GridSample& g);
+// count_to_host = false leaves the count and the stamp in the device scalars (SC_GS_COUNT, SC_GS_OVERFLOW) for a caller
+// that copies them back later with its own result (the FrameResult copy covers both); grid_sample_host_count then reads
+// them from that copy.
+void grid_sample_enqueue(pls_context* ctx, const GridSample& g, bool count_to_host = true);
 uint32_t grid_sample_finish(pls_context* ctx, const GridSample& g);
+uint32_t grid_sample_host_count(pls_context* ctx, bool* overflowed);
 // projmap.cu
 void projmap_reset(pls_context* ctx);
 // pls_process_frames on projective maps, the counterparts of kdmap_batch_*: begin uploads the descriptors into

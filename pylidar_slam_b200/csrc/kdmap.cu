@@ -145,6 +145,7 @@ __global__ void kd_grid_header_kernel(int* __restrict__ bbox, KdGridHeader* __re
 // insertion order (stable sort), nothing finer is needed: every level's cell is a prefix of this id.
 __global__ void kd_cell_key_kernel(const float4* __restrict__ pts, int64_t n, const KdGridHeader* __restrict__ hdr,
                                    uint64_t* __restrict__ keys, uint32_t* __restrict__ vals) {
+    pls_grid_dependency_wait();
     const float mnx = hdr->mn[0], mny = hdr->mn[1], mnz = hdr->mn[2];
     const float scale = hdr->scale;
     const int b0 = hdr->b0;
@@ -189,6 +190,7 @@ __device__ __forceinline__ int cell_claim(uint4* table, uint32_t mask, uint32_t 
 __global__ void __launch_bounds__(256)
 kd_finalize_kernel(const float4* __restrict__ pts, const uint64_t* __restrict__ keys, const uint32_t* __restrict__ order,
                    int64_t n, CellTables T, KdGridHeader* hdr, uint32_t gen, float4* __restrict__ sorted) {
+    pls_grid_dependency_wait();
     const int top = hdr->top;
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
         const uint32_t src = order[i];
@@ -288,6 +290,17 @@ __device__ __forceinline__ unsigned long long* kd_split_record(const FrameResult
 #define KD_SPLIT_ARG
 #define KD_SPLIT_PASS
 #endif
+
+// The block count of a residual or refine launch.  bound_dev null: the launched grid.  Else the host launched for the
+// bound `bound` of a query count the device knows, *bound_dev: the count is that of the grid the host would launch for
+// min(bound, *bound_dev) queries (grid_for), so that the striding, the block partials and the solve ticket -- and with
+// them the bits -- are those of a launch sized on the host; blocks past it return at once.
+__device__ __forceinline__ unsigned kd_logical_blocks(int64_t bound, const uint32_t* __restrict__ bound_dev) {
+    if (!bound_dev) return gridDim.x;
+    const int64_t n = min(bound, (int64_t)*bound_dev);
+    const int64_t b = (n + KD_THREADS - 1) / KD_THREADS;
+    return (unsigned)(b < 1 ? 1 : (b > 8 * kNumSMs ? 8 * kNumSMs : b));
+}
 
 // Appends this block's entries (collected in shared memory by any of its threads) to a global list: one atomic per block.
 __device__ __forceinline__ void block_flush_list(const int* s_list, int n, int* __restrict__ list, uint32_t* count, int* s_base) {
@@ -488,6 +501,7 @@ kd_nn_warp_kernel(KdIndex ix, const float4* __restrict__ queries, const uint32_t
                   int64_t q_stride, const int* __restrict__ hard, uint32_t* lists, int parity, const float* __restrict__ T,
                   const int* __restrict__ done, int* __restrict__ match, float4* __restrict__ nn_state, int want_normals,
                   int* __restrict__ pending, unsigned long long* __restrict__ counters) {
+    pls_grid_dependency_wait();
     kd_nn_warp_body(ix, queries, nq_dev, q_begin, q_stride, hard, lists, parity, T, done, match, nn_state, want_normals,
                     pending, counters, blockIdx.x, gridDim.x);
 }
@@ -552,6 +566,7 @@ __device__ __forceinline__ void kd_normals_warp_body(const KdIndex& ix, int k_no
 __global__ void __launch_bounds__(KD_THREADS)
 kd_normals_warp_kernel(KdIndex ix, int k_normals, const int* __restrict__ worklist, const uint32_t* __restrict__ wl_count,
                        const int* __restrict__ done, unsigned long long* __restrict__ counters) {
+    pls_grid_dependency_wait();
     kd_normals_warp_body(ix, k_normals, worklist, wl_count, done, counters, blockIdx.x, gridDim.x);
 }
 
@@ -586,10 +601,14 @@ __device__ __forceinline__ void kd_residual_body(const KdIndex& ix, const float4
 __global__ void __launch_bounds__(KD_THREADS)
 kd_residual_kernel(KdIndex ix, const float4* __restrict__ queries, const uint32_t* __restrict__ nq_dev, int64_t q_begin,
                    int64_t q_stride, FrameResult* fr, int scheme, float sigma,
-                   const int* __restrict__ match, double* __restrict__ partials, float fuse_threshold) {
+                   const int* __restrict__ match, double* __restrict__ partials, float fuse_threshold, int64_t bound,
+                   const uint32_t* __restrict__ bound_dev) {
+    pls_grid_dependency_wait();
+    const unsigned grid = kd_logical_blocks(bound, bound_dev);
+    if (blockIdx.x >= grid) return;
     KD_SPLIT_BEGIN()
     kd_residual_body(ix, queries, nq_dev, q_begin, q_stride, fr, scheme, sigma, match, partials, fuse_threshold, blockIdx.x,
-                     gridDim.x KD_SPLIT_PASS);
+                     grid KD_SPLIT_PASS);
 }
 
 // ICP iterations after a frame's first, in ONE launch.  Each block takes the queries kd_residual_kernel would give it
@@ -691,10 +710,13 @@ __global__ void __launch_bounds__(KD_REFINE_THREADS)
 kd_icp_refine_kernel(KdIndex ix, const float4* __restrict__ queries, const uint32_t* __restrict__ nq_dev, int64_t q_begin,
                      int64_t q_stride, FrameResult* fr, int scheme, float sigma, int k_normals, int* __restrict__ match,
                      float4* __restrict__ nn_state, double* __restrict__ partials, float fuse_threshold,
-                     unsigned long long* __restrict__ counters) {
+                     unsigned long long* __restrict__ counters, int64_t bound, const uint32_t* __restrict__ bound_dev) {
+    pls_grid_dependency_wait();
+    const unsigned grid = kd_logical_blocks(bound, bound_dev);
+    if (blockIdx.x >= grid) return;
     KD_SPLIT_BEGIN()
     kd_icp_refine_body(ix, queries, nq_dev, q_begin, q_stride, fr, scheme, sigma, k_normals, match, nn_state, partials,
-                       fuse_threshold, counters, blockIdx.x, gridDim.x KD_SPLIT_PASS);
+                       fuse_threshold, counters, blockIdx.x, grid KD_SPLIT_PASS);
 }
 
 // ---- several sequences per launch (pls_process_frames) --------------------------------------------------------------
@@ -886,9 +908,8 @@ void build_index(pls_context* ctx) {
     kd_grid_header_kernel<<<1, 32, 0, st>>>(kd.bbox.as<int>(), kd.grid_hdr.as<KdGridHeader>(), cell_target);
     PLS_CHECK_LAUNCH();
     kd.bbox_clean = true;
-    kd_cell_key_kernel<<<grid_for(M, 256, 8 * kNumSMs), 256, 0, st>>>(pts, M, kd.grid_hdr.as<KdGridHeader>(),
-                                                                       kd.morton.as<uint64_t>(), kd.order.as<uint32_t>());
-    PLS_CHECK_LAUNCH();
+    launch_dependent(kd_cell_key_kernel, grid_for(M, 256, 8 * kNumSMs), 256, st, pts, M, kd.grid_hdr.as<KdGridHeader>(),
+                     kd.morton.as<uint64_t>(), kd.order.as<uint32_t>());
     uint64_t* sk;
     uint32_t* sv;
     radix_sort_pairs(ctx, kd.morton.as<uint64_t>(), kd.order.as<uint32_t>(), M, 4, &sk, &sv, kd.cap_points);
@@ -899,9 +920,8 @@ void build_index(pls_context* ctx) {
         T.table[l] = reinterpret_cast<uint4*>(reinterpret_cast<char*>(kd.cells.p) + kd.table_offset[l]);
         T.mask[l] = kd.table_mask[l];
     }
-    kd_finalize_kernel<<<grid_for(M, 256, 8 * kNumSMs), 256, 0, st>>>(pts, sk, sv, M, T, kd.grid_hdr.as<KdGridHeader>(),
-                                                                       kd.gen, kd.sorted.as<float4>());
-    PLS_CHECK_LAUNCH();
+    launch_dependent(kd_finalize_kernel, grid_for(M, 256, 8 * kNumSMs), 256, st, pts, sk, sv, M, T, kd.grid_hdr.as<KdGridHeader>(),
+                     kd.gen, kd.sorted.as<float4>());
 }
 
 }  // namespace
@@ -1110,16 +1130,14 @@ static void launch_search(pls_context* ctx, const KdPlan& plan, const KdIndex& i
     }
     {
         ProfileScope p7(ctx, 7, 0.0);
-        kd_nn_warp_kernel<<<wblocks < resident_nn ? wblocks : resident_nn, KD_THREADS, 0, st>>>(
-            ix, queries, nq_dev, (int64_t)rank, (int64_t)num_ranks, first ? nullptr : hard_nn, lists, parity, T, done, match, nn_state,
-            normals ? 1 : 0, pending, counters);
-        PLS_CHECK_LAUNCH();
+        launch_dependent(kd_nn_warp_kernel, wblocks < resident_nn ? wblocks : resident_nn, KD_THREADS, st, ix, queries, nq_dev,
+                         (int64_t)rank, (int64_t)num_ranks, first ? nullptr : hard_nn, lists, parity, T, done, match, nn_state,
+                         normals ? 1 : 0, pending, counters);
     }
     if (!normals) return;
     ProfileScope p9(ctx, 9, 0.0);
-    kd_normals_warp_kernel<<<wblocks < resident_kn ? wblocks : resident_kn, KD_THREADS, 0, st>>>(
-        ix, ctx->cfg.num_neighbors_normals, pending, lists + KDL_PENDING + parity, done, counters);
-    PLS_CHECK_LAUNCH();
+    launch_dependent(kd_normals_warp_kernel, wblocks < resident_kn ? wblocks : resident_kn, KD_THREADS, st, ix,
+                     ctx->cfg.num_neighbors_normals, pending, lists + KDL_PENDING + parity, done, counters);
 }
 
 // Later ICP iterations run as one kd_icp_refine_kernel, except on maps of this many points or more.  On the 5 M-point
@@ -1130,9 +1148,10 @@ constexpr int64_t KD_COLD_MAP_POINTS = 2000000;
 
 // One ICP iteration over the device-resident queries (float4 in ctx->query_ptr, count in the FrameResult); writes
 // block partials to ctx->partials and returns the block count.
-int kdmap_icp_iteration(pls_context* ctx, int64_t query_bound, int rank, int num_ranks, int it, float fuse_threshold,
-                        bool* solved) {
+int kdmap_icp_iteration(pls_context* ctx, int64_t query_bound, const uint32_t* bound_dev, int rank, int num_ranks, int it,
+                        float fuse_threshold, bool* solved) {
     PLS_REQUIRE(ctx->kd.valid, "kd map: search before any update");
+    PLS_REQUIRE(!bound_dev || num_ranks == 1, "kd ICP: a device-side query bound needs an unsharded frame");
     cudaStream_t st = ctx->stream;
     FrameResult* fr = frame_result_dev(ctx);
     const uint32_t* nq_dev = reinterpret_cast<const uint32_t*>(&fr->counts[1]);
@@ -1146,17 +1165,15 @@ int kdmap_icp_iteration(pls_context* ctx, int64_t query_bound, int rank, int num
         launch_search(ctx, plan, ix, ctx->query_ptr, nq_dev, rank, num_ranks, fr->T, &fr->done, ctx->nn_prev.as<int>(), it == 0,
                       true, it & 1);
         ProfileScope p10(ctx, 10, 0.0);
-        kd_residual_kernel<<<blocks, KD_THREADS, 0, st>>>(ix, ctx->query_ptr, nq_dev, (int64_t)rank, (int64_t)num_ranks, fr,
-                                                          ctx->cfg.scheme, ctx->cfg.sigma, ctx->nn_prev.as<int>(),
-                                                          ctx->partials.as<double>(), fuse_threshold);
-        PLS_CHECK_LAUNCH();
+        launch_dependent(kd_residual_kernel, blocks, KD_THREADS, st, ix, ctx->query_ptr, nq_dev, (int64_t)rank, (int64_t)num_ranks,
+                         fr, ctx->cfg.scheme, ctx->cfg.sigma, ctx->nn_prev.as<int>(), ctx->partials.as<double>(), fuse_threshold,
+                         plan.mine, bound_dev);
     } else {
         ProfileScope p11(ctx, 11, 0.0);
-        kd_icp_refine_kernel<<<blocks, KD_REFINE_THREADS, 0, st>>>(ix, ctx->query_ptr, nq_dev, (int64_t)rank, (int64_t)num_ranks, fr,
-                                                            ctx->cfg.scheme, ctx->cfg.sigma, ctx->cfg.num_neighbors_normals,
-                                                            ctx->nn_prev.as<int>(), ctx->kd_nn_state.as<float4>(),
-                                                            ctx->partials.as<double>(), fuse_threshold, kd_counters(ctx));
-        PLS_CHECK_LAUNCH();
+        launch_dependent(kd_icp_refine_kernel, blocks, KD_REFINE_THREADS, st, ix, ctx->query_ptr, nq_dev, (int64_t)rank,
+                         (int64_t)num_ranks, fr, ctx->cfg.scheme, ctx->cfg.sigma, ctx->cfg.num_neighbors_normals,
+                         ctx->nn_prev.as<int>(), ctx->kd_nn_state.as<float4>(), ctx->partials.as<double>(), fuse_threshold,
+                         kd_counters(ctx), plan.mine, bound_dev);
     }
     *solved = fuse_threshold >= 0.f;
     return blocks;
@@ -1232,7 +1249,7 @@ void kdmap_batch_iterations(pls_context* lead, pls_context* const* ctxs, const i
             ctx->stream = st;
             bool solved = false;
             try {
-                kdmap_icp_iteration(ctx, query_bounds[i], 0, 1, it, ctx->cfg.threshold_delta_pose, &solved);
+                kdmap_icp_iteration(ctx, query_bounds[i], nullptr, 0, 1, it, ctx->cfg.threshold_delta_pose, &solved);
             } catch (...) {
                 ctx->stream = own;
                 throw;

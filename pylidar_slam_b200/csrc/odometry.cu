@@ -37,11 +37,22 @@ int64_t shard_min_default() {
     return v;
 }
 
-__global__ void frame_begin_kernel(FrameResult* fr, const float* T0 /*16, device or null*/, int max_iters,
-                                   uint32_t* worklist_counts /*2*/) {
+struct Pose16 {
+    float m[16];
+};
+
+// The start of a frame's ICP.  The initial pose is T0_dev if given, else T0 (a kernel argument: no copy in front of the
+// kernel).  The frame's counts: the input stage wrote the low words of counts[1] (queries; copied from counts[2] here
+// when the queries are the valid rows themselves) and counts[2] (valid rows); every other word is cleared.
+__global__ void frame_begin_kernel(FrameResult* fr, const float* T0_dev /*16, or null*/, Pose16 T0, int max_iters,
+                                   uint32_t* worklist_counts /*16*/, int queries_are_rows) {
     int t = threadIdx.x;
     if (t < 16) worklist_counts[t] = 0;  // SC_KD_COUNTERS + SC_KD_LISTS: the kd search's counters and work lists
-    if (t < 16) fr->T[t] = T0 ? T0[t] : ((t % 5 == 0) ? 1.f : 0.f);
+    if (t < 16) fr->T[t] = T0_dev ? T0_dev[t] : T0.m[t];
+    uint32_t* cw = reinterpret_cast<uint32_t*>(fr->counts);  // word 2i: the low half of counts[i]
+    static_assert(sizeof(fr->counts) == 16 * sizeof(uint32_t), "counts: 8 words of 64 bits");
+    if (t < 16 && t != 2 && t != 4) cw[t] = 0u;
+    if (t == 2 && queries_are_rows) cw[2] = cw[4];
     if (t < 6) fr->params[t] = 0.f;
     if (t < kMaxAlign) fr->losses[t] = __int_as_float(0x7fc00000);
     if (t == 0) {
@@ -230,8 +241,8 @@ inline int grid_for(int64_t n, int threads = 256) {
 
 uint32_t* count_slot(pls_context* ctx, int i) { return reinterpret_cast<uint32_t*>(&frame_result_dev(ctx)->counts[i]); }
 
-// Enqueues ICP iterations [first, last) (icp_odometry.py:274-297).
-int enqueue_icp_iterations(pls_context* ctx, int64_t query_bound, int first, int last) {
+// Enqueues ICP iterations [first, last) (icp_odometry.py:274-297).  bound_dev: see kdmap_icp_iteration.
+int enqueue_icp_iterations(pls_context* ctx, int64_t query_bound, const uint32_t* bound_dev, int first, int last) {
     cudaStream_t st = ctx->stream;
     FrameResult* fr = frame_result_dev(ctx);
     int rank = comm_rank(ctx), size = comm_size(ctx);
@@ -240,6 +251,7 @@ int enqueue_icp_iterations(pls_context* ctx, int64_t query_bound, int first, int
     // same deterministic kernels, hence the same bits on every rank, and no exchange at all.  (The bound is a host
     // value every rank computes alike, so the ranks always take the same branch.)
     if (size > 1) {
+        PLS_REQUIRE(!bound_dev, "ICP: a device-side query bound cannot decide the sharding");
         const int64_t work = ctx->cfg.local_map_type == PLS_MAP_KDTREE ? query_bound : (int64_t)ctx->cfg.height * ctx->cfg.width;
         if (!icp_shards(ctx, work)) {
             rank = 0;
@@ -252,7 +264,8 @@ int enqueue_icp_iterations(pls_context* ctx, int64_t query_bound, int first, int
         int blocks;
         bool solved = false;  // the kd kernels finish the iteration themselves on a single GPU
         if (ctx->cfg.local_map_type == PLS_MAP_KDTREE)
-            blocks = kdmap_icp_iteration(ctx, query_bound, rank, size, it, size == 1 ? ctx->cfg.threshold_delta_pose : -1.f, &solved);
+            blocks = kdmap_icp_iteration(ctx, query_bound, bound_dev, rank, size, it,
+                                         size == 1 ? ctx->cfg.threshold_delta_pose : -1.f, &solved);
         else
             blocks = projmap_icp_iteration(ctx, query_bound, rank, size);
         last_blocks = blocks;
@@ -353,10 +366,13 @@ struct BatchTrace {
     }
 };
 
-// The start of a frame's ICP: the FrameResult at T0 (device, or null for the identity), the search counters cleared.
-void frame_begin(pls_context* ctx, const float* T0_dev) {
-    frame_begin_kernel<<<1, kMaxAlign, 0, ctx->stream>>>(frame_result_dev(ctx), T0_dev, ctx->cfg.max_num_alignments,
-                                                         scalar_u32(ctx, SC_KD_COUNTERS));
+// The start of a frame's ICP: the FrameResult at T0 (T0_dev on the device, else T0_host, else the identity), the search
+// counters cleared.
+void frame_begin(pls_context* ctx, const float* T0_host, const float* T0_dev, bool queries_are_rows) {
+    Pose16 T0;
+    for (int i = 0; i < 16; ++i) T0.m[i] = T0_host ? T0_host[i] : ((i % 5 == 0) ? 1.f : 0.f);
+    frame_begin_kernel<<<1, kMaxAlign, 0, ctx->stream>>>(frame_result_dev(ctx), T0_dev, T0, ctx->cfg.max_num_alignments,
+                                                         scalar_u32(ctx, SC_KD_COUNTERS), queries_are_rows ? 1 : 0);
     PLS_CHECK_LAUNCH();
 }
 
@@ -392,16 +408,16 @@ int icp_rounds(pls_context* const* ctxs, int num, Enqueue enqueue, ReadDone read
     return extra;
 }
 
-// The ICP loop of one frame over ctx->query_ptr / counts[1], on ctx->stream.  Returns the block count of the
+// The ICP loop of one frame over ctx->query_ptr / counts[1], on ctx->stream.  Returns the launched block count of the
 // correspondence kernel.
-int run_icp(pls_context* ctx, int64_t query_bound) {
+int run_icp(pls_context* ctx, int64_t query_bound, const uint32_t* bound_dev) {
     cudaStream_t st = ctx->stream;
     FrameResult* fr = frame_result_dev(ctx);
     if (query_bound < 1) query_bound = 1;
     ctx->pm.zbuf_clean = false;  // tmp[3] may have been used by the frame's own projection
     int blocks = 0;
     auto enqueue = [&](int first, int last) {
-        blocks = enqueue_icp_iterations(ctx, query_bound, first, last);
+        blocks = enqueue_icp_iterations(ctx, query_bound, bound_dev, first, last);
         if (first == 0) g_trace.lap(0);
     };
     auto read_done = [&](int* done) {
@@ -502,9 +518,9 @@ namespace {
 
 // What a frame's input stage hands to its ICP and its epilogue.
 struct FrameIn {
-    int64_t pts_bound = 0;    // rows of the frame's own points, NaN rows included
+    int64_t pts_bound = 0;    // rows of the frame's own points, NaN rows included (a bound of them, with n_dev)
     int64_t query_bound = 0;  // bound of the query count
-    const float* T0_dev = nullptr;
+    const uint32_t* n_dev = nullptr;  // the row count on the device, when the host knows only the bound pts_bound
 };
 
 // The caller's outputs of one frame, each nullable.
@@ -555,8 +571,10 @@ GridSample frame_grid_sample(pls_context* ctx, const void* raw, int64_t n, doubl
 // The input stage of a frame (icp_odometry.py:319-358, 301-308): input selection, the map-update flush and
 // frame_begin_kernel, on ctx->stream.  A sequence's first frame only initialises the map (icp_odometry.py:171-181): that
 // is done here, outputs included, and false returned.
-bool frame_input(pls_context* ctx, const void* data_void, int layout, int64_t n, const float* init_pose, FrameIn& in,
-                 const FrameOut& out) {
+// n_dev (nullable): the frame has *n_dev rows, a count still being computed on the device, and n is a bound of it; only
+// the fused selection of a float32 frame on the kd map after the first frame reads its rows from a device count.
+bool frame_input(pls_context* ctx, const void* data_void, int layout, int64_t n, const uint32_t* n_dev,
+                 const float* init_pose, FrameIn& in, const FrameOut& out) {
     cudaStream_t st = ctx->stream;
     // float64 point layouts: same flow, the cloud is rounded to float32 for the queries / map insertion while the frame's
     // own vertex map is projected in float64 (icp_odometry.py:331-352)
@@ -569,7 +587,6 @@ bool frame_input(pls_context* ctx, const void* data_void, int layout, int64_t n,
     const int64_t hw = (int64_t)H * W;
     const bool kd = ctx->cfg.local_map_type == PLS_MAP_KDTREE;
     FrameResult* fr = frame_result_dev(ctx);
-    PLS_CUDA(cudaMemsetAsync(fr->counts, 0, sizeof(fr->counts), st));
     if (layout == PLS_INPUT_NDARRAY) ctx->sample_pointcloud = 1;  // icp_odometry.py:330
     const bool first = ctx->frame_index == 0;
     // the previous frame's buffers may still feed the asynchronous map update: use the other pair
@@ -598,6 +615,7 @@ bool frame_input(pls_context* ctx, const void* data_void, int layout, int64_t n,
         pts_bound = n;
         // the shipped pipelines (float32 points, kd map, any frame but the first): one z-buffer pass and one selection
         fused_input = !is64 && kd && !first && n <= SEL_MAX_N && n < (1ll << 32);
+        PLS_REQUIRE(fused_input || !n_dev, "process_frame: a device-side row count needs the fused kd input stage");
         if (fused_input) {
             const bool pixel_queries = !ctx->sample_pointcloud;
             FrameInputSelect op;
@@ -613,12 +631,12 @@ bool frame_input(pls_context* ctx, const void* data_void, int layout, int64_t n,
                     PLS_CUDA(cudaMemsetAsync(ctx->input_zbuf.p, 0xff, (size_t)hw * sizeof(unsigned long long), st));
                 ctx->input_zbuf_clean = false;  // dirty until the selection below (whose winners reset their pixels) is enqueued
                 ctx->queries.reserve((size_t)(n < hw ? n : hw) * sizeof(float4), st);
-                launch_zbuf_points(ctx, data_dev, n, nullptr, H, W, ctx->cfg.up_fov_deg, ctx->cfg.down_fov_deg,
+                launch_zbuf_points(ctx, data_dev, n, n_dev, H, W, ctx->cfg.up_fov_deg, ctx->cfg.down_fov_deg,
                                    ctx->input_zbuf.as<unsigned long long>());
                 op.zbuf = ctx->input_zbuf.as<unsigned long long>();
                 op.queries = ctx->queries.as<float4>();
             }
-            select_launch(ctx, op, n, nullptr, count_slot(ctx, 2), pixel_queries ? count_slot(ctx, 1) : nullptr);
+            select_launch(ctx, op, n, n_dev, count_slot(ctx, 2), pixel_queries ? count_slot(ctx, 1) : nullptr);
             if (pixel_queries) ctx->input_zbuf_clean = true;
         } else if (is64) {
             pack_valid_rows_f64(ctx, data64, n, frame_pts.as<float4>(), count_slot(ctx, 2));
@@ -638,6 +656,7 @@ bool frame_input(pls_context* ctx, const void* data_void, int layout, int64_t n,
         }
     }
     in.pts_bound = pts_bound;
+    in.n_dev = n_dev;
 
     float eye[16];
     for (int i = 0; i < 16; ++i) eye[i] = (i % 5 == 0) ? 1.f : 0.f;
@@ -665,10 +684,10 @@ bool frame_input(pls_context* ctx, const void* data_void, int layout, int64_t n,
 
     // ---- sample_points (icp_odometry.py:301-308)
     int64_t query_bound;
-    if (ctx->sample_pointcloud && layout != PLS_INPUT_VERTEX_MAP) {
-        // queries = the (NaN-free) input points themselves
+    const bool queries_are_rows = ctx->sample_pointcloud && layout != PLS_INPUT_VERTEX_MAP;
+    if (queries_are_rows) {
+        // queries = the (NaN-free) input points themselves (frame_begin_kernel copies their count)
         ctx->query_ptr = frame_pts.as<float4>();
-        PLS_CUDA(cudaMemcpyAsync(count_slot(ctx, 1), count_slot(ctx, 2), sizeof(uint32_t), cudaMemcpyDeviceToDevice, st));
         query_bound = n;
     } else if (layout == PLS_INPUT_VERTEX_MAP) {
         ctx->query_ptr = ctx->tmp[5].as<float4>();
@@ -685,15 +704,9 @@ bool frame_input(pls_context* ctx, const void* data_void, int layout, int64_t n,
     in.query_bound = query_bound;
 
     // ---- register_new_frame
-    in.T0_dev = nullptr;
-    if (init_pose) {
-        ctx->tmp[6].reserve(16 * sizeof(float), st);
-        PLS_CUDA(cudaMemcpyAsync(ctx->tmp[6].p, init_pose, 16 * sizeof(float), cudaMemcpyHostToDevice, st));
-        in.T0_dev = ctx->tmp[6].as<float>();
-    }
     flush_map_update(ctx);  // (already enqueued by the grid-sample call of this frame, if there was one)
     map_stream_wait(ctx);   // the ICP below reads the local map the previous frame's update is still building
-    frame_begin(ctx, in.T0_dev);
+    frame_begin(ctx, init_pose, nullptr, queries_are_rows);
     return true;
 }
 
@@ -731,20 +744,50 @@ void frame_epilogue(pls_context* ctx, const FrameIn& in, const FrameOut& out, bo
     out.put_samples();
 }
 
-void process_frame_device(pls_context* ctx, const void* data_void, int layout, int64_t n, const float* init_pose,
-                          const FrameOut& out) {
+// One frame, enqueued in one go; the host waits once, for its result.  n_dev: see frame_input -- here it is the count of a
+// grid sample enqueued on compact keys, whose overflow stamp comes back with the result: if the keys overflowed, the
+// frame ran on a wrong sample, nothing is reported or advanced past the input stage, and false is returned for the
+// caller to roll back and replay.
+bool process_frame_device(pls_context* ctx, const void* data_void, int layout, int64_t n, const uint32_t* n_dev,
+                          const float* init_pose, FrameOut out) {
     g_trace.start();
     FrameIn in;
-    if (!frame_input(ctx, data_void, layout, n, init_pose, in, out)) return;
-    const int icp_blocks = run_icp(ctx, in.query_bound);
+    if (!frame_input(ctx, data_void, layout, n, n_dev, init_pose, in, out)) return true;
+    int icp_blocks = run_icp(ctx, in.query_bound, in.n_dev);
     fetch_result(ctx);
-    ctx->icp_result = true;
     g_trace.lap(1);
+    if (in.n_dev) {
+        bool overflowed = false;
+        const int64_t rows = grid_sample_host_count(ctx, &overflowed);
+        if (overflowed) return false;
+        in.pts_bound = rows;
+        out.samples = rows;
+        // the block count the correspondence kernels ran with (kd_logical_blocks)
+        const int64_t q = rows < in.query_bound ? rows : in.query_bound;
+        icp_blocks = grid_for(q < 1 ? 1 : q);
+    }
+    ctx->icp_result = true;
     credit_icp_profile(ctx, frame_result_host(ctx), icp_blocks);
     frame_epilogue(ctx, in, out, true);
     g_trace.lap(3);
     g_trace.end_frame();
+    return true;
 }
+
+// What a frame changes in its context before its result is known: the state a replayed frame starts again from.
+struct FrameEntryState {
+    int frame_slot, frame_index, last_icp_iters;
+    bool input_zbuf_clean;
+    explicit FrameEntryState(const pls_context* ctx)
+        : frame_slot(ctx->frame_slot), frame_index(ctx->frame_index), last_icp_iters(ctx->last_icp_iters),
+          input_zbuf_clean(ctx->input_zbuf_clean) {}
+    void restore(pls_context* ctx) const {
+        ctx->frame_slot = frame_slot;
+        ctx->frame_index = frame_index;
+        ctx->last_icp_iters = last_icp_iters;
+        ctx->input_zbuf_clean = input_zbuf_clean;
+    }
+};
 
 }  // namespace
 
@@ -811,8 +854,8 @@ int pls_register_frame(pls_context* ctx, const float* points, int64_t n, const f
                                  is_device_ptr(T0) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st));
         T0_dev = ctx->tmp[6].as<float>();
     }
-    frame_begin(ctx, T0_dev);
-    const int icp_blocks = run_icp(ctx, n);
+    frame_begin(ctx, nullptr, T0_dev, false);
+    const int icp_blocks = run_icp(ctx, n, nullptr);
     fetch_result(ctx);
     ctx->icp_result = true;
     FrameResult* h = frame_result_host(ctx);
@@ -837,7 +880,7 @@ int pls_process_frame(pls_context* ctx, const void* data, int layout, int64_t n,
     if (const char* why = frame_refusal(ctx, layout & ~(PLS_PTR_DEVICE | PLS_PTR_HOST), n, 0.0))
         throw pls::Error{PLS_E_INVALID, why};
     const void* d = stage_frame_input(ctx, data, &layout, n);
-    process_frame_device(ctx, d, layout, n, init_pose, FrameOut{out_pose, out_params, out_has_pose, out_info, -1});
+    process_frame_device(ctx, d, layout, n, nullptr, init_pose, FrameOut{out_pose, out_params, out_has_pose, out_info, -1});
     PLS_API_END(ctx)
 }
 
@@ -850,12 +893,29 @@ int pls_process_frame_grid_sample(pls_context* ctx, const float* raw_points, int
     PLS_REQUIRE(raw_points && n > 0 && voxel > 0.0, "pls_process_frame_grid_sample: bad arguments");
     if (const char* why = frame_refusal(ctx, layout, n, voxel)) throw pls::Error{PLS_E_INVALID, why};
     const void* d = to_device(ctx, raw_points, (size_t)n * 3 * sizeof(float), ctx->stage_in[0]);
-    // the sample count is needed on the host to size the point-layout frame: one small sync
     const GridSample g = frame_grid_sample(ctx, d, n, voxel);
-    grid_sample_enqueue(ctx, g);
-    PLS_CUDA(cudaStreamSynchronize(ctx->stream));
+    const FrameOut out{out_pose, out_params, out_has_pose, out_info, -1};
+    // After a kd map's first frame, on one GPU, the fused input stage reads the sample count on the device (the raw row
+    // count n bounds it): the frame is enqueued in one go, without waiting for the count.  The sharding decision of a
+    // multi-GPU context and every other input stage size their launches from the count on the host.
+    const bool deferred = ctx->frame_index > 0 && ctx->cfg.local_map_type == PLS_MAP_KDTREE && comm_size(ctx) == 1 &&
+                          n <= SEL_MAX_N;
+    if (deferred) {
+        const FrameEntryState entry(ctx);
+        grid_sample_enqueue(ctx, g, false);
+        if (process_frame_device(ctx, ctx->gs_out_xyz.p, layout, n, scalar_u32(ctx, SC_GS_COUNT), init_pose, out)) return PLS_OK;
+        // a hash overflowed the compact sort keys: the frame ran on a wrong sample and is run again from its entry state
+        // on the raw keys (this frame's map update is not enqueued yet; the cached normals stay valid for the index)
+        entry.restore(ctx);
+    } else {
+        grid_sample_enqueue(ctx, g);
+        PLS_CUDA(cudaStreamSynchronize(ctx->stream));
+    }
+    // the sample count on the host, which sizes the frame; on overflowed compact keys, once more on the raw keys
     const int64_t S = grid_sample_finish(ctx, g);
-    process_frame_device(ctx, ctx->gs_out_xyz.p, layout, S, init_pose, FrameOut{out_pose, out_params, out_has_pose, out_info, S});
+    FrameOut sized = out;
+    sized.samples = S;
+    process_frame_device(ctx, ctx->gs_out_xyz.p, layout, S, nullptr, init_pose, sized);
     PLS_API_END(ctx)
 }
 
@@ -970,7 +1030,8 @@ int pls_process_frames(pls_context* const* ctxs, int num, const void* const* dat
             pls_context* ctx = ctxs[i];
             bool runs_icp = false;
             try {
-                runs_icp = frame_input(ctx, dev[i], lay[i], rows[i], init_poses ? init_poses[i] : nullptr, in[i], outputs(i));
+                runs_icp = frame_input(ctx, dev[i], lay[i], rows[i], nullptr, init_poses ? init_poses[i] : nullptr, in[i],
+                                       outputs(i));
             } catch (const pls::Error& e) {
                 // an input the single path refuses (e.g. a grid sample of no point) is that sequence's error alone
                 if (e.code != PLS_E_INVALID) throw;

@@ -30,12 +30,17 @@ __device__ __forceinline__ void st_volatile_u32(uint32_t* p, uint32_t v) {
 }
 
 // Digit histograms of all passes in one read of the keys; the block that finishes last turns them into
-// exclusive bin offsets (one launch instead of histogram + scan).
+// exclusive bin offsets (one launch instead of histogram + scan).  Also clears the look-back words and tile counters
+// of the passes that follow (status_words of them).
 __global__ void __launch_bounds__(256) sort_hist_kernel(const uint64_t* __restrict__ keys, int64_t n,
                                                         int num_passes, uint32_t* __restrict__ hist,
-                                                        uint32_t* __restrict__ done_counter) {
+                                                        uint32_t* __restrict__ done_counter, uint32_t* __restrict__ status,
+                                                        int64_t status_words) {
     __shared__ uint32_t sh[8 * RADIX];
     __shared__ int s_last;
+    pls_grid_dependency_wait();
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < status_words; i += (int64_t)gridDim.x * blockDim.x)
+        status[i] = 0u;
     for (int i = threadIdx.x; i < num_passes * RADIX; i += blockDim.x) sh[i] = 0;
     __syncthreads();
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
@@ -81,6 +86,7 @@ sort_pass_kernel(const uint64_t* __restrict__ kin, const uint32_t* __restrict__ 
     __shared__ uint64_t s_keys[SORT_TILE];
     __shared__ uint32_t s_vals[SORT_TILE];
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    pls_grid_dependency_wait();
     if (tid == 0) s_tile = atomicAdd(tile_counter, 1u);
     for (int i = tid; i < SORT_WARPS * RADIX; i += SORT_THREADS) (&warp_hist[0][0])[i] = 0;
     __syncthreads();
@@ -293,23 +299,19 @@ void radix_sort_pairs(pls_context* ctx, uint64_t* keys, uint32_t* vals, int64_t 
     s.hist.reserve(hist_bytes, st);
     s.status.reserve(((size_t)num_passes * cap_tiles * RADIX + 8) * sizeof(uint32_t), st);
     PLS_CUDA(cudaMemsetAsync(s.hist.p, 0, hist_bytes, st));
-    PLS_CUDA(cudaMemsetAsync(s.status.p, 0, status_words * sizeof(uint32_t), st));
     // one block per SM at most: every block ends with num_passes * 256 global atomics
     int hist_blocks = (int)((n + 256 * 4 - 1) / (256 * 4));
     if (hist_blocks > kNumSMs) hist_blocks = kNumSMs;
-    sort_hist_kernel<<<hist_blocks, 256, 0, st>>>(keys, n, num_passes, s.hist.as<uint32_t>(),
-                                                  s.hist.as<uint32_t>() + 8 * RADIX);
-    PLS_CHECK_LAUNCH();
+    launch_dependent(sort_hist_kernel, hist_blocks, 256, st, keys, n, num_passes, s.hist.as<uint32_t>(),
+                     s.hist.as<uint32_t>() + 8 * RADIX, s.status.as<uint32_t>(), (int64_t)status_words);
     uint64_t* kin = keys;
     uint32_t* vin = vals;
     uint64_t* kout = s.keys_alt.as<uint64_t>();
     uint32_t* vout = s.vals_alt.as<uint32_t>();
     uint32_t* counters = s.status.as<uint32_t>() + (size_t)num_passes * tiles * RADIX;
     for (int p = 0; p < num_passes; ++p) {
-        sort_pass_kernel<<<(unsigned)tiles, SORT_THREADS, 0, st>>>(
-            kin, vin, kout, vout, n, 8 * p, s.hist.as<uint32_t>() + p * RADIX,
-            s.status.as<uint32_t>() + (size_t)p * tiles * RADIX, counters + p);
-        PLS_CHECK_LAUNCH();
+        launch_dependent(sort_pass_kernel, (unsigned)tiles, SORT_THREADS, st, kin, vin, kout, vout, n, 8 * p,
+                         s.hist.as<uint32_t>() + p * RADIX, s.status.as<uint32_t>() + (size_t)p * tiles * RADIX, counters + p);
         uint64_t* tk = kin; kin = kout; kout = tk;
         uint32_t* tv = vin; vin = vout; vout = tv;
     }

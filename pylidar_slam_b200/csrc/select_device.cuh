@@ -41,6 +41,7 @@ select_kernel(Op op, int64_t n, const uint32_t* __restrict__ n_dev, unsigned lon
               uint32_t* __restrict__ total0, uint32_t* __restrict__ total1) {
     __shared__ uint32_t warp_sums[2][SEL_THREADS / 32];
     __shared__ uint32_t s_excl[2];
+    pls_grid_dependency_wait();
     if (n_dev) n = min(n, (int64_t)*n_dev);
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const uint32_t tile = blockIdx.x;
@@ -140,8 +141,8 @@ void select_launch(pls_context* ctx, const Op& op, int64_t n, const uint32_t* n_
         PLS_CUDA(cudaMemsetAsync(s.status.p, 0, need, st));
         s.epoch = 1;
     }
-    select_kernel<Op><<<(unsigned)tiles, SEL_THREADS, 0, st>>>(op, n, n_dev, s.status.as<unsigned long long>(), s.epoch, total0, total1);
-    PLS_CHECK_LAUNCH();
+    launch_dependent(select_kernel<Op>, (unsigned)tiles, SEL_THREADS, st, op, n, n_dev, s.status.as<unsigned long long>(), s.epoch,
+                     total0, total1);
 }
 
 }  // namespace pls
