@@ -216,6 +216,12 @@ PLS_API int pls_kdmap_nn_search(pls_context* ctx, const float* queries, int64_t 
  * run, if the map was rebuilt since, or if the last ICP split its queries over several ranks. */
 PLS_API int pls_kdmap_last_correspondences(pls_context* ctx, int64_t n, int64_t* out_idx, float* out_neighbors,
                                            float* out_normals, float* out_search_state, double* out_sums);
+/* Test / debug aid: the exact (k+1)-NN lists of the normals search (0 <= k <= 31) for n arbitrary query rows [n,3]
+ * on the current index, ordered by (float32 squared distance, sorted position).  out_idx [n,k+1] insertion index or -1
+ * past the map's size; out_d2 [n,k+1] the float32 squared distance (NaN where out_idx is -1); out_pos [n,k+1] the
+ * position in the Morton-sorted point array or -1 (nullable).  Touches neither the normal cache nor any ICP state. */
+PLS_API int pls_kdmap_knn(pls_context* ctx, const float* queries, int64_t n, int k, int64_t* out_idx, float* out_d2,
+                          int32_t* out_pos);
 /* ProjectiveLocalMap.update (local_map.py:126-202): rel_pose [16]; vertex_map [3,H,W] or NULL. */
 PLS_API int pls_projmap_update(pls_context* ctx, const float* rel_pose, const float* vertex_map);
 PLS_API int pls_projmap_num_frames(pls_context* ctx, int* num_frames);

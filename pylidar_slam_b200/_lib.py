@@ -69,6 +69,7 @@ _SIGNATURES = {
     "pls_kdmap_points": [_P, _P],
     "pls_kdmap_nn_search": [_P, _P, _L, _P, _P, _P],
     "pls_kdmap_last_correspondences": [_P, _L, _P, _P, _P, _P, _P],
+    "pls_kdmap_knn": [_P, _P, _L, _I, _P, _P, _P],
     "pls_projmap_update": [_P, _P, _P],
     "pls_projmap_num_frames": [_P, C.POINTER(_I)],
     "pls_projmap_model": [_P, _P, _P],

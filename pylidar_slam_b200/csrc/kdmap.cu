@@ -827,6 +827,34 @@ __global__ void kd_search_export_kernel(KdIndex ix, const int* __restrict__ matc
     }
 }
 
+// pls_kdmap_knn: the (K)-NN list warp_knn gives each of n query rows [n,3], a warp per query.  Row r of the outputs,
+// entry j < K: insertion index (.w of `sorted`) or -1, the float32 squared distance of the key, the sorted position.
+__global__ void __launch_bounds__(KD_THREADS)
+kd_knn_export_kernel(KdIndex ix, const float* __restrict__ rows, int64_t n, int K, long long* __restrict__ out_idx,
+                     float* __restrict__ out_d2, int* __restrict__ out_pos) {
+    __shared__ unsigned long long s_stage[KD_WARPS][KNN_STAGE];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const KdGridLocal g = kd_load_grid(ix);
+    const float nan = __int_as_float(0x7fc00000);
+    for (int64_t q = (int64_t)blockIdx.x * KD_WARPS + warp; q < n; q += (int64_t)gridDim.x * KD_WARPS) {
+        const float x = rows[3 * q], y = rows[3 * q + 1], z = rows[3 * q + 2];
+        int pos;
+        warp_knn(ix, g, x, y, z, K, lane, pos, nullptr, s_stage[warp]);
+        if (lane < K) {
+            long long idx = -1;
+            float d2 = nan;
+            if (pos >= 0) {
+                const float4 s = __ldg(ix.sorted + pos);
+                idx = (long long)__float_as_uint(s.w);
+                d2 = dist2_point(x, y, z, s);
+            }
+            out_idx[q * K + lane] = idx;
+            out_d2[q * K + lane] = d2;
+            if (out_pos) out_pos[q * K + lane] = pos;
+        }
+    }
+}
+
 size_t cell_table_bytes(int64_t M, uint32_t* masks, size_t* offsets) {
     size_t off = 0;
     for (int l = 0; l < KD_MAX_LEVELS; ++l) {
@@ -1369,6 +1397,29 @@ int pls_kdmap_nn_search(pls_context* ctx, const float* queries, int64_t n, float
     finish_out(ctx, onb);
     finish_out(ctx, onr);
     finish_out(ctx, oix);
+    PLS_CUDA(cudaStreamSynchronize(ctx->stream));
+    PLS_API_END(ctx)
+}
+
+int pls_kdmap_knn(pls_context* ctx, const float* queries, int64_t n, int k, int64_t* out_idx, float* out_d2,
+                  int32_t* out_pos) {
+    PLS_API_BEGIN(ctx)
+    map_stream_wait(ctx);
+    PLS_REQUIRE(queries && out_idx && out_d2 && n > 0, "pls_kdmap_knn: bad arguments");
+    PLS_REQUIRE(k >= 0 && k + 1 <= KD_KMAX, "pls_kdmap_knn: k must be in [0, 31]");
+    if (!ctx->kd.valid) throw pls::Error{PLS_E_STATE, "pls_kdmap_knn: the map is empty"};
+    const int K = k + 1;
+    const size_t entries = (size_t)n * K;
+    const float* d = (const float*)to_device(ctx, queries, (size_t)n * 3 * sizeof(float), ctx->stage_in[0]);
+    OutArg oix = out_arg(ctx, out_idx, entries * sizeof(int64_t), ctx->stage_out[0]);
+    OutArg od2 = out_arg(ctx, out_d2, entries * sizeof(float), ctx->stage_out[1]);
+    OutArg ops = out_arg(ctx, out_pos, entries * sizeof(int32_t), ctx->stage_out[2]);
+    kd_knn_export_kernel<<<grid_for(n, KD_THREADS / 32, 8 * kNumSMs), KD_THREADS, 0, ctx->stream>>>(
+        make_index(ctx), d, n, K, (long long*)oix.dev, (float*)od2.dev, (int*)ops.dev);
+    PLS_CHECK_LAUNCH();
+    finish_out(ctx, oix);
+    finish_out(ctx, od2);
+    finish_out(ctx, ops);
     PLS_CUDA(cudaStreamSynchronize(ctx->stream));
     PLS_API_END(ctx)
 }

@@ -21,6 +21,7 @@ def test_library_builds_and_exports_every_declared_symbol():
     lib = ctypes.CDLL(path)
     declared = _declared()
     assert len(declared) >= 30
+    assert "pls_kdmap_knn" in declared  # the test aid of the normals' neighbour lists
     for name in declared:
         assert hasattr(lib, name), f"{name} declared in the header but not exported"
     assert sorted(_lib.exported_symbols()) == declared, "ctypes signature table and header disagree"

@@ -73,8 +73,8 @@ def scene():
 
 
 # ---------------------------------------------------------------------------------------------------------- driving
-def _context(lib, iters, scheme="geman_mcclure", sigma=0.3):
-    return lib.Context(local_map_type=lib.MAP_KDTREE, local_map_size=1, num_neighbors_normals=K_NORMALS,
+def _context(lib, iters, scheme="geman_mcclure", sigma=0.3, k=K_NORMALS):
+    return lib.Context(local_map_type=lib.MAP_KDTREE, local_map_size=1, num_neighbors_normals=k,
                        scheme=lib.SCHEMES[scheme], sigma=sigma, gn_max_iters=1, max_num_alignments=iters,
                        threshold_delta_pose=0.0)
 
@@ -99,11 +99,11 @@ def _register(lib, ctx, q, T0, iters):
     return dict(T=T.reshape(4, 4), params=params, losses=losses, **_readback(lib, ctx, q.shape[0]))
 
 
-def _runs(lib, m, q, T0, iters, scheme="geman_mcclure", sigma=0.3):
+def _runs(lib, m, q, T0, iters, scheme="geman_mcclure", sigma=0.3, k=K_NORMALS):
     """runs[j - 1] = register call with max_num_alignments = j on a fresh context holding map m."""
     runs = []
     for j in range(1, iters + 1):
-        ctx = _context(lib, j, scheme, sigma)
+        ctx = _context(lib, j, scheme, sigma, k)
         _insert(lib, ctx, m)
         runs.append(_register(lib, ctx, q, T0, j))
         ctx.close()
@@ -112,9 +112,9 @@ def _runs(lib, m, q, T0, iters, scheme="geman_mcclure", sigma=0.3):
     return runs
 
 
-def _fresh_normals(lib, m, idx):
+def _fresh_normals(lib, m, idx, k=K_NORMALS):
     """Normals kd_normals_warp_kernel computes at the map points idx, in a fresh context (nn_search of the points)."""
-    ctx = _context(lib, 1)
+    ctx = _context(lib, 1, k=k)
     _insert(lib, ctx, m)
     pts = np.ascontiguousarray(m[idx])
     nb, nrm = np.empty_like(pts), np.empty_like(pts)
@@ -125,6 +125,18 @@ def _fresh_normals(lib, m, idx):
 
 
 # ----------------------------------------------------------------------------------------------------------- checks
+_POSITIONS = {}
+
+
+def _positions(m):
+    """kernel_sort_positions of map m (cached by the map's bytes)."""
+    from oracle import kd_icp_reference
+    key = (m.shape, hash(m.tobytes()))
+    if key not in _POSITIONS:
+        _POSITIONS[key] = kd_icp_reference.kernel_sort_positions(m)
+    return _POSITIONS[key]
+
+
 def _pose64(T):
     return np.asarray(T, np.float64).reshape(4, 4)
 
@@ -136,7 +148,7 @@ def _euler_round_trip(T):
     return orc.build_pose_matrix(prm)[0].numpy(), prm[0].numpy()
 
 
-def _check_iteration(ref, m, tree, q, T_lin, run, scheme, sigma, min_normals_ok=0.9, tag=""):
+def _check_iteration(ref, m, tree, q, T_lin, run, scheme, sigma, min_normals_ok=0.9, tag="", k=K_NORMALS):
     """Iteration linearised at the float32 pose T_lin, read back in `run`.  Returns the distinct matched indices."""
     n = q.shape[0]
     T64 = _pose64(T_lin)
@@ -164,16 +176,27 @@ def _check_iteration(ref, m, tree, q, T_lin, run, scheme, sigma, min_normals_ok=
     assert bad.sum() == 0, (tag, "runner-up bounds above the runner-up", int(bad.sum()),
                             float((np.sqrt(st[:, 3]) - d_other)[bad].max()))
 
-    # 3. normals of every distinct matched point: the test_a9 bound against exact float64 normals
+    # 3. normals of every distinct matched point: the test_a9 bound against exact float64 normals, and, where the
+    # point's (k+1)-NN list is not ambiguous in float32, tight_normal_bound against the float64 eigenvector of the
+    # reference's float32 moments over that list (whichever kernel computed the normal: normals or refine kernel)
     u, first = np.unique(idx, return_index=True)
     gn = run["nrm"][first].astype(np.float64)
     assert np.abs(np.linalg.norm(gn, axis=1) - 1).max() <= 1e-6, tag
-    nr, gap, uniq = ref.exact_normals(m, tree, u, K_NORMALS)
+    nr, gap, uniq = ref.exact_normals(m, tree, u, k)
     sin = np.linalg.norm(np.cross(gn, nr), axis=1)
     ok = uniq & (gap > 1e-3)
     assert ok.mean() >= min_normals_ok, (tag, ok.mean())
     bad = sin[ok] > 2e-5 / gap[ok] + 2e-7
     assert bad.sum() == 0, (tag, "normals off the a9 bound", int(bad.sum()))
+    lists, _, _, amb = ref.knn_lists(m, m[u], k, _positions(m), tree)
+    covs = ref.reference_covs(m, u, lists, k).astype(np.float64)
+    v = np.linalg.eigh(covs)[1][:, :, 0]
+    bound, tgap = ref.tight_normal_bound(covs)
+    tsin = np.linalg.norm(np.cross(gn, v), axis=1)
+    sure = ~amb & (tgap > 1e-9)
+    assert sure.mean() >= min_normals_ok, (tag, sure.mean())
+    assert (tsin[sure] <= bound[sure]).all(), (tag, "normals off the tight bound", int((tsin[sure] > bound[sure]).sum()),
+                                               float((tsin[sure] / bound[sure]).max()))
 
     # 4. accumulators: float64 sums of the GPU's own correspondences (its matches, its normals) within the float32
     # rounding of r, |p - q| and p x n (8 ulp of |p| + |q|) plus 1e-6 of sum |term|
@@ -206,17 +229,18 @@ def _check_pose_update(ref, T_lin, run, j):
     assert np.abs(run["params"] - prm).max() <= 2e-6 * scale
 
 
-def _check_runs(lib, ref, m, tree, q, T0, runs, scheme="geman_mcclure", sigma=0.3, min_normals_ok=0.9, tag=""):
+def _check_runs(lib, ref, m, tree, q, T0, runs, scheme="geman_mcclure", sigma=0.3, min_normals_ok=0.9, tag="",
+                k=K_NORMALS):
     """Every check on every iteration; returns per iteration the set of distinct matched points."""
     matched = []
     for j, run in enumerate(runs, start=1):
         T_lin = T0 if j == 1 else runs[j - 2]["T"]
-        matched.append(_check_iteration(ref, m, tree, q, T_lin, run, scheme, sigma, min_normals_ok, f"{tag} it {j}"))
+        matched.append(_check_iteration(ref, m, tree, q, T_lin, run, scheme, sigma, min_normals_ok, f"{tag} it {j}", k))
         _check_pose_update(ref, T_lin, run, j)
     # normals computed in later iterations (inside the refine kernel or by the normals kernel) are the bits a fresh
     # context's nn_search computes at the same map points
     every = np.unique(np.concatenate(matched))
-    fresh = _fresh_normals(lib, m, every)
+    fresh = _fresh_normals(lib, m, every, k)
     for j, (run, u) in enumerate(zip(runs, matched), start=1):
         rows = np.searchsorted(every, u)
         first = np.unique(run["idx"], return_index=True)[1]
@@ -230,9 +254,19 @@ def _first_matched_late(matched):
 
 
 # -------------------------------------------------------------------------------------------------------- scenarios
+_CFG2_RUNS = {}
+
+
+def _cfg2_runs(lib, scene, k):
+    """The cfg2 scenario's six register calls at num_neighbors_normals = k."""
+    if k not in _CFG2_RUNS:
+        _CFG2_RUNS[k] = _runs(lib, scene["m"], scene["q"], scene["T0"], 6, k=k)
+    return _CFG2_RUNS[k]
+
+
 @pytest.fixture(scope="module")
 def cfg2_runs(lib, scene):
-    return _runs(lib, scene["m"], scene["q"], scene["T0"], 6)
+    return _cfg2_runs(lib, scene, K_NORMALS)
 
 
 def test_cfg2_six_iterations_refine_kernel(lib, ref, scene, cfg2_runs):
@@ -242,6 +276,18 @@ def test_cfg2_six_iterations_refine_kernel(lib, ref, scene, cfg2_runs):
     changed = max(np.mean(a["idx"] != b["idx"]) for a, b in zip(cfg2_runs[:-1], cfg2_runs[1:]))
     assert changed >= 0.01, changed                       # later iterations really re-search
     assert len(_first_matched_late(matched)) >= 100       # ... and compute new normals
+
+
+@pytest.mark.parametrize("k", [3, 31])
+def test_cfg2_six_iterations_refine_kernel_at_other_k(lib, ref, scene, k):
+    """The cfg2 scenario with the fewest and the most normal neighbours the map accepts: the normals of iterations 2-6
+    come from kd_icp_refine_kernel's own (k+1)-NN searches and meet the tight bound like the first iteration's."""
+    runs = _cfg2_runs(lib, scene, k)
+    matched = _check_runs(lib, ref, scene["m"], scene["tree"], scene["q"], scene["T0"], runs, tag=f"cfg2 k={k}", k=k)
+    assert len(_first_matched_late(matched)) >= 100
+    # the normals differ from those at k = 10: the context's k reached the kernels
+    base = _cfg2_runs(lib, scene, K_NORMALS)[0]
+    assert not np.array_equal(runs[0]["nrm"], base["nrm"])
 
 
 @pytest.mark.parametrize("scheme", SCHEMES)
@@ -261,7 +307,7 @@ def test_refine_kernel_rounds_beyond_the_first(lib, ref, scene):
     assert (runs[1]["idx"][late] != runs[0]["idx"][late]).any()   # the second round had matches to change
 
 
-def _filler(scene, runs, need, seed=5):
+def _filler(scene, runs, need, seed=5, k=K_NORMALS):
     """Points strictly inside the scene map's bounding box, clear of every query (at every pose the runs linearised
     at) by more than its match distance and of every matched point by more than its 11th neighbour: they change no
     match and no normal."""
@@ -275,7 +321,7 @@ def _filler(scene, runs, need, seed=5):
         centres.append(p)
         radii.append(d1 * 1.001 + 0.01)
     matched = np.unique(np.concatenate([r["idx"] for r in runs]))
-    r12, _ = tree.query(m64[matched], k=K_NORMALS + 2, workers=-1)
+    r12, _ = tree.query(m64[matched], k=k + 2, workers=-1)
     centres.append(m64[matched])
     radii.append(r12[:, -1] * 1.001 + 0.01)
     centres, radii = np.concatenate(centres), np.concatenate(radii)
@@ -302,13 +348,22 @@ def test_four_launch_path_on_a_filled_map(lib, ref, scene, cfg2_runs):
     as verify / queued 1-NN / normals / residual, and give the bits the refine kernel gives on the unfilled map (the
     same bounding box keeps the quantisation and the relative sorted order of the scene points, so ties resolve
     alike)."""
+    _four_launch_path(lib, ref, scene, cfg2_runs, K_NORMALS)
+
+
+def test_four_launch_path_on_a_filled_map_at_k31(lib, ref, scene):
+    """The same with 31 normal neighbours: the filler keeps clear of every matched point's 32nd neighbour."""
+    _four_launch_path(lib, ref, scene, _cfg2_runs(lib, scene, 31), 31)
+
+
+def _four_launch_path(lib, ref, scene, cfg2_runs, k):
     m = scene["m"]
     unfilled = cfg2_runs[:4]
-    fill, centres, radii = _filler(scene, unfilled, COLD_MAP_POINTS - m.shape[0] + 1000)
+    fill, centres, radii = _filler(scene, unfilled, COLD_MAP_POINTS - m.shape[0] + 1000, k=k)
     big = np.ascontiguousarray(np.concatenate([m, fill]))
     assert big.shape[0] >= COLD_MAP_POINTS
     assert (big.min(0) == m.min(0)).all() and (big.max(0) == m.max(0)).all()
-    runs = _runs(lib, big, scene["q"], scene["T0"], 4)
+    runs = _runs(lib, big, scene["q"], scene["T0"], 4, k=k)
     for j, (a, b) in enumerate(zip(runs, unfilled), start=1):
         for key in ("T", "params", "losses", "idx", "nrm", "sums"):
             assert a[key].tobytes() == b[key].tobytes(), (j, key)
@@ -316,7 +371,7 @@ def test_four_launch_path_on_a_filled_map(lib, ref, scene, cfg2_runs):
     ftree = cKDTree(fill.astype(np.float64))
     df, _ = ftree.query(centres, k=1, workers=-1)
     assert (df > radii).all()
-    _check_runs(lib, ref, big, cKDTree(big.astype(np.float64)), scene["q"], scene["T0"], runs, tag="filled")
+    _check_runs(lib, ref, big, cKDTree(big.astype(np.float64)), scene["q"], scene["T0"], runs, tag=f"filled k={k}", k=k)
 
 
 def test_later_iterations_across_an_overflowed_level(lib, ref):

@@ -234,6 +234,22 @@ def test_sequences_at_different_phases(lib):
     pair.finish()
 
 
+def test_sequences_with_different_normal_neighbour_counts(lib):
+    """k = 3, 10 and 31 normal neighbours in one call: the normals and refine kernels read each sequence's own k from
+    its descriptor.  All three run the same frames, so their normals must differ from one another."""
+    ks = (3, 10, 31)
+    pair = Pair(lib, 3, per_seq=[dict(num_neighbors_normals=k) for k in ks])
+    for k in range(16):
+        f = sampled(k)
+        pair.step([Frame(lib, kind, f) for kind in ("tensor", "ndarray", "tensor")], tag=k)
+        if k == 1:
+            nq = int(pair.outs[0]["info"][2])
+            nrm = [readback(lib, c, nq)[1]["nrm"] for c in pair.bat]
+            assert all(not np.array_equal(nrm[i], nrm[j]) for i, j in ((0, 1), (0, 2), (1, 2)))
+    assert all(len(it) == 16 for it in pair.iters) and max(max(it) for it in pair.iters) >= 2, pair.iters
+    pair.finish()
+
+
 def test_iteration_spread_and_extra_rounds(lib):
     """Sequence 0 takes every third frame and starts from the identity on odd steps: more iterations than the previous
     frame's count + 1, beside a sequence that converges in one or two."""
