@@ -304,6 +304,19 @@ PLS_API int pls_voxel_statistics(pls_context* ctx, const void* xyz, int is_f64, 
 PLS_API int pls_align_p2point(pls_context* ctx, const void* ref, const void* tgt, int64_t n, int is_f64, int scheme,
                       double sigma, int max_iters, double norm_stop, const void* x0, void* out_dT, void* out_x,
                       void* out_loss);
+/* The two alignments on a batch of `batch` correspondence sets of n points each, in one call: ref/tgt/nrm
+ * [batch,n,3], x0 [batch,6] or NULL, out_dT [batch,16], out_x [batch,6], out_loss [batch,n] or NULL, out_iters
+ * (host int, nullable) the iterations executed.  GaussNewton.compute's batch semantics (optimization.py:318-341):
+ * every iteration works on all elements; the tiny-residual guard takes the norm of all batch*n residuals
+ * (PLS_W_TINY_RESIDUAL, every x unchanged), one element with |det H| < 1e-7 fails the call (PLS_E_SINGULAR), and
+ * all elements stop together once |dx| over all batch*6 increments is below norm_stop.  pls_align_p2plane /
+ * pls_align_p2point are this call at batch 1. */
+PLS_API int pls_align_p2plane_batch(pls_context* ctx, const void* ref, const void* tgt, const void* nrm, int64_t batch,
+                                    int64_t n, int is_f64, int scheme, double sigma, int max_iters, double norm_stop,
+                                    const void* x0, void* out_dT, void* out_x, void* out_loss, int* out_iters);
+PLS_API int pls_align_p2point_batch(pls_context* ctx, const void* ref, const void* tgt, int64_t batch, int64_t n,
+                                    int is_f64, int scheme, double sigma, int max_iters, double norm_stop,
+                                    const void* x0, void* out_dT, void* out_x, void* out_loss, int* out_iters);
 /* weighted_procrustes, numpy path (slam/common/registration.py:15-76): rigid T (float64 [16]) with
  * T * tgt ~ ref.  tgt / ref [n,3] and weights [n] (nullable) share one dtype; the weights only enter the centroids. */
 PLS_API int pls_weighted_procrustes(pls_context* ctx, const void* tgt, const void* ref, const void* weights, int64_t n,

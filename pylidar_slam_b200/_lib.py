@@ -55,6 +55,8 @@ _SIGNATURES = {
     "pls_distort": [_P, _P, _I, _P, _I, _L, _P, _I, _P],
     "pls_voxel_statistics": [_P, _P, _I, _L, _D, _P, _P, _P, _P, _P, _P, C.POINTER(_L)],
     "pls_align_p2point": [_P, _P, _P, _L, _I, _I, _D, _I, _D, _P, _P, _P, _P],
+    "pls_align_p2plane_batch": [_P, _P, _P, _P, _L, _L, _I, _I, _D, _I, _D, _P, _P, _P, _P, _P],
+    "pls_align_p2point_batch": [_P, _P, _P, _L, _L, _I, _I, _D, _I, _D, _P, _P, _P, _P, _P],
     "pls_weighted_procrustes": [_P, _P, _P, _P, _L, _I, _P],
     "pls_p2plane_loss": [_P, _P, _P, _P, _P, _P, _I, _I, _I, _F, _F, _I, _F, _P, _P, _P, _P],
     "pls_kitti_correct_scan": [_P, _P, _L, _I, _P],

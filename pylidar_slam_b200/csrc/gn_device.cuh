@@ -1,10 +1,11 @@
 // Per-correspondence device math of the point-to-plane Gauss-Newton step, shared by the
 // stand-alone alignment kernel (gn.cu) and the fused correspondence+reduction kernels
-// (kdmap.cu, projmap.cu).
+// (kdmap.cu, projmap.cu); and the joint rules of the stand-alone alignment's batched solve.
 #pragma once
 #include <cuda_runtime.h>
 
 #include "../../include/plslam_b200.h"
+#include "pose_device.cuh"
 
 namespace pls {
 
@@ -149,6 +150,85 @@ __device__ __forceinline__ void block_reduce_store(double* acc, double* out) {
 #pragma unroll
         for (int w = 0; w < WARPS; ++w) s += red[w][threadIdx.x];
         out[threadIdx.x] = s;
+    }
+}
+
+// ---- the joint rules of a batched Gauss-Newton iteration (optimization.py:318-341) -----------------------------------
+// GaussNewton.compute treats the B elements of a batch as one problem: the tiny-residual guard looks at the norm of all
+// B*N residuals, one singular element fails the whole call, and the stop test looks at the norm of all B*6 increments.
+// Each element's own 6x6 solve is a GnStep; the functions below turn the B steps into the joint decision and apply it.
+// They are shared by gn_solve_kernel (gn.cu) and the host harness of the CPU tests.
+
+struct GnStep {          // one element's solve: H dx = -g, det H, and its sum of unweighted r^2
+    double dx[6];
+    double det;
+    double r2;
+};
+
+struct GnHead {          // the batch-wide state of one alignment call
+    double dx_norm;      // |dx| over all elements of the last applied step
+    int done;            // latched: later iterations are no-ops
+    int status;          // PLS_OK, PLS_W_TINY_RESIDUAL or PLS_E_SINGULAR
+    int iters;           // iterations executed
+    unsigned ticket;     // blocks of the current solve launch that have finished their elements
+};
+
+struct GnJoint {         // joint sums: sum r^2 over B*N residuals, sum dx^2 over B*6 increments (as stored in T)
+    double r2;
+    double dx2;
+    int singular;
+};
+
+// Adds elements first, first + stride, ... < batch to j, in that order.
+template <typename T>
+__host__ __device__ inline void gn_joint_reduce(const GnStep* steps, int64_t batch, int64_t first, int64_t stride,
+                                                GnJoint& j) {
+    for (int64_t b = first; b < batch; b += stride) {
+        const GnStep& s = steps[b];
+        j.r2 += s.r2;
+        double e = 0.0;
+        for (int i = 0; i < 6; ++i) {
+            const T d = (T)s.dx[i];
+            e += (double)d * (double)d;
+        }
+        j.dx2 += e;
+        if (!(fabs(s.det) >= 1e-7)) j.singular = 1;
+    }
+}
+
+__host__ __device__ inline void gn_joint_merge(GnJoint& a, const GnJoint& b) {
+    a.r2 += b.r2;
+    a.dx2 += b.dx2;
+    a.singular |= b.singular;
+}
+
+// The reference's order: tiny residual (warn, x unchanged), then any singular element (raise), then the update and the
+// joint stop test.  Returns the status of this iteration; only PLS_OK lets gn_joint_apply move x.
+template <typename T>
+__host__ __device__ inline int gn_joint_decide(GnHead* head, const GnJoint& j, T norm_stop) {
+    head->iters += 1;
+    int status = PLS_OK;
+    if (sqrt(j.r2) < 1e-7) status = PLS_W_TINY_RESIDUAL;
+    else if (j.singular) status = PLS_E_SINGULAR;
+    if (status != PLS_OK) {
+        head->status = status;
+        head->done = 1;
+        return status;
+    }
+    head->dx_norm = sqrt(j.dx2);
+    if (head->dx_norm < (double)norm_stop) head->done = 1;
+    return status;
+}
+
+// Elements first, first + stride, ...: x += (T)dx when the step is taken (status PLS_OK), and dT = pose(x).
+template <typename T>
+__host__ __device__ inline void gn_joint_apply(const GnStep* steps, int64_t batch, int64_t first, int64_t stride,
+                                               int status, T* x /*[B,6]*/, T* dT /*[B,16]*/) {
+    for (int64_t b = first; b < batch; b += stride) {
+        T* xb = x + 6 * b;
+        if (status == PLS_OK)
+            for (int i = 0; i < 6; ++i) xb[i] = xb[i] + (T)steps[b].dx[i];
+        build_pose(xb, dT + 16 * b);
     }
 }
 

@@ -255,14 +255,26 @@ class GaussNewtonPointToPlaneConfig(RigidAlignmentConfig):
     gauss_newton_config: Dict[str, Any] = field(default_factory=lambda: dict(max_iters=1))
 
 
-def _reject_mask(mask, n):
-    """`mask` of RigidAlignment.align ([1,n,1], alignment.py:96-121,158-182).  The reference cannot apply one: its cost
+def _reject_mask(mask, b, n):
+    """`mask` of RigidAlignment.align ([b,n,1], alignment.py:96-121,158-182).  The reference cannot apply one: its cost
     functions multiply the [b,n,6] Jacobian IN PLACE by `mask.unsqueeze(1)` ([b,1,n,1]; optimization.py:391-392,500-501),
     which fails to broadcast -- every call with a mask ends in a RuntimeError.  Same error type here, after the
     reference's own shape check."""
-    check_tensor(mask, [1, n, 1])
-    raise RuntimeError(f"output with shape [1, {n}, 6] doesn't match the broadcast shape [1, 1, {n}, 6] "
+    check_tensor(mask, [b, n, 1])
+    raise RuntimeError(f"output with shape [{b}, {n}, 6] doesn't match the broadcast shape [{b}, {b}, {n}, 6] "
                        f"(the reference's alignments cannot apply a mask: optimization.py:391-392, 500-501)")
+
+
+def _initial_params(pose, x0, b, is64, conv):
+    """initial_estimate as [b,6] parameters: given as parameters, or as [b,4,4] float32 pose matrices (alignment.py:110-118)."""
+    x0 = conv(x0)
+    if x0.ndim == 3:
+        check_tensor(x0, [b, 4, 4])
+        assert_debug(not is64, "pose-matrix initial estimates are float32")
+        x0 = pose.from_pose_matrix(x0)
+    assert_debug((x0.size if isinstance(x0, np.ndarray) else x0.numel()) == 6 * b,
+                 f"initial_estimate must be [{b},6] parameters or [{b},4,4] pose matrices")
+    return conv(x0.reshape(b, 6))
 
 
 def _gn_settings(gn_cfg) -> dict:
@@ -297,13 +309,16 @@ class GaussNewtonPointToPlaneAlignment(RigidAlignment):
         return self._ctx or default_context()
 
     def align(self, ref_points, tgt_points, ref_normals=None, initial_estimate=None, mask=None, **kwargs):
+        """[B,N,3] points and normals (numpy or torch, host or CUDA, float32 or float64), initial_estimate [B,6] or
+        [B,4,4] -> (dT [B,4,4], x [B,6], (w r)^2 [B,N]).  B > 1 aligns the batch in one call (pls_align_p2plane_batch)
+        with GaussNewton.compute's joint guards and stop test (optimization.py:318-341)."""
         assert_debug(ref_normals is not None, "The argument 'ref_normals' is required for a point to plane alignemnt")
-        check_tensor(tgt_points, [1, -1, 3])
-        n = tgt_points.shape[1]
+        check_tensor(tgt_points, [-1, -1, 3])
+        b, n = tgt_points.shape[0], tgt_points.shape[1]
         if mask is not None:
-            _reject_mask(mask, n)
-        check_tensor(ref_points, [1, n, 3])
-        check_tensor(ref_normals, [1, n, 3])
+            _reject_mask(mask, b, n)
+        check_tensor(ref_points, [b, n, 3])
+        check_tensor(ref_normals, [b, n, 3])
         is_np = isinstance(tgt_points, np.ndarray)
         is64 = (tgt_points.dtype == (np.float64 if is_np else torch.float64))
         dt_np, dt_t = (np.float64, torch.float64) if is64 else (np.float32, torch.float32)
@@ -311,16 +326,16 @@ class GaussNewtonPointToPlaneAlignment(RigidAlignment):
         ref, tgt, nrm = conv(ref_points), conv(tgt_points), conv(ref_normals)
         x0 = None
         if initial_estimate is not None:
-            x0 = conv(initial_estimate)
-            if x0.ndim == 3:
-                assert_debug(not is64, "pose-matrix initial estimates are float32")
-                x0 = self.pose.from_pose_matrix(x0)
-            x0 = conv(x0.reshape(6))
+            x0 = _initial_params(self.pose, initial_estimate, b, is64, conv)
         mk = (lambda s: np.empty(s, dtype=dt_np)) if is_np else (lambda s: torch.empty(s, dtype=dt_t, device=tgt.device))
-        dT, x, loss = mk((1, 4, 4)), mk((1, 6)), mk((1, n))
-        self.ctx.call("pls_align_p2plane", _lib.ptr(ref), _lib.ptr(tgt), _lib.ptr(nrm), n, int(is64),
-                      _lib.SCHEMES[self.gn["scheme"]], self.gn["sigma"], self.gn["max_iters"], self.gn["norm_stop"],
-                      _lib.ptr(x0), _lib.ptr(dT), _lib.ptr(x), _lib.ptr(loss))
+        dT, x, loss = mk((b, 4, 4)), mk((b, 6)), mk((b, n))
+        gn = (_lib.SCHEMES[self.gn["scheme"]], self.gn["sigma"], self.gn["max_iters"], self.gn["norm_stop"])
+        if b == 1:
+            self.ctx.call("pls_align_p2plane", _lib.ptr(ref), _lib.ptr(tgt), _lib.ptr(nrm), n, int(is64), *gn,
+                          _lib.ptr(x0), _lib.ptr(dT), _lib.ptr(x), _lib.ptr(loss))
+        else:
+            self.ctx.call("pls_align_p2plane_batch", _lib.ptr(ref), _lib.ptr(tgt), _lib.ptr(nrm), b, n, int(is64), *gn,
+                          _lib.ptr(x0), _lib.ptr(dT), _lib.ptr(x), _lib.ptr(loss), None)
         return dT, x, loss
 
 
@@ -353,14 +368,15 @@ class GaussNewtonPointToPointAlignment(RigidAlignment):
         return self._ctx or default_context()
 
     def align(self, ref_points, tgt_points, initial_estimate=None, mask=None, **kwargs):
+        """As GaussNewtonPointToPlaneAlignment.align without normals; B > 1 -> pls_align_p2point_batch."""
         assert_debug(not self.config.initialize_with_svd,
                      "initialize_with_svd fails inside the reference itself (registration.py:58-59 builds a [b,16,16] "
                      "tensor); use pylidar_slam_b200.common.weighted_procrustes and pass it as initial_estimate")
-        check_tensor(tgt_points, [1, -1, 3])
-        n = tgt_points.shape[1]
-        check_tensor(ref_points, [1, n, 3])
+        check_tensor(tgt_points, [-1, -1, 3])
+        b, n = tgt_points.shape[0], tgt_points.shape[1]
+        check_tensor(ref_points, [b, n, 3])
         if mask is not None:
-            _reject_mask(mask, n)
+            _reject_mask(mask, b, n)
         is_np = isinstance(tgt_points, np.ndarray)
         is64 = (tgt_points.dtype == (np.float64 if is_np else torch.float64))
         dt_np, dt_t = (np.float64, torch.float64) if is64 else (np.float32, torch.float32)
@@ -368,17 +384,16 @@ class GaussNewtonPointToPointAlignment(RigidAlignment):
         ref, tgt = conv(ref_points), conv(tgt_points)
         x0 = None
         if initial_estimate is not None:
-            x0 = conv(initial_estimate)
-            if x0.ndim == 3:
-                check_tensor(x0, [1, 4, 4])
-                assert_debug(not is64, "pose-matrix initial estimates are float32")
-                x0 = self.pose.from_pose_matrix(x0)
-            x0 = conv(x0.reshape(6))
+            x0 = _initial_params(self.pose, initial_estimate, b, is64, conv)
         mk = (lambda s: np.empty(s, dtype=dt_np)) if is_np else (lambda s: torch.empty(s, dtype=dt_t, device=tgt.device))
-        dT, x, loss = mk((1, 4, 4)), mk((1, 6)), mk((1, n))
-        self.ctx.call("pls_align_p2point", _lib.ptr(ref), _lib.ptr(tgt), n, int(is64), _lib.SCHEMES[self.gn["scheme"]],
-                      self.gn["sigma"], self.gn["max_iters"], self.gn["norm_stop"], _lib.ptr(x0), _lib.ptr(dT), _lib.ptr(x),
-                      _lib.ptr(loss))
+        dT, x, loss = mk((b, 4, 4)), mk((b, 6)), mk((b, n))
+        gn = (_lib.SCHEMES[self.gn["scheme"]], self.gn["sigma"], self.gn["max_iters"], self.gn["norm_stop"])
+        if b == 1:
+            self.ctx.call("pls_align_p2point", _lib.ptr(ref), _lib.ptr(tgt), n, int(is64), *gn, _lib.ptr(x0), _lib.ptr(dT),
+                          _lib.ptr(x), _lib.ptr(loss))
+        else:
+            self.ctx.call("pls_align_p2point_batch", _lib.ptr(ref), _lib.ptr(tgt), b, n, int(is64), *gn, _lib.ptr(x0),
+                          _lib.ptr(dT), _lib.ptr(x), _lib.ptr(loss), None)
         return dT, x, loss
 
 
