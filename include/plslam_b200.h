@@ -222,11 +222,25 @@ PLS_API int pls_kdmap_last_correspondences(pls_context* ctx, int64_t n, int64_t*
  * position in the Morton-sorted point array or -1 (nullable).  Touches neither the normal cache nor any ICP state. */
 PLS_API int pls_kdmap_knn(pls_context* ctx, const float* queries, int64_t n, int k, int64_t* out_idx, float* out_d2,
                           int32_t* out_pos);
+/* KdTreeLocalMap.set_map_pointcloud (local_map.py:289-299): the map becomes the cloud xyz [n,3] (float32, or float64
+ * if is_f64, rounded to float32; host or device), in order, with a new search index and no cached normal.  The cloud is
+ * held as no frame: a later update moves it and appends frames, and once more than local_map_size frames are held the
+ * eviction drops as many rows from the FRONT of the map as the oldest frame had -- prior-map rows first, as the
+ * reference's `_local_map[size_first_cloud:]` does.  A row with a NaN or infinite coordinate is refused
+ * (PLS_E_INVALID, the map unchanged): the reference keeps such rows, but its search cannot handle them.  n == 0 leaves
+ * an empty map. */
+PLS_API int pls_kdmap_set_points(pls_context* ctx, const void* xyz, int is_f64, int64_t n);
+/* The point counts of the frames the kd map holds, oldest first: *out_num frames (at most local_map_size), out_counts
+ * [local_map_size] or NULL.  Rows of the map before the first counted frame are a cloud set by pls_kdmap_set_points. */
+PLS_API int pls_kdmap_frames(pls_context* ctx, int64_t* out_counts, int* out_num);
 /* ProjectiveLocalMap.update (local_map.py:126-202): rel_pose [16]; vertex_map [3,H,W] or NULL. */
 PLS_API int pls_projmap_update(pls_context* ctx, const float* rel_pose, const float* vertex_map);
 PLS_API int pls_projmap_num_frames(pls_context* ctx, int* num_frames);
 /* The re-projected model maps _model_vmap/_model_nmap, each [K,3,H,W]. */
 PLS_API int pls_projmap_model(pls_context* ctx, float* out_vmap, float* out_nmap);
+/* The newest frame's vertex map [3,H,W] as it was inserted (ProjectiveLocalMap.get_last_frame, local_map.py:238-240).
+ * PLS_E_STATE if the map holds no frame. */
+PLS_API int pls_projmap_last_frame(pls_context* ctx, float* out_vmap);
 /* ProjectiveLocalMap.nearest_neighbor_search (local_map.py:205-235): queries [n,3];
  * outputs [Nc,3] each (capacity H*W rows), row-major pixel order; *out_count = Nc. */
 PLS_API int pls_projmap_nn_search(pls_context* ctx, const float* queries, int64_t n,
@@ -241,6 +255,16 @@ PLS_API int pls_odometry_init(pls_context* ctx);
  * *out_iters = iterations executed (= len(losses)). */
 PLS_API int pls_register_frame(pls_context* ctx, const float* points, int64_t n, const float* T0,
                        float* out_T, float* out_params, float* out_losses, int* out_iters);
+/* B hypotheses of one scan on the kd map, in one call (no reference counterpart: relocalisation registers a scan from
+ * many initial guesses).  points [n,3] as pls_register_frame; T0s [B,16].  out_T [B,16], out_params [B,6], out_losses
+ * [B,max_num_alignments], out_iters [B]: hypothesis b's are the bits pls_register_frame gives with T0s[b] on the same map.
+ * out_status [B] (nullable): PLS_OK, PLS_W_TINY_RESIDUAL or PLS_E_SINGULAR per hypothesis; without it the call returns
+ * PLS_E_SINGULAR if a hypothesis was singular (every output still written).  The map is not updated; afterwards the
+ * last hypothesis is the context's last search (pls_kdmap_last_correspondences, pls_last_icp_sums).  Every kernel of an
+ * ICP iteration is one launch for up to PLS_MAX_SEQUENCES hypotheses, larger B runs in chunks of that many.  Needs a
+ * kd-tree map, gn_max_iters == 1, no communicator, B > 0 and n > 0. */
+PLS_API int pls_register_hypotheses(pls_context* ctx, const float* points, int64_t n, const float* T0s, int B,
+                                    float* out_T, float* out_params, float* out_losses, int* out_iters, int* out_status);
 /* ICPFrameToModel.do_process_next_frame (icp_odometry.py:157-246): `data` is [n,3] points
  * (PLS_INPUT_NDARRAY / PLS_INPUT_TENSOR: float; the _F64 variants: double) or a float [3,H,W] vertex map
  * (PLS_INPUT_VERTEX_MAP, n ignored).  init_pose [16] or NULL (identity).  On frame 0 the map is initialised and

@@ -72,12 +72,16 @@ _SIGNATURES = {
     "pls_kdmap_nn_search": [_P, _P, _L, _P, _P, _P],
     "pls_kdmap_last_correspondences": [_P, _L, _P, _P, _P, _P, _P],
     "pls_kdmap_knn": [_P, _P, _L, _I, _P, _P, _P],
+    "pls_kdmap_set_points": [_P, _P, _I, _L],
+    "pls_kdmap_frames": [_P, _P, C.POINTER(_I)],
+    "pls_projmap_last_frame": [_P, _P],
     "pls_projmap_update": [_P, _P, _P],
     "pls_projmap_num_frames": [_P, C.POINTER(_I)],
     "pls_projmap_model": [_P, _P, _P],
     "pls_projmap_nn_search": [_P, _P, _L, _P, _P, _P, C.POINTER(_L)],
     "pls_odometry_init": [_P],
     "pls_register_frame": [_P, _P, _L, _P, _P, _P, _P, C.POINTER(_I)],
+    "pls_register_hypotheses": [_P, _P, _L, _P, _I, _P, _P, _P, _P, _P],
     "pls_process_frame": [_P, _P, _I, _L, _P, _P, _P, C.POINTER(_I), _P],
     "pls_process_frame_grid_sample": [_P, _P, _L, _D, _I, _P, _P, _P, C.POINTER(_I), _P],
     "pls_process_frames": [_P, _I, _P, _P, _P, _D, _P, _P, _P, _P, _P, _P],

@@ -1,6 +1,7 @@
 // Internal declarations shared by the translation units of libplslam_b200.so.
 #pragma once
 #include <cuda_runtime.h>
+#include <stddef.h>
 #include <stdint.h>
 #include <stdio.h>
 #include <string.h>
@@ -238,6 +239,7 @@ struct pls_context {
     pls::DBuf kd_nn_state;              // per query: position at its last full search + runner-up bound (float4)
     pls::DBuf partials;                 // [blocks][NACC] doubles
     pls::DBuf batch_buf;                // pls_process_frames led by this context: sequence descriptors, then done flags
+    pls::DBuf hyp_buf;                  // pls_register_hypotheses: FrameResults and per-query state of the hypotheses
     cudaEvent_t ev_batch = nullptr;     // pls_process_frames: this context's input stage, before the batched ICP
     pls::DBuf gs_keys, gs_vals, gs_out_xyz, gs_out_idx;
     uint32_t gs_seq = 0;                // stamp of the last compact-key grid sample (overflow detection)
@@ -399,13 +401,18 @@ void kdmap_update(pls_context* ctx, const float* rel_pose_host, const float* pts
 void kdmap_update_packed(pls_context* ctx, const float* rel_pose_host, const float4* fresh_dev, int64_t num_new,
                          bool has_new);
 // pls_process_frames: the ICP of `num` sequences (distinct kd-map contexts, no communicator) in batched launches on st.
-// begin uploads their descriptors into lead->batch_buf and returns the launch widths in grid[3]; iterations enqueues
+// begin uploads their descriptors into lead->batch_buf and returns the launch widths in grid[5]; iterations enqueues
 // ICP iterations [first, last) of all of them; done reads every sequence's done flag with one copy and one sync.
 void kdmap_batch_begin(pls_context* lead, pls_context* const* ctxs, const int64_t* query_bounds, int num, cudaStream_t st,
                        int* grid);
-void kdmap_batch_iterations(pls_context* lead, pls_context* const* ctxs, const int64_t* query_bounds, int num, cudaStream_t st,
-                            const int* grid, int first, int last);
+void kdmap_batch_iterations(pls_context* lead, int num, cudaStream_t st, const int* grid, int first, int last);
 void kdmap_batch_done(pls_context* lead, int num, cudaStream_t st, int* out);
+// pls_register_hypotheses: `num` <= PLS_MAX_SEQUENCES hypotheses of the scan in ctx->query_ptr on ctx's map, driven by
+// kdmap_batch_iterations / kdmap_batch_done with lead = ctx.  begin returns their FrameResults and 16 counter and
+// work-list words each (for the caller to initialise, as frame_begin does); adopt makes hypothesis h ctx's last search.
+void kdmap_hypotheses_begin(pls_context* ctx, int64_t query_bound, int num, cudaStream_t st, int* grid, FrameResult** frs,
+                            uint32_t** words);
+void kdmap_hypothesis_adopt(pls_context* ctx, int64_t query_bound, int h, cudaStream_t st);
 // ICP iteration `it` of the frame over ctx->query_ptr; returns the number of partial rows written
 // it == 0: no previous matches; fuse_threshold >= 0: finish the iteration (sum + solve + pose update) in the last
 // block of the reduction kernel (*solved tells).  bound_dev (nullable, unsharded frames only): a device-side count that

@@ -104,6 +104,15 @@ __global__ void kd_pack_rows_kernel(const T* __restrict__ pts, int64_t n, const 
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
         if (flags[i]) out[pos[i]] = make_float4((float)pts[3 * i], (float)pts[3 * i + 1], (float)pts[3 * i + 2], 0.f);
 }
+// pls_kdmap_set_points: counts the rows with a NaN or an infinite coordinate once rounded to float32.
+template <typename T>
+__global__ void kd_nonfinite_rows_kernel(const T* __restrict__ pts, int64_t n, uint32_t* __restrict__ count) {
+    uint32_t bad = 0;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
+        bad += !(isfinite((float)pts[3 * i]) && isfinite((float)pts[3 * i + 1]) && isfinite((float)pts[3 * i + 2]));
+    bad = __reduce_add_sync(0xffffffffu, bad);
+    if ((threadIdx.x & 31) == 0 && bad) atomicAdd(count, bad);
+}
 // vertex map [3,H,W] -> pixels with |p| > min_norm and no NaN
 __global__ void kd_valid_pixels_kernel(const float* __restrict__ vmap, int64_t hw, float min_norm,
                                        uint8_t* __restrict__ flags) {
@@ -386,10 +395,11 @@ __device__ __forceinline__ void block_partial_and_finish(double* acc, FrameResul
 
 // Iterations after a frame's first on maps of KD_COLD_MAP_POINTS or more: a thread per query keeps its previous match
 // if match_proven; the few others are queued for kd_nn_warp_kernel.
-__global__ void __launch_bounds__(KD_THREADS)
-kd_nn_verify_kernel(KdIndex ix, const float4* __restrict__ queries, const uint32_t* __restrict__ nq_dev, int64_t q_begin,
-                    int64_t q_stride, const float* __restrict__ T, const int* __restrict__ done, const int* __restrict__ match,
-                    const float4* __restrict__ nn_state, int* __restrict__ hard, uint32_t* lists, int parity) {
+__device__ __forceinline__ void kd_nn_verify_body(const KdIndex& ix, const float4* __restrict__ queries,
+                                                  const uint32_t* __restrict__ nq_dev, int64_t q_begin, int64_t q_stride,
+                                                  const float* __restrict__ T, const int* __restrict__ done,
+                                                  const int* __restrict__ match, const float4* __restrict__ nn_state,
+                                                  int* __restrict__ hard, uint32_t* lists, int parity, unsigned block) {
     if (done && *done) return;
     __shared__ float sT[12];
     __shared__ int s_hard[KD_THREADS];
@@ -397,12 +407,12 @@ kd_nn_verify_kernel(KdIndex ix, const float4* __restrict__ queries, const uint32
     if (threadIdx.x < 12) sT[threadIdx.x] = T[threadIdx.x];
     if (threadIdx.x == 0) {
         s_nh = 0;
-        if (blockIdx.x == 0)
+        if (block == 0)
             for (int l = 0; l < KDL_WORDS; l += 2) lists[l + (parity ^ 1)] = 0;
     }
     __syncthreads();
     const int64_t nq = (int64_t)*nq_dev;
-    const int64_t qi = q_begin + ((int64_t)blockIdx.x * KD_THREADS + threadIdx.x) * q_stride;
+    const int64_t qi = q_begin + ((int64_t)block * KD_THREADS + threadIdx.x) * q_stride;
     if (qi < nq) {
         float p[3];
         transform_query(sT, queries[qi], p);
@@ -410,6 +420,13 @@ kd_nn_verify_kernel(KdIndex ix, const float4* __restrict__ queries, const uint32
     }
     __syncthreads();
     block_flush_list(s_hard, s_nh, hard, lists + KDL_HARD_NN + parity, &s_base);
+}
+
+__global__ void __launch_bounds__(KD_THREADS)
+kd_nn_verify_kernel(KdIndex ix, const float4* __restrict__ queries, const uint32_t* __restrict__ nq_dev, int64_t q_begin,
+                    int64_t q_stride, const float* __restrict__ T, const int* __restrict__ done, const int* __restrict__ match,
+                    const float4* __restrict__ nn_state, int* __restrict__ hard, uint32_t* lists, int parity) {
+    kd_nn_verify_body(ix, queries, nq_dev, q_begin, q_stride, T, done, match, nn_state, hard, lists, parity, blockIdx.x);
 }
 
 // Each kernel of an ICP iteration below is one __device__ body, called by two entry points: the kernel of one sequence,
@@ -731,6 +748,7 @@ struct KdSeq {
     int* match;
     float4* nn_state;
     int* pending;               // normals work list
+    int* hard;                  // queries the verify kernel could not prove (maps of KD_COLD_MAP_POINTS or more)
     uint32_t* lists;            // work-list words (SC_KD_LISTS)
     double* partials;
     unsigned long long* counters;
@@ -740,7 +758,8 @@ struct KdSeq {
     float fuse_threshold;
     int max_iters;              // max_num_alignments: launches of later iterations leave the sequence alone
     int blocks;                 // grid_for(query bound): the residual kernel's geometry on the single path
-    int refine_blocks;          // blocks, or 0 on a map of KD_COLD_MAP_POINTS or more (its own four launches)
+    int refine_blocks;          // blocks, or 0 on a map of KD_COLD_MAP_POINTS or more (the four-launch path)
+    int verify_blocks;          // kd_nn_verify_kernel's grid on the single path: a thread per query
     int nn_blocks, kn_blocks;   // its share of the resident wave of the 1-NN / normals kernels
 };
 static_assert(sizeof(KdSeq) % sizeof(int) == 0, "KdSeq is copied in 4-byte words");
@@ -762,27 +781,42 @@ __device__ __forceinline__ void load_seq(const KdSeq* __restrict__ seqs, KdSeq& 
 #define KD_SPLIT_NONE()
 #endif
 
-// A frame's first iteration: every query, parity 0.
-__global__ void __launch_bounds__(KD_THREADS) kd_nn_warp_batch_kernel(const KdSeq* __restrict__ seqs) {
-    __shared__ KdSeq s;
-    load_seq(seqs, s);
-    if ((int)blockIdx.x >= s.nn_blocks) return;
-    kd_nn_warp_body(s.ix, s.queries, s.nq_dev, 0, 1, nullptr, s.lists, 0, s.fr->T, &s.fr->done, s.match, s.nn_state, 1,
-                    s.pending, s.counters, blockIdx.x, s.nn_blocks);
+// Does iteration `it` of the sequence run through the four launches below?  Its first iteration always does; a later one
+// on a map of KD_COLD_MAP_POINTS or more, while the sequence has not reached its max_iters.
+__device__ __forceinline__ bool four_launch_step(const KdSeq& s, int it) {
+    return it == 0 || (s.refine_blocks == 0 && it < s.max_iters);
 }
 
-__global__ void __launch_bounds__(KD_THREADS) kd_normals_warp_batch_kernel(const KdSeq* __restrict__ seqs) {
+// Iteration `it` >= 1 of the sequences on maps of KD_COLD_MAP_POINTS or more: kd_nn_verify_kernel of each.
+__global__ void __launch_bounds__(KD_THREADS) kd_nn_verify_batch_kernel(const KdSeq* __restrict__ seqs, int it) {
     __shared__ KdSeq s;
     load_seq(seqs, s);
-    if ((int)blockIdx.x >= s.kn_blocks) return;
-    kd_normals_warp_body(s.ix, s.k_normals, s.pending, s.lists + KDL_PENDING, &s.fr->done, s.counters, blockIdx.x,
-                         s.kn_blocks);
+    if ((int)blockIdx.x >= s.verify_blocks || !four_launch_step(s, it)) return;
+    kd_nn_verify_body(s.ix, s.queries, s.nq_dev, 0, 1, s.fr->T, &s.fr->done, s.match, s.nn_state, s.hard, s.lists, it & 1,
+                      blockIdx.x);
 }
 
-__global__ void __launch_bounds__(KD_THREADS) kd_residual_batch_kernel(const KdSeq* __restrict__ seqs) {
+// Iteration 0: every query of every sequence.  Iteration `it` >= 1: the queued queries of the four-launch sequences.
+__global__ void __launch_bounds__(KD_THREADS) kd_nn_warp_batch_kernel(const KdSeq* __restrict__ seqs, int it) {
     __shared__ KdSeq s;
     load_seq(seqs, s);
-    if ((int)blockIdx.x >= s.blocks) return;
+    if ((int)blockIdx.x >= s.nn_blocks || !four_launch_step(s, it)) return;
+    kd_nn_warp_body(s.ix, s.queries, s.nq_dev, 0, 1, it == 0 ? nullptr : s.hard, s.lists, it & 1, s.fr->T, &s.fr->done,
+                    s.match, s.nn_state, 1, s.pending, s.counters, blockIdx.x, s.nn_blocks);
+}
+
+__global__ void __launch_bounds__(KD_THREADS) kd_normals_warp_batch_kernel(const KdSeq* __restrict__ seqs, int it) {
+    __shared__ KdSeq s;
+    load_seq(seqs, s);
+    if ((int)blockIdx.x >= s.kn_blocks || !four_launch_step(s, it)) return;
+    kd_normals_warp_body(s.ix, s.k_normals, s.pending, s.lists + KDL_PENDING + (it & 1), &s.fr->done, s.counters,
+                         blockIdx.x, s.kn_blocks);
+}
+
+__global__ void __launch_bounds__(KD_THREADS) kd_residual_batch_kernel(const KdSeq* __restrict__ seqs, int it) {
+    __shared__ KdSeq s;
+    load_seq(seqs, s);
+    if ((int)blockIdx.x >= s.blocks || !four_launch_step(s, it)) return;
     KD_SPLIT_NONE()
     kd_residual_body(s.ix, s.queries, s.nq_dev, 0, 1, s.fr, s.scheme, s.sigma, s.match, s.partials, s.fuse_threshold,
                      blockIdx.x, s.blocks KD_SPLIT_PASS);
@@ -1207,16 +1241,62 @@ int kdmap_icp_iteration(pls_context* ctx, int64_t query_bound, const uint32_t* b
     return blocks;
 }
 
+// The descriptor of one sequence's (or one hypothesis's) ICP on ctx's map, with its per-query and per-block state at the
+// given addresses; fr is its FrameResult, nq_dev its query count.
+static KdSeq make_seq(pls_context* ctx, const KdPlan& plan, FrameResult* fr, const uint32_t* nq_dev, int* match,
+                      float4* nn_state, int* worklist, uint32_t* words, double* partials, int share_nn, int share_kn) {
+    KdSeq s;
+    s.ix = make_index(ctx);
+    s.queries = ctx->query_ptr;
+    s.nq_dev = nq_dev;
+    s.fr = fr;
+    s.match = match;
+    s.nn_state = nn_state;
+    s.pending = worklist;
+    s.hard = worklist + plan.slots;
+    s.lists = words + (SC_KD_LISTS - SC_KD_COUNTERS);
+    s.partials = partials;
+    s.counters = reinterpret_cast<unsigned long long*>(words);
+    s.scheme = ctx->cfg.scheme;
+    s.sigma = ctx->cfg.sigma;
+    s.k_normals = ctx->cfg.num_neighbors_normals;
+    s.fuse_threshold = ctx->cfg.threshold_delta_pose;
+    s.max_iters = ctx->cfg.max_num_alignments;
+    s.blocks = plan.blocks;
+    s.refine_blocks = ctx->kd.indexed >= KD_COLD_MAP_POINTS ? 0 : plan.blocks;
+    s.verify_blocks = (int)((plan.mine + KD_THREADS - 1) / KD_THREADS);
+    s.nn_blocks = plan.wblocks < share_nn ? plan.wblocks : share_nn;
+    s.kn_blocks = plan.wblocks < share_kn ? plan.wblocks : share_kn;
+    return s;
+}
+
+// The launch widths of kdmap_batch_iterations for these descriptors (see kdmap_batch_begin), and their upload into
+// lead->batch_buf on st.
+static void upload_seqs(pls_context* lead, const std::vector<KdSeq>& seqs, cudaStream_t st, int* grid) {
+    grid[0] = grid[1] = grid[2] = 1;
+    grid[3] = grid[4] = 0;
+    for (const KdSeq& s : seqs) {
+        grid[0] = grid[0] > s.blocks ? grid[0] : s.blocks;
+        grid[1] = grid[1] > s.nn_blocks ? grid[1] : s.nn_blocks;
+        grid[2] = grid[2] > s.kn_blocks ? grid[2] : s.kn_blocks;
+        if (s.refine_blocks == 0) grid[3] = grid[3] > s.verify_blocks ? grid[3] : s.verify_blocks;
+        else grid[4] = 1;
+    }
+    const size_t bytes = seqs.size() * sizeof(KdSeq);
+    lead->batch_buf.reserve(bytes + PLS_MAX_SEQUENCES * sizeof(int), st);
+    PLS_CUDA(cudaMemcpyAsync(lead->batch_buf.p, seqs.data(), bytes, cudaMemcpyHostToDevice, st));
+}
+
 // pls_process_frames: the descriptors of the sequences whose ICP runs in this call, into lead->batch_buf (uploaded on
 // st), and every buffer their iterations use reserved as their single path reserves it.
-// grid[3]: the launch widths, the largest residual / 1-NN / normals block count of a sequence.
+// grid[5]: the launch widths, the largest residual / 1-NN / normals block count of a sequence, the largest verify block
+// count of a sequence on a map of KD_COLD_MAP_POINTS or more (0: none is), and 1 if any sequence's map is smaller.
 void kdmap_batch_begin(pls_context* lead, pls_context* const* ctxs, const int64_t* query_bounds, int num, cudaStream_t st,
                        int* grid) {
     static const int resident_nn = resident_blocks((const void*)kd_nn_warp_batch_kernel);
     static const int resident_kn = resident_blocks((const void*)kd_normals_warp_batch_kernel);
     const int share_nn = (resident_nn + num - 1) / num, share_kn = (resident_kn + num - 1) / num;
-    std::vector<KdSeq> seqs((size_t)num);
-    grid[0] = grid[1] = grid[2] = 1;
+    std::vector<KdSeq> seqs;
     for (int i = 0; i < num; ++i) {
         pls_context* ctx = ctxs[i];
         PLS_REQUIRE(ctx->kd.valid, "kd map: search before any update");
@@ -1224,67 +1304,81 @@ void kdmap_batch_begin(pls_context* lead, pls_context* const* ctxs, const int64_
         ctx->last_sharded = false;
         record_search(ctx->kd, true, false, true, 0);
         FrameResult* fr = frame_result_dev(ctx);
-        KdSeq& s = seqs[(size_t)i];
-        s.ix = make_index(ctx);
-        s.queries = ctx->query_ptr;
-        s.nq_dev = reinterpret_cast<const uint32_t*>(&fr->counts[1]);
-        s.fr = fr;
-        s.match = ctx->nn_prev.as<int>();
-        s.nn_state = ctx->kd_nn_state.as<float4>();
-        s.pending = ctx->kd_worklist.as<int>();
-        s.lists = scalar_u32(ctx, SC_KD_LISTS);
-        s.partials = ctx->partials.as<double>();
-        s.counters = kd_counters(ctx);
-        s.scheme = ctx->cfg.scheme;
-        s.sigma = ctx->cfg.sigma;
-        s.k_normals = ctx->cfg.num_neighbors_normals;
-        s.fuse_threshold = ctx->cfg.threshold_delta_pose;
-        s.max_iters = ctx->cfg.max_num_alignments;
-        s.blocks = plan.blocks;
-        s.refine_blocks = ctx->kd.indexed >= KD_COLD_MAP_POINTS ? 0 : plan.blocks;
-        s.nn_blocks = plan.wblocks < share_nn ? plan.wblocks : share_nn;
-        s.kn_blocks = plan.wblocks < share_kn ? plan.wblocks : share_kn;
-        grid[0] = grid[0] > s.blocks ? grid[0] : s.blocks;
-        grid[1] = grid[1] > s.nn_blocks ? grid[1] : s.nn_blocks;
-        grid[2] = grid[2] > s.kn_blocks ? grid[2] : s.kn_blocks;
+        seqs.push_back(make_seq(ctx, plan, fr, reinterpret_cast<const uint32_t*>(&fr->counts[1]), ctx->nn_prev.as<int>(),
+                                ctx->kd_nn_state.as<float4>(), ctx->kd_worklist.as<int>(), scalar_u32(ctx, SC_KD_COUNTERS),
+                                ctx->partials.as<double>(), share_nn, share_kn));
     }
-    const size_t bytes = seqs.size() * sizeof(KdSeq);
-    lead->batch_buf.reserve(bytes + PLS_MAX_SEQUENCES * sizeof(int), st);
-    PLS_CUDA(cudaMemcpyAsync(lead->batch_buf.p, seqs.data(), bytes, cudaMemcpyHostToDevice, st));
+    upload_seqs(lead, seqs, st, grid);
 }
 
-// ICP iterations [first, last) of the sequences kdmap_batch_begin described, on st: one launch per kernel for all of
-// them; a sequence on a map of KD_COLD_MAP_POINTS or more runs its later iterations through its own four launches.
-void kdmap_batch_iterations(pls_context* lead, pls_context* const* ctxs, const int64_t* query_bounds, int num, cudaStream_t st,
-                            const int* grid, int first, int last) {
+// ICP iterations [first, last) of the sequences kdmap_batch_begin (or kdmap_hypotheses_begin) described, on st: one
+// launch per kernel for all of them.  A later iteration is kd_icp_refine_batch_kernel for the sequences on maps below
+// KD_COLD_MAP_POINTS and the four launches verify / 1-NN / normals / residual for the others; no launch grows with num.
+void kdmap_batch_iterations(pls_context* lead, int num, cudaStream_t st, const int* grid, int first, int last) {
     const KdSeq* seqs = lead->batch_buf.as<KdSeq>();
     for (int it = first; it < last; ++it) {
-        if (it == 0) {
-            kd_nn_warp_batch_kernel<<<dim3(grid[1], num), KD_THREADS, 0, st>>>(seqs);
+        if (it > 0 && grid[4]) {
+            kd_icp_refine_batch_kernel<<<dim3(grid[0], num), KD_REFINE_THREADS, 0, st>>>(seqs, it);
             PLS_CHECK_LAUNCH();
-            kd_normals_warp_batch_kernel<<<dim3(grid[2], num), KD_THREADS, 0, st>>>(seqs);
-            PLS_CHECK_LAUNCH();
-            kd_residual_batch_kernel<<<dim3(grid[0], num), KD_THREADS, 0, st>>>(seqs);
-            PLS_CHECK_LAUNCH();
-            continue;
         }
-        kd_icp_refine_batch_kernel<<<dim3(grid[0], num), KD_REFINE_THREADS, 0, st>>>(seqs, it);
+        if (it > 0 && !grid[3]) continue;
+        if (it > 0) {
+            kd_nn_verify_batch_kernel<<<dim3(grid[3], num), KD_THREADS, 0, st>>>(seqs, it);
+            PLS_CHECK_LAUNCH();
+        }
+        kd_nn_warp_batch_kernel<<<dim3(grid[1], num), KD_THREADS, 0, st>>>(seqs, it);
         PLS_CHECK_LAUNCH();
-        for (int i = 0; i < num; ++i) {
-            pls_context* ctx = ctxs[i];
-            if (ctx->kd.indexed < KD_COLD_MAP_POINTS || it >= ctx->cfg.max_num_alignments) continue;
-            cudaStream_t own = ctx->stream;
-            ctx->stream = st;
-            bool solved = false;
-            try {
-                kdmap_icp_iteration(ctx, query_bounds[i], nullptr, 0, 1, it, ctx->cfg.threshold_delta_pose, &solved);
-            } catch (...) {
-                ctx->stream = own;
-                throw;
-            }
-            ctx->stream = own;
-        }
+        kd_normals_warp_batch_kernel<<<dim3(grid[2], num), KD_THREADS, 0, st>>>(seqs, it);
+        PLS_CHECK_LAUNCH();
+        kd_residual_batch_kernel<<<dim3(grid[0], num), KD_THREADS, 0, st>>>(seqs, it);
+        PLS_CHECK_LAUNCH();
     }
+}
+
+// pls_register_hypotheses: the ICP state of `num` hypotheses of one scan (ctx->query_ptr, count in ctx's FrameResult) on
+// ctx's map, each a slice of ctx->hyp_buf laid out as pls_register_frame's own buffers; their descriptors into
+// ctx->batch_buf.  Returns the hypotheses' FrameResults (contiguous) and their 16 counter and work-list words each, for
+// the caller to initialise before the first iteration; grid[5] as kdmap_batch_begin.
+void kdmap_hypotheses_begin(pls_context* ctx, int64_t query_bound, int num, cudaStream_t st, int* grid, FrameResult** frs,
+                            uint32_t** words) {
+    PLS_REQUIRE(ctx->kd.valid, "kd map: search before any update");
+    static const int resident_nn = resident_blocks((const void*)kd_nn_warp_batch_kernel);
+    static const int resident_kn = resident_blocks((const void*)kd_normals_warp_batch_kernel);
+    const KdPlan plan = plan_kd_iteration(ctx, query_bound, 1);  // ctx's own buffers: the last hypothesis is copied there
+    ctx->last_sharded = false;
+    record_search(ctx->kd, true, false, true, 0);
+    auto up = [](size_t b) { return (b + 255) & ~(size_t)255; };
+    const size_t fr_bytes = up((size_t)num * sizeof(FrameResult)), word_bytes = up((size_t)num * 16 * sizeof(uint32_t));
+    const size_t match_b = up((size_t)query_bound * sizeof(int)), state_b = up(plan.slots * sizeof(float4)),
+                 list_b = up(2 * plan.slots * sizeof(int)), part_b = up((size_t)plan.blocks * NACC * sizeof(double));
+    const size_t per = match_b + state_b + list_b + part_b;
+    ctx->hyp_buf.reserve(fr_bytes + word_bytes + (size_t)num * per, st);
+    char* base = ctx->hyp_buf.as<char>();
+    *frs = reinterpret_cast<FrameResult*>(base);
+    *words = reinterpret_cast<uint32_t*>(base + fr_bytes);
+    const FrameResult* fr_ctx = frame_result_dev(ctx);
+    const uint32_t* nq_dev = reinterpret_cast<const uint32_t*>(&fr_ctx->counts[1]);  // one packed scan for all
+    const int share_nn = (resident_nn + num - 1) / num, share_kn = (resident_kn + num - 1) / num;
+    std::vector<KdSeq> seqs;
+    for (int h = 0; h < num; ++h) {
+        char* p = base + fr_bytes + word_bytes + (size_t)h * per;
+        seqs.push_back(make_seq(ctx, plan, *frs + h, nq_dev, reinterpret_cast<int*>(p), reinterpret_cast<float4*>(p + match_b),
+                                reinterpret_cast<int*>(p + match_b + state_b), *words + 16 * h,
+                                reinterpret_cast<double*>(p + match_b + state_b + list_b), share_nn, share_kn));
+    }
+    upload_seqs(ctx, seqs, st, grid);
+}
+
+// Hypothesis h's matches, search states and FrameResult (all but the counts) into ctx's own: pls_kdmap_last_correspondences
+// and pls_last_icp_sums then read that hypothesis as the last search.
+void kdmap_hypothesis_adopt(pls_context* ctx, int64_t query_bound, int h, cudaStream_t st) {
+    KdSeq s;
+    PLS_CUDA(cudaMemcpyAsync(&s, ctx->batch_buf.as<KdSeq>() + h, sizeof(KdSeq), cudaMemcpyDeviceToHost, st));
+    PLS_CUDA(cudaStreamSynchronize(st));
+    PLS_CUDA(cudaMemcpyAsync(ctx->nn_prev.p, s.match, (size_t)query_bound * sizeof(int), cudaMemcpyDeviceToDevice, st));
+    PLS_CUDA(cudaMemcpyAsync(ctx->kd_nn_state.p, s.nn_state, (size_t)query_bound * sizeof(float4), cudaMemcpyDeviceToDevice,
+                             st));
+    PLS_CUDA(cudaMemcpyAsync(frame_result_dev(ctx), s.fr, offsetof(FrameResult, counts), cudaMemcpyDeviceToDevice, st));
 }
 
 // The done flag of every sequence of the batch: one gather launch, one copy, one synchronisation.
@@ -1313,6 +1407,55 @@ int pls_kdmap_update_points(pls_context* ctx, const float* rel_pose, const float
     const float* d = (points && n > 0) ? (const float*)to_device(ctx, points, (size_t)n * 3 * sizeof(float), ctx->stage_in[0]) : nullptr;
     kdmap_update(ctx, rel, d, d ? n : 0, nullptr, 0, 0, -1);
     PLS_CUDA(cudaStreamSynchronize(ctx->stream));
+    PLS_API_END(ctx)
+}
+
+int pls_kdmap_set_points(pls_context* ctx, const void* xyz, int is_f64, int64_t n) {
+    PLS_API_BEGIN(ctx)
+    PLS_REQUIRE(ctx->cfg.local_map_type == PLS_MAP_KDTREE, "context holds a projective map");
+    PLS_REQUIRE(n >= 0 && (xyz || n == 0), "pls_kdmap_set_points: points must be [n,3] with n >= 0");
+    PLS_REQUIRE(n < (1ll << 30), "kd map: too many points");
+    sync_all(ctx);
+    cudaStream_t st = ctx->stream;
+    const size_t elem = is_f64 ? sizeof(double) : sizeof(float);
+    const void* d = n > 0 ? to_device(ctx, xyz, (size_t)n * 3 * elem, ctx->stage_in[0]) : nullptr;
+    if (n > 0) {  // every row must be searchable: checked before the map changes
+        uint32_t* bad = scalar_u32(ctx, SC_SPARE0);
+        PLS_CUDA(cudaMemsetAsync(bad, 0, sizeof(uint32_t), st));
+        const int g = grid_for(n, 256, 8 * kNumSMs);
+        if (is_f64) kd_nonfinite_rows_kernel<double><<<g, 256, 0, st>>>((const double*)d, n, bad);
+        else kd_nonfinite_rows_kernel<float><<<g, 256, 0, st>>>((const float*)d, n, bad);
+        PLS_CHECK_LAUNCH();
+        uint32_t nbad = 0;
+        PLS_CUDA(cudaMemcpyAsync(&nbad, bad, sizeof(nbad), cudaMemcpyDeviceToHost, st));
+        PLS_CUDA(cudaStreamSynchronize(st));
+        PLS_REQUIRE(nbad == 0, "pls_kdmap_set_points: the cloud has rows with a NaN or infinite coordinate, which the "
+                               "kd map cannot search");
+    }
+    kdmap_reset(ctx);
+    if (n > 0) {
+        // no row is dropped (all are finite): the packers give the rows in order, as float4
+        ctx->tmp[4].reserve((size_t)n * sizeof(float4), st);
+        if (is_f64) pack_valid_rows_f64(ctx, (const double*)d, n, ctx->tmp[4].as<float4>(), scalar_u32(ctx, SC_INSERT_COUNT));
+        else pack_valid_rows(ctx, (const float*)d, n, ctx->tmp[4].as<float4>(), scalar_u32(ctx, SC_INSERT_COUNT));
+    }
+    // the map's first insertion (identity, nothing to move or evict) ...
+    kdmap_update_packed(ctx, nullptr, ctx->tmp[4].as<float4>(), n, true);
+    // ... held as no frame: the frames inserted later count from the first update on, and the steady-state capacity
+    // plan follows them, not the cloud
+    ctx->kd.frame_counts.clear();
+    ctx->kd.max_frame = 0;
+    PLS_CUDA(cudaStreamSynchronize(st));
+    PLS_API_END(ctx)
+}
+
+int pls_kdmap_frames(pls_context* ctx, int64_t* out_counts, int* out_num) {
+    PLS_API_BEGIN(ctx)
+    PLS_REQUIRE(out_num, "pls_kdmap_frames: null output");
+    const std::deque<int64_t>& fc = ctx->kd.frame_counts;
+    *out_num = (int)fc.size();
+    if (out_counts)
+        for (size_t i = 0; i < fc.size(); ++i) out_counts[i] = fc[i];
     PLS_API_END(ctx)
 }
 

@@ -44,8 +44,8 @@ struct Pose16 {
 // The start of a frame's ICP.  The initial pose is T0_dev if given, else T0 (a kernel argument: no copy in front of the
 // kernel).  The frame's counts: the input stage wrote the low words of counts[1] (queries; copied from counts[2] here
 // when the queries are the valid rows themselves) and counts[2] (valid rows); every other word is cleared.
-__global__ void frame_begin_kernel(FrameResult* fr, const float* T0_dev /*16, or null*/, Pose16 T0, int max_iters,
-                                   uint32_t* worklist_counts /*16*/, int queries_are_rows) {
+__device__ __forceinline__ void frame_begin_body(FrameResult* fr, const float* T0_dev /*16, or null*/, const Pose16& T0,
+                                                 uint32_t* worklist_counts /*16*/, int queries_are_rows) {
     int t = threadIdx.x;
     if (t < 16) worklist_counts[t] = 0;  // SC_KD_COUNTERS + SC_KD_LISTS: the kd search's counters and work lists
     if (t < 16) fr->T[t] = T0_dev ? T0_dev[t] : T0.m[t];
@@ -62,6 +62,16 @@ __global__ void frame_begin_kernel(FrameResult* fr, const float* T0_dev /*16, or
         fr->pad = 0;  // last-block ticket of the fused correspondence+solve kernels
     }
     if (t < NACC) fr->last_sums[t] = 0.0;
+}
+
+__global__ void frame_begin_kernel(FrameResult* fr, const float* T0_dev /*16, or null*/, Pose16 T0, int max_iters,
+                                   uint32_t* worklist_counts /*16*/, int queries_are_rows) {
+    frame_begin_body(fr, T0_dev, T0, worklist_counts, queries_are_rows);
+}
+
+// pls_register_hypotheses: block h starts hypothesis h at T0s[16 h], as frame_begin_kernel starts a frame.
+__global__ void hypotheses_begin_kernel(FrameResult* frs, const float* __restrict__ T0s, uint32_t* words) {
+    frame_begin_body(frs + blockIdx.x, T0s + 16 * blockIdx.x, Pose16{}, words + 16 * blockIdx.x, 0);
 }
 
 
@@ -873,6 +883,74 @@ int pls_register_frame(pls_context* ctx, const float* points, int64_t n, const f
     PLS_API_END(ctx)
 }
 
+int pls_register_hypotheses(pls_context* ctx, const float* points, int64_t n, const float* T0s, int B, float* out_T,
+                            float* out_params, float* out_losses, int* out_iters, int* out_status) {
+    PLS_API_BEGIN(ctx)
+    PLS_REQUIRE(points && n > 0, "pls_register_hypotheses: points must be [n,3] with n > 0");
+    PLS_REQUIRE(T0s && B > 0, "pls_register_hypotheses: T0s must be [B,16] with B > 0");
+    PLS_REQUIRE(ctx->cfg.gn_max_iters == 1, "fused ICP path supports gauss_newton_config.max_iters == 1");
+    PLS_REQUIRE(ctx->cfg.local_map_type == PLS_MAP_KDTREE, "pls_register_hypotheses: needs a kd-tree local map");
+    PLS_REQUIRE(!ctx->comm, "pls_register_hypotheses: a context with a multi-GPU communicator is not supported");
+    PLS_REQUIRE(ctx->kd.valid, "kd map: search before any update");
+    cudaStream_t st = ctx->stream;
+    map_stream_wait(ctx);
+    // the scan is packed once, as pls_register_frame packs it; every hypothesis reads it
+    const float* d = (const float*)to_device(ctx, points, (size_t)n * 3 * sizeof(float), ctx->stage_in[0]);
+    const float* T0_dev = (const float*)to_device(ctx, T0s, (size_t)B * 16 * sizeof(float), ctx->stage_in[1]);
+    FrameResult* fr = frame_result_dev(ctx);
+    PLS_CUDA(cudaMemsetAsync(fr->counts, 0, sizeof(fr->counts), st));
+    ctx->queries.reserve((size_t)n * sizeof(float4), st);
+    pack_valid_rows(ctx, d, n, ctx->queries.as<float4>(), count_slot(ctx, 1));
+    ctx->query_ptr = ctx->queries.as<float4>();
+    const int M = ctx->cfg.max_num_alignments;
+    std::vector<FrameResult> h((size_t)PLS_MAX_SEQUENCES);
+    std::vector<float> T((size_t)B * 16), params((size_t)B * 6), losses((size_t)B * M);
+    std::vector<int> iters((size_t)B), status((size_t)B);
+    int first_error = PLS_OK, last = 0;
+    for (int c0 = 0; c0 < B; c0 += PLS_MAX_SEQUENCES) {  // chunks of at most PLS_MAX_SEQUENCES hypotheses
+        const int num = B - c0 < PLS_MAX_SEQUENCES ? B - c0 : PLS_MAX_SEQUENCES;
+        int grid[5];
+        FrameResult* frs = nullptr;
+        uint32_t* words = nullptr;
+        kdmap_hypotheses_begin(ctx, n, num, st, grid, &frs, &words);
+        hypotheses_begin_kernel<<<num, kMaxAlign, 0, st>>>(frs, T0_dev + 16 * (size_t)c0, words);
+        PLS_CHECK_LAUNCH();
+        // every hypothesis has ctx's settings: icp_rounds sees num copies of ctx
+        std::vector<pls_context*> same((size_t)num, ctx);
+        icp_rounds(same.data(), num, [&](int a, int b) { kdmap_batch_iterations(ctx, num, st, grid, a, b); },
+                   [&](int* done) { kdmap_batch_done(ctx, num, st, done); });
+        PLS_CUDA(cudaMemcpyAsync(h.data(), frs, (size_t)num * sizeof(FrameResult), cudaMemcpyDeviceToHost, st));
+        PLS_CUDA(cudaStreamSynchronize(st));
+        for (int j = 0; j < num; ++j) {
+            const FrameResult& r = h[(size_t)j];
+            const size_t b = (size_t)(c0 + j);
+            memcpy(&T[16 * b], r.T, 16 * sizeof(float));
+            memcpy(&params[6 * b], r.params, 6 * sizeof(float));
+            memcpy(&losses[(size_t)M * b], r.losses, (size_t)M * sizeof(float));
+            iters[b] = r.iters;
+            status[b] = r.status;
+            if (first_error == PLS_OK && (r.status == PLS_E_SINGULAR || r.status == PLS_E_COMM)) first_error = r.status;
+        }
+        last = num - 1;
+    }
+    // the last hypothesis is this context's last search and last ICP result, as if pls_register_frame had run it last
+    kdmap_hypothesis_adopt(ctx, n, last, st);
+    fetch_result(ctx);
+    ctx->icp_result = true;
+    auto put = [&](void* dst, const void* src, size_t bytes) {  // host or device outputs, as pls_register_frame
+        if (!dst) return;
+        if (is_device_ptr(dst)) PLS_CUDA(cudaMemcpy(dst, src, bytes, cudaMemcpyHostToDevice));
+        else memcpy(dst, src, bytes);
+    };
+    put(out_T, T.data(), T.size() * sizeof(float));
+    put(out_params, params.data(), params.size() * sizeof(float));
+    put(out_losses, losses.data(), losses.size() * sizeof(float));
+    put(out_iters, iters.data(), iters.size() * sizeof(int));
+    put(out_status, status.data(), status.size() * sizeof(int));
+    if (!out_status) raise_status(ctx, first_error);
+    PLS_API_END(ctx)
+}
+
 int pls_process_frame(pls_context* ctx, const void* data, int layout, int64_t n, const float* init_pose,
                       float* out_pose, float* out_params, int* out_has_pose, double* out_info) {
     PLS_API_BEGIN(ctx)  // (enqueues the last frame's map update first, unless this frame's grid-sample call already did)
@@ -1055,12 +1133,12 @@ int pls_process_frames(pls_context* const* ctxs, int num, const void* const* dat
         trace.inputs_done(st, (int)active.size(), m);
         if (m > 0) {
             cur = icp_seq[0];
-            int grid[4];
+            int grid[5];
             const bool kd = lead->cfg.local_map_type == PLS_MAP_KDTREE;
             if (kd) kdmap_batch_begin(lead, icp.data(), bounds.data(), m, st, grid);
             else projmap_batch_begin(lead, icp.data(), bounds.data(), m, st, grid);
             auto enqueue = [&](int first, int last) {
-                if (kd) kdmap_batch_iterations(lead, icp.data(), bounds.data(), m, st, grid, first, last);
+                if (kd) kdmap_batch_iterations(lead, m, st, grid, first, last);
                 else projmap_batch_iterations(lead, icp.data(), bounds.data(), m, st, grid, first, last);
             };
             auto read_done = [&](int* done) {

@@ -1161,6 +1161,22 @@ int pls_projmap_num_frames(pls_context* ctx, int* num_frames) {
     PLS_API_END(ctx)
 }
 
+int pls_projmap_last_frame(pls_context* ctx, float* out_vmap) {
+    PLS_API_BEGIN(ctx)
+    map_stream_wait(ctx);
+    PLS_REQUIRE(out_vmap, "pls_projmap_last_frame: null output");
+    const ProjMap& pm = ctx->pm;
+    if (pm.K == 0) throw pls::Error{PLS_E_STATE, "pls_projmap_last_frame: the map holds no frame"};
+    const size_t frame_bytes = (size_t)3 * ctx->cfg.height * ctx->cfg.width * sizeof(float);
+    const size_t slot = (size_t)((pm.head + pm.K - 1) % (ctx->cfg.local_map_size + 1));  // the ring slot of the newest
+    OutArg o = out_arg(ctx, out_vmap, frame_bytes, ctx->stage_out[0]);
+    PLS_CUDA(cudaMemcpyAsync(o.dev, pm.vmaps.as<char>() + slot * frame_bytes, frame_bytes, cudaMemcpyDeviceToDevice,
+                             ctx->stream));
+    finish_out(ctx, o);
+    PLS_CUDA(cudaStreamSynchronize(ctx->stream));
+    PLS_API_END(ctx)
+}
+
 int pls_projmap_model(pls_context* ctx, float* out_vmap, float* out_nmap) {
     PLS_API_BEGIN(ctx)
     map_stream_wait(ctx);

@@ -123,8 +123,26 @@ def _new(x, shape, dtype=torch.float32):
     return torch.empty(shape, dtype=dtype, device=x.device)
 
 
+# The reference's set_map_pointcloud(pointcloud, normals) stores the [N,3] normals where its search reads a fourth column
+# (local_map.py:297-299, 399): every search with normals then raises IndexError, until the next update or init rebuilds
+# the normal cache.  The flag lives on the context, which the map shares with the odometry that registers on it.
+_NORMALS_INDEX_ERROR = "index 3 is out of bounds for axis 1 with size 3"
+
+
+def _set_given_normals(ctx, given: bool):
+    ctx.kd_given_normals = given
+
+
+def _check_given_normals(ctx):
+    if getattr(ctx, "kd_given_normals", False):
+        raise IndexError(_NORMALS_INDEX_ERROR)
+
+
 class KdTreeLocalMap(LocalMap):
-    """KdTreeLocalMap (local_map.py:254-427) on the GPU: exact 1-NN over the hashed cell pyramid + lazily cached 10-NN normals."""
+    """KdTreeLocalMap (local_map.py:254-427) on the GPU: exact 1-NN over the hashed cell pyramid + lazily cached 10-NN normals.
+
+    Pass `ctx=odometry.ctx` to work on the map an ICPFrameToModel registers against, e.g. to load a prior map with
+    set_map_pointcloud and localise scans in it with register_new_frame_hypotheses."""
 
     def __init__(self, config: KdTreeLocalMapConfig, projector=None, ctx: Optional[_lib.Context] = None, **kwargs):
         super().__init__(config)
@@ -133,8 +151,47 @@ class KdTreeLocalMap(LocalMap):
 
     def init(self):
         self.ctx.call("pls_map_init")
+        _set_given_normals(self.ctx, False)
+
+    def set_map_pointcloud(self, pointcloud: np.ndarray, normals: Optional[np.ndarray] = None):
+        """KdTreeLocalMap.set_map_pointcloud (local_map.py:289-299): the map becomes `pointcloud` [N,3] (float32, or
+        float64 rounded to float32), held as no frame.  Later updates move it and append frames; once more than
+        local_map_size frames are held, each eviction drops the oldest frame's row count from the front of the map --
+        prior-map rows first, as the reference does.  One divergence: a row with a NaN or an infinite coordinate raises
+        AssertionError and leaves the map unchanged (the reference stores it, and its search cannot handle it).
+        `normals` [N,3] is checked and, as in the reference, makes every search with normals raise IndexError until
+        the next update."""
+        check_tensor(pointcloud, [-1, 3])
+        if not isinstance(pointcloud, np.ndarray):  # the reference's check_tensor(.., np.ndarray): typeguard 2's TypeError
+            raise TypeError(f"{type(pointcloud).__module__}.{type(pointcloud).__name__} is not an instance of numpy.ndarray")
+        is64 = pointcloud.dtype == np.float64
+        pc = np.ascontiguousarray(pointcloud, dtype=np.float64 if is64 else np.float32)
+        self.ctx.call("pls_kdmap_set_points", _lib.ptr(pc), int(is64), pc.shape[0])
+        _set_given_normals(self.ctx, False)
+        if normals is not None:
+            check_tensor(normals, [*pointcloud.shape])
+            if not isinstance(normals, np.ndarray):
+                raise TypeError(f"{type(normals).__module__}.{type(normals).__name__} is not an instance of numpy.ndarray")
+            _set_given_normals(self.ctx, True)
+
+    def frame_counts(self) -> list:
+        """The point counts of the frames the map holds, oldest first (rows before them are a set cloud)."""
+        counts = np.zeros(max(int(self.ctx.cfg.local_map_size), 1) + 1, dtype=np.int64)
+        num = C.c_int(0)
+        self.ctx.call("pls_kdmap_frames", _lib.ptr(counts), C.byref(num))
+        return [int(c) for c in counts[:num.value]]
+
+    def get_last_frame(self) -> torch.Tensor:
+        """KdTreeLocalMap.get_last_frame (local_map.py:425-427): the rows of the last inserted frame, as a float32 CPU
+        tensor.  IndexError while no frame is held (after set_map_pointcloud or init); a last frame of zero rows gives
+        the whole map, as the reference's `[-0:]` slice does."""
+        counts = self.frame_counts()
+        if not counts:
+            raise IndexError("list index out of range")
+        return torch.from_numpy(self.points()[-counts[-1]:])
 
     def update(self, relative_pose, new_pc_data=None, new_vertex_map=None, **kwargs):
+        _set_given_normals(self.ctx, False)
         rel = _pose16(relative_pose)
         if new_pc_data is not None:
             pts = _f32c(new_pc_data.reshape(-1, 3))
@@ -159,6 +216,8 @@ class KdTreeLocalMap(LocalMap):
     def nearest_neighbor_search(self, target_points, with_normals: bool = True, with_new_target_points: bool = True,
                                 **kwargs):
         check_tensor(target_points, [-1, 3])
+        if with_normals:
+            _check_given_normals(self.ctx)
         q = _f32c(target_points)
         n = q.shape[0]
         nb = _new(q, (n, 3))
@@ -207,6 +266,17 @@ class ProjectiveLocalMap(LocalMap):
         n = np.empty((k.value, 3, H, W), dtype=np.float32)
         self.ctx.call("pls_projmap_model", _lib.ptr(v), _lib.ptr(n))
         return v, n
+
+    def get_last_frame(self) -> torch.Tensor:
+        """ProjectiveLocalMap.get_last_frame (local_map.py:238-240): projection_map_to_points of the newest vertex map,
+        [H*W,3] float32 on the CPU.  TypeError on a map that holds no frame (the reference indexes None)."""
+        k = C.c_int(0)
+        self.ctx.call("pls_projmap_num_frames", C.byref(k))
+        if k.value == 0:
+            raise TypeError("'NoneType' object is not subscriptable")
+        v = np.empty((3, self.projector.height, self.projector.width), dtype=np.float32)
+        self.ctx.call("pls_projmap_last_frame", _lib.ptr(v))
+        return torch.from_numpy(v).permute(1, 2, 0).reshape(-1, 3)
 
     def nearest_neighbor_search(self, target_points, with_normals: bool = True, with_new_target_points: bool = True,
                                 **kwargs):
@@ -722,6 +792,7 @@ class ICPFrameToModel(OdometryAlgorithm):
 
     # -- fine-grained entry kept for parity tests: register_new_frame (icp_odometry.py:248-299)
     def register_new_frame(self, target_points, initial_estimate=None, **kwargs):
+        _check_given_normals(self.ctx)
         pts = _f32c(target_points)
         T0 = None if initial_estimate is None else _pose16(initial_estimate)
         T, params = np.zeros((1, 4, 4), np.float32), np.zeros((1, 6), np.float32)
@@ -730,6 +801,36 @@ class ICPFrameToModel(OdometryAlgorithm):
         self.ctx.call("pls_register_frame", _lib.ptr(pts), pts.shape[0], _lib.ptr(T0), _lib.ptr(T), _lib.ptr(params),
                       _lib.ptr(losses), C.byref(iters))
         return params, T, list(losses[:iters.value])
+
+    def register_new_frame_hypotheses(self, target_points, initial_estimates):
+        """register_new_frame for B initial estimates [B,4,4] of one scan [n,3], in one call (pls_register_hypotheses;
+        no reference counterpart): relocalisation in a prior map registers a scan from many guesses -- a yaw sweep, a
+        grid of positions, place-recognition candidates -- and keeps the best converged result.  Registers against the
+        map this odometry's context holds (a KdTreeLocalMap built with ctx=self.ctx, e.g. after set_map_pointcloud)
+        and leaves it unchanged.  Returns (params [B,6], T [B,4,4], losses: B lists, iterations [B]); hypothesis b's are
+        what register_new_frame(target_points, initial_estimates[b]) returns, bit for bit.  A singular hypothesis does
+        not stop the others: it is logged, and last_hypotheses_status[b] holds each one's status (PLS_OK,
+        PLS_W_TINY_RESIDUAL or PLS_E_SINGULAR)."""
+        _check_given_normals(self.ctx)
+        check_tensor(target_points, [-1, 3])
+        pts = _f32c(target_points)
+        if isinstance(initial_estimates, torch.Tensor):
+            initial_estimates = initial_estimates.detach().cpu().numpy()
+        check_tensor(initial_estimates, [-1, 4, 4])
+        T0 = np.ascontiguousarray(initial_estimates, dtype=np.float32)
+        B, M = T0.shape[0], int(self.config.max_num_alignments)
+        T, params = np.zeros((B, 4, 4), np.float32), np.zeros((B, 6), np.float32)
+        losses = np.zeros((B, M), np.float32)
+        iters, status = np.zeros(B, np.int32), np.zeros(B, np.int32)
+        self.ctx.call("pls_register_hypotheses", _lib.ptr(pts), pts.shape[0], _lib.ptr(T0), B, _lib.ptr(T),
+                      _lib.ptr(params), _lib.ptr(losses), _lib.ptr(iters), _lib.ptr(status))
+        self.last_hypotheses_status = status
+        singular = np.flatnonzero(status == _lib.PLS_E_SINGULAR)
+        if singular.size:
+            import logging
+            logging.error(f"Invalid Jacobian in Gauss Newton minimization, the hessian is not invertible "
+                          f"(hypotheses {singular.tolist()})")
+        return params, T, [list(losses[b, :iters[b]]) for b in range(B)], iters
 
 
 class ICPFrameToModelBatch:
