@@ -87,7 +87,7 @@ typedef struct pls_config {
     float up_fov_deg, down_fov_deg; /* projector vertical field of view */
     int32_t local_map_type;         /* PLS_MAP_* */
     int32_t local_map_size;         /* frames kept (20) */
-    int32_t num_neighbors_normals;  /* kd map: k for normals (10) */
+    int32_t num_neighbors_normals;  /* kd map: k for normals (10), 3 <= k <= 255 */
     int32_t normals_kernel_size;    /* projective map: box size (5) */
     int32_t scheme;                 /* PLS_SCHEME_* */
     float sigma;                    /* scheme parameter */
@@ -103,6 +103,7 @@ typedef struct pls_config {
 
 /* ---- lifetime ------------------------------------------------------------------- */
 PLS_API int pls_config_default(pls_config* cfg);
+/* PLS_E_INVALID (nothing created) for a config out of range, e.g. num_neighbors_normals outside [3, 255]. */
 PLS_API int pls_create(const pls_config* cfg, pls_context** out);
 PLS_API int pls_destroy(pls_context* ctx);
 PLS_API const char* pls_last_error(pls_context* ctx);
@@ -202,8 +203,8 @@ PLS_API int pls_kdmap_size(pls_context* ctx, int64_t* num_points);
 PLS_API int pls_kdmap_stats(pls_context* ctx, unsigned long long* out16);
 PLS_API int pls_kdmap_points(pls_context* ctx, float* out /* [M,3], insertion order */);
 /* KdTreeLocalMap.nearest_neighbor_search (local_map.py:372-422): exact 1-NN; normals from
- * the 10 nearest map neighbours of the matched map point (smallest-eigenvalue direction),
- * cached per map point until the next update.  out_idx [n] (int64, insertion order) or NULL. */
+ * the cfg.num_neighbors_normals nearest map neighbours of the matched map point (smallest-eigenvalue
+ * direction), cached per map point until the next update.  out_idx [n] (int64, insertion order) or NULL. */
 PLS_API int pls_kdmap_nn_search(pls_context* ctx, const float* queries, int64_t n,
                         float* out_neighbors, float* out_normals, int64_t* out_idx);
 /* Test / debug aid: the correspondences of the last kd search of this context -- the last executed iteration of
@@ -216,7 +217,7 @@ PLS_API int pls_kdmap_nn_search(pls_context* ctx, const float* queries, int64_t 
  * run, if the map was rebuilt since, or if the last ICP split its queries over several ranks. */
 PLS_API int pls_kdmap_last_correspondences(pls_context* ctx, int64_t n, int64_t* out_idx, float* out_neighbors,
                                            float* out_normals, float* out_search_state, double* out_sums);
-/* Test / debug aid: the exact (k+1)-NN lists of the normals search (0 <= k <= 31) for n arbitrary query rows [n,3]
+/* Test / debug aid: the exact (k+1)-NN lists of the normals search (0 <= k <= 255) for n arbitrary query rows [n,3]
  * on the current index, ordered by (float32 squared distance, sorted position).  out_idx [n,k+1] insertion index or -1
  * past the map's size; out_d2 [n,k+1] the float32 squared distance (NaN where out_idx is -1); out_pos [n,k+1] the
  * position in the Morton-sorted point array or -1 (nullable).  Touches neither the normal cache nor any ICP state. */

@@ -260,6 +260,8 @@ class Context:
         self.cfg = cfg
         self.handle = _P()
         st = lib.pls_create(C.byref(cfg), C.byref(self.handle))
+        if st == PLS_E_INVALID and not 3 <= cfg.num_neighbors_normals <= 255:
+            raise AssertionError(f"num_neighbors_normals must be in [3, 255], got {cfg.num_neighbors_normals}")
         if st != PLS_OK:
             raise RuntimeError(f"pls_create failed with status {st}: a CUDA device and the sm_90a library are "
                                f"required (there is no CPU fallback)")

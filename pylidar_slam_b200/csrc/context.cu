@@ -2,6 +2,7 @@
 #include <utility>
 
 #include "internal.cuh"
+#include "kdmap_device.cuh"
 
 namespace pls {
 
@@ -259,7 +260,7 @@ int pls_create(const pls_config* cfg, pls_context** out) {
     if (cfg->device < 0 || cfg->device >= ndev) return PLS_E_INVALID;
     if (cfg->height <= 0 || cfg->width <= 0 || cfg->local_map_size <= 0) return PLS_E_INVALID;
     if (cfg->max_num_alignments < 1 || cfg->max_num_alignments > kMaxAlign) return PLS_E_INVALID;
-    if (cfg->num_neighbors_normals < 3 || cfg->num_neighbors_normals > 31) return PLS_E_INVALID;
+    if (cfg->num_neighbors_normals < 3 || cfg->num_neighbors_normals + 1 > KD_KMAX_WIDE) return PLS_E_INVALID;
     if (cfg->normals_kernel_size < 1 || cfg->normals_kernel_size > 9 || (cfg->normals_kernel_size % 2) == 0)
         return PLS_E_INVALID;
     pls_context* ctx = new pls_context();

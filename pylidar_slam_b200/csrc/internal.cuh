@@ -401,8 +401,9 @@ void kdmap_update(pls_context* ctx, const float* rel_pose_host, const float* pts
 void kdmap_update_packed(pls_context* ctx, const float* rel_pose_host, const float4* fresh_dev, int64_t num_new,
                          bool has_new);
 // pls_process_frames: the ICP of `num` sequences (distinct kd-map contexts, no communicator) in batched launches on st.
-// begin uploads their descriptors into lead->batch_buf and returns the launch widths in grid[5]; iterations enqueues
+// begin uploads their descriptors into lead->batch_buf and returns the launch widths in grid[KD_BATCH_GRID]; iterations enqueues
 // ICP iterations [first, last) of all of them; done reads every sequence's done flag with one copy and one sync.
+constexpr int KD_BATCH_GRID = 6;
 void kdmap_batch_begin(pls_context* lead, pls_context* const* ctxs, const int64_t* query_bounds, int num, cudaStream_t st,
                        int* grid);
 void kdmap_batch_iterations(pls_context* lead, int num, cudaStream_t st, const int* grid, int first, int last);

@@ -241,7 +241,8 @@ __global__ void kd_export_kernel(const float4* __restrict__ pts, int64_t n, floa
 //   p = T p0; q = NN(p); n = normal(q); r = n.(p - q); J = [n, p x n]; w; reduce
 // A frame's first iteration is three launches: kd_nn_warp_kernel, kd_normals_warp_kernel and kd_residual_kernel, which
 // also runs the solve in its last block.  Every later iteration is one launch, kd_icp_refine_kernel, or, on maps of
-// KD_COLD_MAP_POINTS or more, four: kd_nn_verify_kernel and the same three on the queries it could not prove.
+// KD_COLD_MAP_POINTS or more and for k > 31 normal neighbours (kd_later_four_launch), four: kd_nn_verify_kernel and the
+// same three on the queries it could not prove.
 // KD_THREADS is the block size of the kernels that own a thread per query, and the number of query slots of a
 // kd_icp_refine_kernel block: both striding and block partials follow from it.
 constexpr int KD_THREADS = 256;
@@ -347,12 +348,20 @@ __device__ __forceinline__ bool match_proven(const KdIndex& ix, const float* p, 
     return (d + eps) * 1.00001f + 1e-6f < sqrtf(s.w);
 }
 
-// Second moments of map point c's k nearest OTHER map points, from its exact (k+1)-NN by the whole warp.
+// Second moments of map point c's k nearest OTHER map points, from its exact (k+1)-NN by the whole warp.  R = 1: k <= 31
+// (warp_knn); else the wide list of R keys per lane, k + 1 <= 32 R (warp_knn_wide).
+template <int R = 1>
 __device__ __forceinline__ void warp_normal_moments(const KdIndex& ix, const KdGridLocal& g, const float4& c, int k, int lane,
                                                     int* cand, unsigned long long* stage, float* cov) {
-    int ni;
-    const int found = warp_knn(ix, g, c.x, c.y, c.z, k + 1, lane, ni, cand, stage);
-    warp_second_moments(ix, c, k, found, ni, lane, cov);
+    if constexpr (R == 1) {
+        int ni;
+        const int found = warp_knn(ix, g, c.x, c.y, c.z, k + 1, lane, ni, cand, stage);
+        warp_second_moments(ix, c, k, found, ni, lane, cov);
+    } else {
+        unsigned long long kept[R];
+        const int found = warp_knn_wide<R>(ix, g, c.x, c.y, c.z, k + 1, lane, kept, cand, stage);
+        warp_second_moments_wide<R>(ix, c, k, found, kept, lane, cov);
+    }
 }
 
 // The normal of map point `pos` from its second moments, stored with `valid`, the state word kd_normal_valid(ix.gen).
@@ -523,8 +532,10 @@ kd_nn_warp_kernel(KdIndex ix, const float4* __restrict__ queries, const uint32_t
                     pending, counters, blockIdx.x, gridDim.x);
 }
 
-// Normals: a warp per queued map point, exact (k+1)-NN over the cell pyramid (warp_knn), second moments; the
-// eigen-solves are deferred and run lane-parallel (each lane one point) so that no warp idles behind a serial solve.
+// Normals: a warp per queued map point, exact (k+1)-NN over the cell pyramid (warp_knn, or warp_knn_wide<R> for R > 1),
+// second moments; the eigen-solves are deferred and run lane-parallel (each lane one point) so that no warp idles behind
+// a serial solve.
+template <int R = 1>
 __device__ __forceinline__ void kd_normals_warp_body(const KdIndex& ix, int k_normals, const int* __restrict__ worklist,
                                                      const uint32_t* __restrict__ wl_count, const int* __restrict__ done,
                                                      unsigned long long* __restrict__ counters, unsigned block, unsigned grid) {
@@ -553,7 +564,7 @@ __device__ __forceinline__ void kd_normals_warp_body(const KdIndex& ix, int k_no
             cn = __ldg(ix.sorted + posn);
         }
         float cov[6];
-        warp_normal_moments(ix, g, c, k_normals, lane, &cand, stage, cov);
+        warp_normal_moments<R>(ix, g, c, k_normals, lane, &cand, stage, cov);
         if (lane == held) {
 #pragma unroll
             for (int a = 0; a < 6; ++a) mycov[a] = cov[a];
@@ -585,6 +596,16 @@ kd_normals_warp_kernel(KdIndex ix, int k_normals, const int* __restrict__ workli
                        const int* __restrict__ done, unsigned long long* __restrict__ counters) {
     pls_grid_dependency_wait();
     kd_normals_warp_body(ix, k_normals, worklist, wl_count, done, counters, blockIdx.x, gridDim.x);
+}
+
+// The same for a wide k: k + 1 in 33 ... 32 R.  Launched with KD_THREADS threads.  Left to its default, ptxas gives this
+// kernel 80 registers and spills the list across the division slow paths' calls; 128 (two blocks per SM) it fits in.
+template <int R>
+__global__ void __maxnreg__(128)
+kd_normals_wide_kernel(KdIndex ix, int k_normals, const int* __restrict__ worklist, const uint32_t* __restrict__ wl_count,
+                       const int* __restrict__ done, unsigned long long* __restrict__ counters) {
+    pls_grid_dependency_wait();
+    kd_normals_warp_body<R>(ix, k_normals, worklist, wl_count, done, counters, blockIdx.x, gridDim.x);
 }
 
 // A thread per query: accumulate_match -> block partials; the last block sums them in fixed order and runs the solve,
@@ -758,7 +779,7 @@ struct KdSeq {
     float fuse_threshold;
     int max_iters;              // max_num_alignments: launches of later iterations leave the sequence alone
     int blocks;                 // grid_for(query bound): the residual kernel's geometry on the single path
-    int refine_blocks;          // blocks, or 0 on a map of KD_COLD_MAP_POINTS or more (the four-launch path)
+    int refine_blocks;          // blocks, or 0 where later iterations take the four launches (kd_later_four_launch)
     int verify_blocks;          // kd_nn_verify_kernel's grid on the single path: a thread per query
     int nn_blocks, kn_blocks;   // its share of the resident wave of the 1-NN / normals kernels
 };
@@ -805,12 +826,24 @@ __global__ void __launch_bounds__(KD_THREADS) kd_nn_warp_batch_kernel(const KdSe
                     s.match, s.nn_state, 1, s.pending, s.counters, blockIdx.x, s.nn_blocks);
 }
 
+// The normals of the sequences whose k is at most 31; kd_normals_wide_batch_kernel<R> takes the others.
 __global__ void __launch_bounds__(KD_THREADS) kd_normals_warp_batch_kernel(const KdSeq* __restrict__ seqs, int it) {
     __shared__ KdSeq s;
     load_seq(seqs, s);
-    if ((int)blockIdx.x >= s.kn_blocks || !four_launch_step(s, it)) return;
+    if ((int)blockIdx.x >= s.kn_blocks || !four_launch_step(s, it) || kd_wide_k(s.k_normals)) return;
     kd_normals_warp_body(s.ix, s.k_normals, s.pending, s.lists + KDL_PENDING + (it & 1), &s.fr->done, s.counters,
                          blockIdx.x, s.kn_blocks);
+}
+
+// The normals of the sequences with a wide k, k + 1 <= 32 R.  Which warp computes a normal does not change its bits, so
+// the sequences share the block counts of the narrow kernel.
+template <int R>
+__global__ void __launch_bounds__(KD_THREADS) kd_normals_wide_batch_kernel(const KdSeq* __restrict__ seqs, int it) {
+    __shared__ KdSeq s;
+    load_seq(seqs, s);
+    if ((int)blockIdx.x >= s.kn_blocks || !four_launch_step(s, it) || !kd_wide_k(s.k_normals)) return;
+    kd_normals_warp_body<R>(s.ix, s.k_normals, s.pending, s.lists + KDL_PENDING + (it & 1), &s.fr->done, s.counters,
+                            blockIdx.x, s.kn_blocks);
 }
 
 __global__ void __launch_bounds__(KD_THREADS) kd_residual_batch_kernel(const KdSeq* __restrict__ seqs, int it) {
@@ -822,7 +855,7 @@ __global__ void __launch_bounds__(KD_THREADS) kd_residual_batch_kernel(const KdS
                      blockIdx.x, s.blocks KD_SPLIT_PASS);
 }
 
-// Iteration `it` (>= 1) of every sequence that has not reached its max_iters and whose map is below KD_COLD_MAP_POINTS.
+// Iteration `it` (>= 1) of every sequence that has not reached its max_iters and whose later iterations take one launch.
 __global__ void __launch_bounds__(KD_REFINE_THREADS) kd_icp_refine_batch_kernel(const KdSeq* __restrict__ seqs, int it) {
     __shared__ KdSeq s;
     load_seq(seqs, s);
@@ -885,6 +918,39 @@ kd_knn_export_kernel(KdIndex ix, const float* __restrict__ rows, int64_t n, int 
             out_idx[q * K + lane] = idx;
             out_d2[q * K + lane] = d2;
             if (out_pos) out_pos[q * K + lane] = pos;
+        }
+    }
+}
+
+// The same for 32 < K <= 32 R (warp_knn_wide): lane l writes entries l, l + 32, ... of the row.  KD_THREADS threads;
+// the register cap is kd_normals_wide_kernel's.
+template <int R>
+__global__ void __maxnreg__(128)
+kd_knn_wide_export_kernel(KdIndex ix, const float* __restrict__ rows, int64_t n, int K, long long* __restrict__ out_idx,
+                          float* __restrict__ out_d2, int* __restrict__ out_pos) {
+    __shared__ unsigned long long s_stage[KD_WARPS][KNN_STAGE];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const KdGridLocal g = kd_load_grid(ix);
+    const float nan = __int_as_float(0x7fc00000);
+    for (int64_t q = (int64_t)blockIdx.x * KD_WARPS + warp; q < n; q += (int64_t)gridDim.x * KD_WARPS) {
+        const float x = rows[3 * q], y = rows[3 * q + 1], z = rows[3 * q + 2];
+        unsigned long long kept[R];
+        warp_knn_wide<R>(ix, g, x, y, z, K, lane, kept, nullptr, s_stage[warp]);
+#pragma unroll
+        for (int r = 0; r < R; ++r) {
+            const int j = r * 32 + lane;
+            if (j >= K) break;
+            const int pos = kept[r] != KNN_NONE ? (int)(unsigned)kept[r] : -1;
+            long long idx = -1;
+            float d2 = nan;
+            if (pos >= 0) {
+                const float4 s = __ldg(ix.sorted + pos);
+                idx = (long long)__float_as_uint(s.w);
+                d2 = dist2_point(x, y, z, s);
+            }
+            out_idx[q * K + j] = idx;
+            out_d2[q * K + j] = d2;
+            if (out_pos) out_pos[q * K + j] = pos;
         }
     }
 }
@@ -1169,6 +1235,15 @@ static KdPlan plan_kd_iteration(pls_context* ctx, int64_t query_bound, int num_r
     return p;
 }
 
+// kd_normals_wide_kernel<R> over the queued map points, at most one resident wave.
+template <int R>
+static void launch_normals_wide(pls_context* ctx, int wblocks, const KdIndex& ix, const int* pending, const uint32_t* count,
+                                const int* done, unsigned long long* counters) {
+    static const int resident = resident_blocks((const void*)kd_normals_wide_kernel<R>);
+    launch_dependent(kd_normals_wide_kernel<R>, wblocks < resident ? wblocks : resident, KD_THREADS, ctx->stream, ix,
+                     ctx->cfg.num_neighbors_normals, pending, count, done, counters);
+}
+
 // The search of one ICP iteration (or of one fine-grained API call).  first: every query is searched; later iterations
 // first verify the previous matches and search only the unproven ones.
 static void launch_search(pls_context* ctx, const KdPlan& plan, const KdIndex& ix, const float4* queries, const uint32_t* nq_dev,
@@ -1198,8 +1273,17 @@ static void launch_search(pls_context* ctx, const KdPlan& plan, const KdIndex& i
     }
     if (!normals) return;
     ProfileScope p9(ctx, 9, 0.0);
-    launch_dependent(kd_normals_warp_kernel, wblocks < resident_kn ? wblocks : resident_kn, KD_THREADS, st, ix,
-                     ctx->cfg.num_neighbors_normals, pending, lists + KDL_PENDING + parity, done, counters);
+    const int k = ctx->cfg.num_neighbors_normals;
+    if (!kd_wide_k(k)) {
+        launch_dependent(kd_normals_warp_kernel, wblocks < resident_kn ? wblocks : resident_kn, KD_THREADS, st, ix, k, pending,
+                         lists + KDL_PENDING + parity, done, counters);
+        return;
+    }
+    switch (kd_wide_regs(k + 1)) {
+        case 2: launch_normals_wide<2>(ctx, wblocks, ix, pending, lists + KDL_PENDING + parity, done, counters); break;
+        case 4: launch_normals_wide<4>(ctx, wblocks, ix, pending, lists + KDL_PENDING + parity, done, counters); break;
+        default: launch_normals_wide<8>(ctx, wblocks, ix, pending, lists + KDL_PENDING + parity, done, counters); break;
+    }
 }
 
 // Later ICP iterations run as one kd_icp_refine_kernel, except on maps of this many points or more.  On the 5 M-point
@@ -1207,6 +1291,11 @@ static void launch_search(pls_context* ctx, const KdPlan& plan, const KdIndex& i
 // the four launches; the same with the kernel at 120 registers and no spills), on the 0.65 M-point cfg2 map faster.
 // The cut-off between the two is not tuned: no map size in between has been measured.
 constexpr int64_t KD_COLD_MAP_POINTS = 2000000;
+
+// Do an ICP's later iterations on a map of `indexed` points with k normal neighbours take the four launches (verify /
+// 1-NN / normals / residual) rather than kd_icp_refine_kernel?  On large maps (above), and for a wide k: the refine
+// kernel computes normals inline with the one-key-per-lane warp_knn only, so its registers stay those of k <= 31.
+static bool kd_later_four_launch(int64_t indexed, int k) { return indexed >= KD_COLD_MAP_POINTS || kd_wide_k(k); }
 
 // One ICP iteration over the device-resident queries (float4 in ctx->query_ptr, count in the FrameResult); writes
 // block partials to ctx->partials and returns the block count.
@@ -1223,7 +1312,7 @@ int kdmap_icp_iteration(pls_context* ctx, int64_t query_bound, const uint32_t* b
     const KdPlan plan = plan_kd_iteration(ctx, query_bound, num_ranks);
     const int blocks = plan.blocks;
     record_search(ctx->kd, true, num_ranks > 1, true, 0);
-    if (it == 0 || ctx->kd.indexed >= KD_COLD_MAP_POINTS) {
+    if (it == 0 || kd_later_four_launch(ctx->kd.indexed, ctx->cfg.num_neighbors_normals)) {
         launch_search(ctx, plan, ix, ctx->query_ptr, nq_dev, rank, num_ranks, fr->T, &fr->done, ctx->nn_prev.as<int>(), it == 0,
                       true, it & 1);
         ProfileScope p10(ctx, 10, 0.0);
@@ -1263,7 +1352,7 @@ static KdSeq make_seq(pls_context* ctx, const KdPlan& plan, FrameResult* fr, con
     s.fuse_threshold = ctx->cfg.threshold_delta_pose;
     s.max_iters = ctx->cfg.max_num_alignments;
     s.blocks = plan.blocks;
-    s.refine_blocks = ctx->kd.indexed >= KD_COLD_MAP_POINTS ? 0 : plan.blocks;
+    s.refine_blocks = kd_later_four_launch(ctx->kd.indexed, ctx->cfg.num_neighbors_normals) ? 0 : plan.blocks;
     s.verify_blocks = (int)((plan.mine + KD_THREADS - 1) / KD_THREADS);
     s.nn_blocks = plan.wblocks < share_nn ? plan.wblocks : share_nn;
     s.kn_blocks = plan.wblocks < share_kn ? plan.wblocks : share_kn;
@@ -1274,13 +1363,17 @@ static KdSeq make_seq(pls_context* ctx, const KdPlan& plan, FrameResult* fr, con
 // lead->batch_buf on st.
 static void upload_seqs(pls_context* lead, const std::vector<KdSeq>& seqs, cudaStream_t st, int* grid) {
     grid[0] = grid[1] = grid[2] = 1;
-    grid[3] = grid[4] = 0;
+    grid[3] = grid[4] = grid[5] = 0;
     for (const KdSeq& s : seqs) {
         grid[0] = grid[0] > s.blocks ? grid[0] : s.blocks;
         grid[1] = grid[1] > s.nn_blocks ? grid[1] : s.nn_blocks;
         grid[2] = grid[2] > s.kn_blocks ? grid[2] : s.kn_blocks;
         if (s.refine_blocks == 0) grid[3] = grid[3] > s.verify_blocks ? grid[3] : s.verify_blocks;
         else grid[4] = 1;
+        if (kd_wide_k(s.k_normals)) {
+            const int r = kd_wide_regs(s.k_normals + 1);
+            grid[5] = grid[5] > r ? grid[5] : r;
+        }
     }
     const size_t bytes = seqs.size() * sizeof(KdSeq);
     lead->batch_buf.reserve(bytes + PLS_MAX_SEQUENCES * sizeof(int), st);
@@ -1289,8 +1382,9 @@ static void upload_seqs(pls_context* lead, const std::vector<KdSeq>& seqs, cudaS
 
 // pls_process_frames: the descriptors of the sequences whose ICP runs in this call, into lead->batch_buf (uploaded on
 // st), and every buffer their iterations use reserved as their single path reserves it.
-// grid[5]: the launch widths, the largest residual / 1-NN / normals block count of a sequence, the largest verify block
-// count of a sequence on a map of KD_COLD_MAP_POINTS or more (0: none is), and 1 if any sequence's map is smaller.
+// grid[KD_BATCH_GRID]: the launch widths, the largest residual / 1-NN / normals block count of a sequence, the largest
+// verify block count of a sequence whose later iterations take the four launches (0: none does), 1 if any sequence's
+// take kd_icp_refine_kernel, and the keys per lane R of the widest k above 31 (0: every k is at most 31).
 void kdmap_batch_begin(pls_context* lead, pls_context* const* ctxs, const int64_t* query_bounds, int num, cudaStream_t st,
                        int* grid) {
     static const int resident_nn = resident_blocks((const void*)kd_nn_warp_batch_kernel);
@@ -1312,8 +1406,9 @@ void kdmap_batch_begin(pls_context* lead, pls_context* const* ctxs, const int64_
 }
 
 // ICP iterations [first, last) of the sequences kdmap_batch_begin (or kdmap_hypotheses_begin) described, on st: one
-// launch per kernel for all of them.  A later iteration is kd_icp_refine_batch_kernel for the sequences on maps below
-// KD_COLD_MAP_POINTS and the four launches verify / 1-NN / normals / residual for the others; no launch grows with num.
+// launch per kernel for all of them.  A later iteration is kd_icp_refine_batch_kernel for the sequences whose later
+// iterations take one launch and the four launches verify / 1-NN / normals / residual for the others; the normals of a
+// wide k are one more launch, made only if some sequence has one.  No launch grows with num.
 void kdmap_batch_iterations(pls_context* lead, int num, cudaStream_t st, const int* grid, int first, int last) {
     const KdSeq* seqs = lead->batch_buf.as<KdSeq>();
     for (int it = first; it < last; ++it) {
@@ -1330,6 +1425,13 @@ void kdmap_batch_iterations(pls_context* lead, int num, cudaStream_t st, const i
         PLS_CHECK_LAUNCH();
         kd_normals_warp_batch_kernel<<<dim3(grid[2], num), KD_THREADS, 0, st>>>(seqs, it);
         PLS_CHECK_LAUNCH();
+        if (grid[5]) {
+            const dim3 g(grid[2], num);
+            if (grid[5] == 2) kd_normals_wide_batch_kernel<2><<<g, KD_THREADS, 0, st>>>(seqs, it);
+            else if (grid[5] == 4) kd_normals_wide_batch_kernel<4><<<g, KD_THREADS, 0, st>>>(seqs, it);
+            else kd_normals_wide_batch_kernel<8><<<g, KD_THREADS, 0, st>>>(seqs, it);
+            PLS_CHECK_LAUNCH();
+        }
         kd_residual_batch_kernel<<<dim3(grid[0], num), KD_THREADS, 0, st>>>(seqs, it);
         PLS_CHECK_LAUNCH();
     }
@@ -1338,7 +1440,7 @@ void kdmap_batch_iterations(pls_context* lead, int num, cudaStream_t st, const i
 // pls_register_hypotheses: the ICP state of `num` hypotheses of one scan (ctx->query_ptr, count in ctx's FrameResult) on
 // ctx's map, each a slice of ctx->hyp_buf laid out as pls_register_frame's own buffers; their descriptors into
 // ctx->batch_buf.  Returns the hypotheses' FrameResults (contiguous) and their 16 counter and work-list words each, for
-// the caller to initialise before the first iteration; grid[5] as kdmap_batch_begin.
+// the caller to initialise before the first iteration; grid as kdmap_batch_begin.
 void kdmap_hypotheses_begin(pls_context* ctx, int64_t query_bound, int num, cudaStream_t st, int* grid, FrameResult** frs,
                             uint32_t** words) {
     PLS_REQUIRE(ctx->kd.valid, "kd map: search before any update");
@@ -1549,7 +1651,7 @@ int pls_kdmap_knn(pls_context* ctx, const float* queries, int64_t n, int k, int6
     PLS_API_BEGIN(ctx)
     map_stream_wait(ctx);
     PLS_REQUIRE(queries && out_idx && out_d2 && n > 0, "pls_kdmap_knn: bad arguments");
-    PLS_REQUIRE(k >= 0 && k + 1 <= KD_KMAX, "pls_kdmap_knn: k must be in [0, 31]");
+    PLS_REQUIRE(k >= 0 && k + 1 <= KD_KMAX_WIDE, "pls_kdmap_knn: k must be in [0, 255]");
     if (!ctx->kd.valid) throw pls::Error{PLS_E_STATE, "pls_kdmap_knn: the map is empty"};
     const int K = k + 1;
     const size_t entries = (size_t)n * K;
@@ -1557,8 +1659,16 @@ int pls_kdmap_knn(pls_context* ctx, const float* queries, int64_t n, int k, int6
     OutArg oix = out_arg(ctx, out_idx, entries * sizeof(int64_t), ctx->stage_out[0]);
     OutArg od2 = out_arg(ctx, out_d2, entries * sizeof(float), ctx->stage_out[1]);
     OutArg ops = out_arg(ctx, out_pos, entries * sizeof(int32_t), ctx->stage_out[2]);
-    kd_knn_export_kernel<<<grid_for(n, KD_THREADS / 32, 8 * kNumSMs), KD_THREADS, 0, ctx->stream>>>(
-        make_index(ctx), d, n, K, (long long*)oix.dev, (float*)od2.dev, (int*)ops.dev);
+    const int blocks = grid_for(n, KD_THREADS / 32, 8 * kNumSMs);
+    const KdIndex ix = make_index(ctx);
+    long long* pi = (long long*)oix.dev;
+    float* pd = (float*)od2.dev;
+    int* pp = (int*)ops.dev;
+    cudaStream_t st = ctx->stream;
+    if (K <= KD_KMAX) kd_knn_export_kernel<<<blocks, KD_THREADS, 0, st>>>(ix, d, n, K, pi, pd, pp);
+    else if (kd_wide_regs(K) == 2) kd_knn_wide_export_kernel<2><<<blocks, KD_THREADS, 0, st>>>(ix, d, n, K, pi, pd, pp);
+    else if (kd_wide_regs(K) == 4) kd_knn_wide_export_kernel<4><<<blocks, KD_THREADS, 0, st>>>(ix, d, n, K, pi, pd, pp);
+    else kd_knn_wide_export_kernel<8><<<blocks, KD_THREADS, 0, st>>>(ix, d, n, K, pi, pd, pp);
     PLS_CHECK_LAUNCH();
     finish_out(ctx, oix);
     finish_out(ctx, od2);

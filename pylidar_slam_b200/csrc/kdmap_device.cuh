@@ -34,7 +34,8 @@ constexpr int KD_MIN_B0 = 3;                            // level-0 cell ids then
 constexpr int KD_MAX_LEVELS = KD_COORD_BITS - KD_MIN_B0 + 1;  // levels 0 .. top, top <= 10
 constexpr float KD_CELL_TARGET = 0.20f;   // default level-0 cell side, metres (PLS_KD_CELL overrides)
 constexpr float KD_CELL_MARGIN = 2e-3f;   // quantisation slack, metres
-constexpr int KD_KMAX = 32;               // k + 1 <= 32
+constexpr int KD_KMAX = 32;               // k + 1 <= 32: warp_knn, one key per lane
+constexpr int KD_KMAX_WIDE = 256;         // k + 1 <= 256: warp_knn_wide, up to 8 keys per lane
 constexpr unsigned FULL = 0xffffffffu;
 
 struct KdGridHeader {
@@ -453,6 +454,170 @@ __device__ __forceinline__ void warp_second_moments(const KdIndex& ix, const flo
     cov[0] = __fdiv_rn(sxx, kk); cov[1] = __fdiv_rn(sxy, kk); cov[2] = __fdiv_rn(sxz, kk);
     cov[3] = __fdiv_rn(syy, kk); cov[4] = __fdiv_rn(syz, kk); cov[5] = __fdiv_rn(szz, kk);
 }
+
+// ---- wide lists: K = k + 1 in 33 ... 256 ---------------------------------------------------------------------------
+// A list of 32 R keys lives in R registers per lane, entry e = r * 32 + lane in register r: entry j of a neighbour list is
+// in lane j % 32, register j / 32.  Keys are unique (they carry the sorted position), so the order is total.
+
+// The key of entry r * 32 + sel_lane, every lane (r warp-uniform; a select chain keeps the list in registers).
+template <int R>
+__device__ __forceinline__ unsigned long long wide_entry(const unsigned long long (&a)[R], int r, int sel_lane) {
+    unsigned long long v = a[0];
+#pragma unroll
+    for (int j = 1; j < R; ++j)
+        if (j == r) v = a[j];
+    return __shfl_sync(FULL, v, sel_lane);
+}
+
+// The 32 R smallest of an ascending list `a` of 32 R keys and an ascending 32-key list b (one per lane), ascending in a.
+// Padded with KNN_NONE to 32 R entries and reversed, b is non-increasing; its element-wise minimum with a is a bitonic
+// sequence holding the 32 R smallest, which log2(32 R) merge stages sort: the strides of 32 and more pair registers of
+// one lane, the shorter ones lanes of one register.
+template <int R>
+__device__ __forceinline__ void warp_merge_wide(unsigned long long (&a)[R], unsigned long long b, int lane) {
+    a[R - 1] = min(a[R - 1], __shfl_sync(FULL, b, 31 - lane));
+#pragma unroll
+    for (int j = R / 2; j > 0; j >>= 1) {
+#pragma unroll
+        for (int r = 0; r < R; ++r) {
+            if ((r & j) == 0) {
+                const unsigned long long lo = min(a[r], a[r + j]), hi = max(a[r], a[r + j]);
+                a[r] = lo;
+                a[r + j] = hi;
+            }
+        }
+    }
+#pragma unroll
+    for (int j = 16; j > 0; j >>= 1) {
+#pragma unroll
+        for (int r = 0; r < R; ++r) {
+            const unsigned long long o = __shfl_xor_sync(FULL, a[r], j);
+            a[r] = (lane & j) ? max(a[r], o) : min(a[r], o);
+        }
+    }
+}
+
+// Exact K-NN for 32 < K <= 32 R (warp-uniform): the same list as warp_knn would give with room for K keys -- the order
+// (float32 d^2, sorted position), the cell-pyramid walk, the overflowed-level rule and the bound of the finer level's
+// K-th key.  On return entry j < found of `kept` (lane j % 32, register j / 32) holds the key of the j-th nearest point,
+// entries past it KNN_NONE; returns found = min(K, M).  `stage` is a warp-private shared buffer of KNN_STAGE keys.
+// Every level streams its candidates: the keys at or below the bound are compacted into `stage`, and every 32 of them
+// are sorted (warp_sort_keys) and merged into the level's running list (warp_merge_wide).  Once that list holds K keys,
+// its K-th key bounds the level's remaining candidates too.  No level keeps the finer level's list: each rebuilds its
+// own from its block.
+template <int R>
+__device__ __forceinline__ int warp_knn_wide(const KdIndex& ix, const KdGridLocal& g, float x, float y, float z, int K,
+                                             int lane, unsigned long long (&kept)[R], int* cand_out,
+                                             unsigned long long* stage) {
+#pragma unroll
+    for (int r = 0; r < R; ++r) kept[r] = KNN_NONE;
+    unsigned long long bound = KNN_NONE;  // K-th key of the previous (finer) level
+    float bound_d = FLT_MAX;              // ... its distance
+    int found = 0;
+    const int kr = (K - 1) >> 5, kl = (K - 1) & 31;  // where entry K - 1 lives
+    if (lane == 0) kd_stat(ix, 4);
+    const unsigned lanes_below = (1u << lane) - 1u;
+    for (int level = 0; level <= g.top; ++level) {
+        int start, count;
+        float box2;
+        const float r2 = warp_probe_block(ix, g, level, x, y, z, lane, start, count, box2);
+        if (r2 < 0.f) {  // this level's table overflowed: nothing scanned, the list of the finer level stands
+            if (ix.stats && lane == 0 && level == 0) kd_stat(ix, 6);
+            continue;
+        }
+        if (box2 > bound_d) count = 0;
+        int incl;
+        const int total = warp_scan_counts(count, lane, incl);
+        const int adj = start - (incl - count);
+        if (cand_out) *cand_out += total;
+        if (ix.stats && lane == 0) kd_stat(ix, 7, (unsigned long long)total);
+        unsigned long long best[R];
+#pragma unroll
+        for (int r = 0; r < R; ++r) best[r] = KNN_NONE;
+        unsigned long long cut = bound;  // keys above it cannot enter this level's K
+        int staged = 0;
+        for (int base = 0; base < total; base += 32) {
+            const int t = base + lane;
+            const bool active = t < total;
+            const int idx = warp_candidate(incl, adj, active ? t : total - 1);
+            unsigned long long key = KNN_NONE;
+            if (active) key = knn_key(dist2_point(x, y, z, __ldg(ix.sorted + idx)), idx);
+            const bool keep = active && key <= cut;
+            const unsigned b = __ballot_sync(FULL, keep);
+            if (keep) stage[staged + __popc(b & lanes_below)] = key;
+            staged += __popc(b);
+            if (staged >= 32) {
+                __syncwarp();
+                warp_merge_wide<R>(best, warp_sort_keys(stage[lane], lane), lane);
+                __syncwarp();
+                if (lane < staged - 32) stage[lane] = stage[32 + lane];
+                staged -= 32;
+                __syncwarp();
+                cut = min(cut, wide_entry<R>(best, kr, kl));
+            }
+        }
+        if (staged > 0) {
+            __syncwarp();
+            warp_merge_wide<R>(best, warp_sort_keys(lane < staged ? stage[lane] : KNN_NONE, lane), lane);
+        }
+        __syncwarp();  // `stage` is reused by the next level
+        found = 0;
+#pragma unroll
+        for (int r = 0; r < R; ++r) {
+            kept[r] = r * 32 + lane < K ? best[r] : KNN_NONE;
+            found += __popc(__ballot_sync(FULL, kept[r] != KNN_NONE));
+        }
+        const unsigned long long kth = wide_entry<R>(kept, kr, kl);
+        const bool exact = (found == K && __uint_as_float((unsigned)(kth >> 32)) <= r2) || level >= g.top;
+        if (ix.stats && lane == 0 && level == 0) kd_stat(ix, exact ? 5 : 6);
+        if (exact) break;
+        if (found == K) {
+            bound = kth;
+            bound_d = __uint_as_float((unsigned)(kth >> 32));
+        }
+    }
+    return found;
+}
+
+// warp_second_moments over a wide list: the same float32 arithmetic, neighbours 1 .. found - 1 summed sequentially in
+// list order (entry j in lane j % 32, register j / 32) and divided by k.  Every lane returns the same six moments.
+template <int R>
+__device__ __forceinline__ void warp_second_moments_wide(const KdIndex& ix, const float4& c, int k, int found,
+                                                         const unsigned long long (&kept)[R], int lane, float* cov) {
+    float dx[R], dy[R], dz[R];
+#pragma unroll
+    for (int r = 0; r < R; ++r) {
+        const int j = r * 32 + lane;
+        dx[r] = dy[r] = dz[r] = 0.f;
+        if (j >= 1 && j < found) {
+            const float4 q = __ldg(ix.sorted + (int)(unsigned)kept[r]);
+            dx[r] = __fsub_rn(q.x, c.x);
+            dy[r] = __fsub_rn(q.y, c.y);
+            dz[r] = __fsub_rn(q.z, c.z);
+        }
+    }
+    float sxx = 0.f, sxy = 0.f, sxz = 0.f, syy = 0.f, syz = 0.f, szz = 0.f;
+#pragma unroll
+    for (int r = 0; r < R; ++r) {
+        const int n = min(found - r * 32, 32);
+        for (int l = r == 0 ? 1 : 0; l < n; ++l) {
+            const float bx = __shfl_sync(FULL, dx[r], l), by = __shfl_sync(FULL, dy[r], l), bz = __shfl_sync(FULL, dz[r], l);
+            sxx = __fadd_rn(sxx, __fmul_rn(bx, bx));
+            sxy = __fadd_rn(sxy, __fmul_rn(bx, by));
+            sxz = __fadd_rn(sxz, __fmul_rn(bx, bz));
+            syy = __fadd_rn(syy, __fmul_rn(by, by));
+            syz = __fadd_rn(syz, __fmul_rn(by, bz));
+            szz = __fadd_rn(szz, __fmul_rn(bz, bz));
+        }
+    }
+    const float kk = (float)k;
+    cov[0] = __fdiv_rn(sxx, kk); cov[1] = __fdiv_rn(sxy, kk); cov[2] = __fdiv_rn(sxz, kk);
+    cov[3] = __fdiv_rn(syy, kk); cov[4] = __fdiv_rn(syz, kk); cov[5] = __fdiv_rn(szz, kk);
+}
+
+// Does k normal neighbours take the wide list (k + 1 > KD_KMAX)?  Its keys per lane for K = k + 1 entries: 2, 4 or 8.
+__host__ __device__ constexpr bool kd_wide_k(int k) { return k + 1 > KD_KMAX; }
+__host__ __device__ constexpr int kd_wide_regs(int K) { return K <= 64 ? 2 : (K <= 128 ? 4 : 8); }
 
 // State words of the normal cache.
 __device__ __forceinline__ uint32_t kd_normal_claimed(uint32_t gen) { return 2u * gen; }

@@ -909,7 +909,7 @@ int pls_register_hypotheses(pls_context* ctx, const float* points, int64_t n, co
     int first_error = PLS_OK, last = 0;
     for (int c0 = 0; c0 < B; c0 += PLS_MAX_SEQUENCES) {  // chunks of at most PLS_MAX_SEQUENCES hypotheses
         const int num = B - c0 < PLS_MAX_SEQUENCES ? B - c0 : PLS_MAX_SEQUENCES;
-        int grid[5];
+        int grid[KD_BATCH_GRID];
         FrameResult* frs = nullptr;
         uint32_t* words = nullptr;
         kdmap_hypotheses_begin(ctx, n, num, st, grid, &frs, &words);
@@ -1133,7 +1133,7 @@ int pls_process_frames(pls_context* const* ctxs, int num, const void* const* dat
         trace.inputs_done(st, (int)active.size(), m);
         if (m > 0) {
             cur = icp_seq[0];
-            int grid[5];
+            int grid[KD_BATCH_GRID];
             const bool kd = lead->cfg.local_map_type == PLS_MAP_KDTREE;
             if (kd) kdmap_batch_begin(lead, icp.data(), bounds.data(), m, st, grid);
             else projmap_batch_begin(lead, icp.data(), bounds.data(), m, st, grid);
