@@ -256,14 +256,16 @@ PLS_API int pls_odometry_init(pls_context* ctx);
  * *out_iters = iterations executed (= len(losses)). */
 PLS_API int pls_register_frame(pls_context* ctx, const float* points, int64_t n, const float* T0,
                        float* out_T, float* out_params, float* out_losses, int* out_iters);
-/* B hypotheses of one scan on the kd map, in one call (no reference counterpart: relocalisation registers a scan from
- * many initial guesses).  points [n,3] as pls_register_frame; T0s [B,16].  out_T [B,16], out_params [B,6], out_losses
- * [B,max_num_alignments], out_iters [B]: hypothesis b's are the bits pls_register_frame gives with T0s[b] on the same map.
+/* B hypotheses of one scan on the local map (kd-tree or projective), in one call (no reference counterpart:
+ * relocalisation registers a scan from many initial guesses).  points [n,3] as pls_register_frame; T0s [B,16].
+ * out_T [B,16], out_params [B,6], out_losses [B,max_num_alignments], out_iters [B]: hypothesis b's are the bits
+ * pls_register_frame gives with T0s[b] on the same map.
  * out_status [B] (nullable): PLS_OK, PLS_W_TINY_RESIDUAL or PLS_E_SINGULAR per hypothesis; without it the call returns
  * PLS_E_SINGULAR if a hypothesis was singular (every output still written).  The map is not updated; afterwards the
  * last hypothesis is the context's last search (pls_kdmap_last_correspondences, pls_last_icp_sums).  Every kernel of an
- * ICP iteration is one launch for up to PLS_MAX_SEQUENCES hypotheses, larger B runs in chunks of that many.  Needs a
- * kd-tree map, gn_max_iters == 1, no communicator, B > 0 and n > 0. */
+ * ICP iteration is one launch for up to PLS_MAX_SEQUENCES hypotheses, larger B runs in chunks of that many (on a
+ * projective map off the TMA path each hypothesis's correspondence kernel is its own launch).  Needs a map that has had
+ * an update, gn_max_iters == 1, no communicator, B > 0 and n > 0. */
 PLS_API int pls_register_hypotheses(pls_context* ctx, const float* points, int64_t n, const float* T0s, int B,
                                     float* out_T, float* out_params, float* out_losses, int* out_iters, int* out_status);
 /* ICPFrameToModel.do_process_next_frame (icp_odometry.py:157-246): `data` is [n,3] points

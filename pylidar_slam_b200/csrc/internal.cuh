@@ -462,6 +462,12 @@ void projmap_batch_begin(pls_context* lead, pls_context* const* ctxs, const int6
 void projmap_batch_iterations(pls_context* lead, pls_context* const* ctxs, const int64_t* query_bounds, int num, cudaStream_t st,
                               const int* grid, int first, int last);
 void projmap_batch_done(pls_context* lead, int num, cudaStream_t st, int* out);
+// pls_register_hypotheses on a projective map: `num` <= PLS_MAX_SEQUENCES hypotheses of the scan in ctx->query_ptr on
+// ctx's model, driven by projmap_hypotheses_iterations and projmap_batch_done with lead = ctx.  begin returns their
+// FrameResults and 16 words each (for hypotheses_begin_kernel); adopt makes hypothesis h ctx's last ICP result.
+void projmap_hypotheses_begin(pls_context* ctx, int num, cudaStream_t st, FrameResult** frs, uint32_t** words);
+void projmap_hypotheses_iterations(pls_context* ctx, int64_t query_bound, int num, cudaStream_t st, int first, int last);
+void projmap_hypothesis_adopt(pls_context* ctx, int h, cudaStream_t st);
 // odometry.cu: would an ICP iteration over `work` items be split across the ranks (the rule of enqueue_icp_iterations)?
 bool icp_shards(pls_context* ctx, int64_t work);
 // comm.cu

@@ -889,9 +889,10 @@ int pls_register_hypotheses(pls_context* ctx, const float* points, int64_t n, co
     PLS_REQUIRE(points && n > 0, "pls_register_hypotheses: points must be [n,3] with n > 0");
     PLS_REQUIRE(T0s && B > 0, "pls_register_hypotheses: T0s must be [B,16] with B > 0");
     PLS_REQUIRE(ctx->cfg.gn_max_iters == 1, "fused ICP path supports gauss_newton_config.max_iters == 1");
-    PLS_REQUIRE(ctx->cfg.local_map_type == PLS_MAP_KDTREE, "pls_register_hypotheses: needs a kd-tree local map");
+    const bool kd = ctx->cfg.local_map_type == PLS_MAP_KDTREE;
     PLS_REQUIRE(!ctx->comm, "pls_register_hypotheses: a context with a multi-GPU communicator is not supported");
-    PLS_REQUIRE(ctx->kd.valid, "kd map: search before any update");
+    if (kd) PLS_REQUIRE(ctx->kd.valid, "kd map: search before any update");
+    else PLS_REQUIRE(ctx->pm.valid, "projective map: search before any update");
     cudaStream_t st = ctx->stream;
     map_stream_wait(ctx);
     // the scan is packed once, as pls_register_frame packs it; every hypothesis reads it
@@ -912,13 +913,18 @@ int pls_register_hypotheses(pls_context* ctx, const float* points, int64_t n, co
         int grid[KD_BATCH_GRID];
         FrameResult* frs = nullptr;
         uint32_t* words = nullptr;
-        kdmap_hypotheses_begin(ctx, n, num, st, grid, &frs, &words);
+        if (kd) kdmap_hypotheses_begin(ctx, n, num, st, grid, &frs, &words);
+        else projmap_hypotheses_begin(ctx, num, st, &frs, &words);
         hypotheses_begin_kernel<<<num, kMaxAlign, 0, st>>>(frs, T0_dev + 16 * (size_t)c0, words);
         PLS_CHECK_LAUNCH();
         // every hypothesis has ctx's settings: icp_rounds sees num copies of ctx
         std::vector<pls_context*> same((size_t)num, ctx);
-        icp_rounds(same.data(), num, [&](int a, int b) { kdmap_batch_iterations(ctx, num, st, grid, a, b); },
-                   [&](int* done) { kdmap_batch_done(ctx, num, st, done); });
+        if (kd)
+            icp_rounds(same.data(), num, [&](int a, int b) { kdmap_batch_iterations(ctx, num, st, grid, a, b); },
+                       [&](int* done) { kdmap_batch_done(ctx, num, st, done); });
+        else
+            icp_rounds(same.data(), num, [&](int a, int b) { projmap_hypotheses_iterations(ctx, n, num, st, a, b); },
+                       [&](int* done) { projmap_batch_done(ctx, num, st, done); });
         PLS_CUDA(cudaMemcpyAsync(h.data(), frs, (size_t)num * sizeof(FrameResult), cudaMemcpyDeviceToHost, st));
         PLS_CUDA(cudaStreamSynchronize(st));
         for (int j = 0; j < num; ++j) {
@@ -934,7 +940,8 @@ int pls_register_hypotheses(pls_context* ctx, const float* points, int64_t n, co
         last = num - 1;
     }
     // the last hypothesis is this context's last search and last ICP result, as if pls_register_frame had run it last
-    kdmap_hypothesis_adopt(ctx, n, last, st);
+    if (kd) kdmap_hypothesis_adopt(ctx, n, last, st);
+    else projmap_hypothesis_adopt(ctx, last, st);
     fetch_result(ctx);
     ctx->icp_result = true;
     auto put = [&](void* dst, const void* src, size_t bytes) {  // host or device outputs, as pls_register_frame

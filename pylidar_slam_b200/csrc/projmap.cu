@@ -563,6 +563,101 @@ proj_icp_tma_kernel(const float* __restrict__ model_v, const float4* __restrict_
                       policy_resident, policy_stream, partials, blockIdx.x, gridDim.x);
 }
 
+// ---- many pose hypotheses of one scan (pls_register_hypotheses) -----------------------------------------------------
+// Hypothesis h of a chunk owns FrameResult frs[h], the h-th hw-pixel slice of the query z-buffers `zbufs` and of the
+// target maps `tgts`, and the h-th `part_rows`-double range of the partial rows; the scan's queries and the model are
+// shared.  Every hypothesis's arithmetic is its single call's (projmap_icp_iteration), so it gets that call's bits.
+
+// project_to_pixel with the range rounded as query_zbuf_kernel's compiled code rounds it, sqrt(fma(z, z, fma(y, y, x x))):
+// a range one ulp off can change a z-buffer winner.  The compiler is free to contract x x + y y + z z either way, and does
+// so differently in different kernels, so the roundings here and in query_zbuf_hyp_kernel's transform are spelled out
+// from the SASS of query_zbuf_kernel as this compiler builds it.  CONDITION: they must stay equal to that kernel's.  If a
+// compiler contracts query_zbuf_kernel differently, these lines must follow it; nothing but the GPU bit-identity tests
+// of pls_register_hypotheses (tests/test_proj_hypotheses_gpu.py) would notice.
+__device__ __forceinline__ bool project_to_pixel_zbuf(float x, float y, float z, const ProjConst& pc, int& pix, float& r_out) {
+    const float kPi = 3.14159274101257324f;
+    const float r = __fsqrt_rn(__fmaf_rn(z, z, __fmaf_rn(y, y, __fmul_rn(x, x))));
+    r_out = r;
+    const bool null = (r == 0.0f);
+    const float rr = null ? 0.001f : r;
+    const float theta = -atan2f(y, x);
+    const float phi = asinf(__fdiv_rn(z, rr));
+    float c = __fmul_rn(0.5f, __fadd_rn(__fdiv_rn(theta, kPi), 1.0f));
+    float rw = __fsub_rn(1.0f, __fdiv_rn(__fadd_rn(phi, pc.abs_down), pc.fov));
+    c = __fmul_rn(c, pc.Wf);
+    rw = __fmul_rn(rw, pc.Hf);
+    const float row = null ? -1.0f : rw, col = null ? -1.0f : c;
+    const float pr = rintf(row), pcn = rintf(col);
+    const bool ok = (pr >= 0.0f) && (pr <= (float)(pc.H - 1)) && (pcn >= 0.0f) && (pcn <= (float)(pc.W - 1)) && (r > 0.0f);
+    if (!ok) return false;
+    pix = (int)pr * pc.W + (int)pcn;
+    return true;
+}
+
+// Each query is loaded once and z-buffered into the z-buffer of every live hypothesis, transformed by that hypothesis's
+// pose with query_zbuf_kernel's roundings (fma(z, T2, fma(x, T0, y T1)) + T3 per row, as its compiled code does; the
+// CONDITION above).  The 64-bit atomic-min keys make every z-buffer the one its single call builds, whatever the order.
+__global__ void __launch_bounds__(256)
+query_zbuf_hyp_kernel(const float4* __restrict__ queries, const uint32_t* __restrict__ nq_dev,
+                      const FrameResult* __restrict__ frs, int num, ProjConst pc, int64_t hw,
+                      unsigned long long* __restrict__ zbufs) {
+    __shared__ float sT[PLS_MAX_SEQUENCES][12];
+    __shared__ int live[PLS_MAX_SEQUENCES];
+    __shared__ int s_live;
+    if (threadIdx.x == 0) {
+        int c = 0;
+        for (int h = 0; h < num; ++h)
+            if (!frs[h].done) live[c++] = h;
+        s_live = c;
+    }
+    __syncthreads();
+    const int nl = s_live;
+    if (nl == 0) return;
+    for (int i = threadIdx.x; i < nl * 12; i += blockDim.x) sT[i / 12][i % 12] = frs[live[i / 12]].T[i % 12];
+    __syncthreads();
+    const int64_t nq = (int64_t)*nq_dev;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < nq; i += (int64_t)gridDim.x * blockDim.x) {
+        const float4 p0 = queries[i];
+        for (int j = 0; j < nl; ++j) {
+            const float* T = sT[j];
+            float p[3];
+#pragma unroll
+            for (int c = 0; c < 3; ++c)
+                p[c] = __fadd_rn(__fmaf_rn(p0.z, T[4 * c + 2], __fmaf_rn(p0.x, T[4 * c], __fmul_rn(p0.y, T[4 * c + 1]))),
+                                 T[4 * c + 3]);
+            int pix;
+            float r;
+            if (project_to_pixel_zbuf(p[0], p[1], p[2], pc, pix, r)) {
+                unsigned long long key = ((unsigned long long)__float_as_uint(r) << 32) | (unsigned long long)(uint32_t)i;
+                atomicMin(&zbufs[(size_t)live[j] * hw + pix], key);
+            }
+        }
+    }
+}
+
+// blockIdx.y = hypothesis: its z-buffer winners into its target map, leaving its z-buffer cleared.
+__global__ void query_resolve_hyp_kernel(unsigned long long* __restrict__ zbufs, const float4* __restrict__ queries,
+                                         const FrameResult* __restrict__ frs, int64_t hw, float4* __restrict__ tgts) {
+    const int h = blockIdx.y;
+    query_resolve_body(zbufs + (size_t)h * hw, queries, frs[h].T, &frs[h].done, 0, hw, tgts + (size_t)h * hw, blockIdx.x,
+                       gridDim.x);
+}
+
+// The TMA kernel of every live hypothesis: proj_icp_tma_body on hypothesis h's target map, FrameResult and partial rows,
+// as CTA `cta` of the single call's `blocks` (same tiles in the same order, same pixel per thread, same partial row), so
+// each hypothesis's rows are its single call's by construction.  blockIdx.x = cta * num + h: the CTAs of all hypotheses
+// that read one tile range are neighbours in the launch order, so they run in one wave and can share the model tiles
+// through L2.  A done hypothesis's CTAs return at once (the body's own test), before any copy.
+__global__ void __launch_bounds__(PT_TILE)
+proj_icp_tma_hyp_kernel(const float* __restrict__ model_v, const float4* __restrict__ model_n, int K, int kcap,
+                        const float4* __restrict__ tgts, int64_t hw, const FrameResult* __restrict__ frs, int num,
+                        int blocks, int64_t tiles, int scheme, float sigma, int stages, int ktma, int64_t resident_end,
+                        double* __restrict__ partials, int64_t part_rows) {
+    const int cta = (int)blockIdx.x / num, h = (int)blockIdx.x % num;
+    proj_icp_tma_body(model_v, model_n, K, kcap, tgts + (size_t)h * hw, frs + h, 0, tiles, scheme, sigma, stages, ktma,
+                      resident_end, L2_EVICT_LAST, L2_EVICT_FIRST, partials + (size_t)h * part_rows, cta, blocks);
+}
+
 // ---- several sequences per launch (pls_process_frames) --------------------------------------------------------------
 // What the kernels of one ICP iteration need of one sequence: the arguments its single path passes (one rank: every
 // tile and every pixel), and its share of each launch.  Built on the host by projmap_batch_begin and uploaded once per
@@ -1099,6 +1194,132 @@ void projmap_batch_done(pls_context* lead, int num, cudaStream_t st, int* out) {
     PLS_CHECK_LAUNCH();
     PLS_CUDA(cudaMemcpyAsync(out, dev, (size_t)num * sizeof(int), cudaMemcpyDeviceToHost, st));
     PLS_CUDA(cudaStreamSynchronize(st));
+}
+
+namespace {
+
+// Where the state of `num` hypotheses lives in ctx->hyp_buf: their FrameResults, 16 begin words each (the counter words
+// frame_begin_body clears), then per hypothesis a query z-buffer, a target map (TMA path) and the single call's partial
+// rows.
+struct HypLayout {
+    ProjPlan plan;
+    int64_t hw;
+    size_t fr_off, words_off, zbuf_off, tgt_off, part_off, total;
+};
+
+HypLayout hyp_layout(const pls_context* ctx, int num) {
+    auto up = [](size_t b) { return (b + 255) & ~(size_t)255; };
+    HypLayout L;
+    L.plan = plan_proj_iteration(ctx, 0, 1);
+    L.hw = (int64_t)ctx->cfg.height * ctx->cfg.width;
+    L.fr_off = 0;
+    L.words_off = up((size_t)num * sizeof(FrameResult));
+    L.zbuf_off = L.words_off + up((size_t)num * 16 * sizeof(uint32_t));
+    L.tgt_off = L.zbuf_off + up((size_t)num * L.hw * sizeof(unsigned long long));
+    L.part_off = L.tgt_off + (L.plan.use_tma ? up((size_t)num * L.hw * sizeof(float4)) : 0);
+    L.total = L.part_off + (size_t)num * L.plan.blocks * NACC * sizeof(double);
+    return L;
+}
+
+}  // namespace
+
+// pls_register_hypotheses on ctx's projective map: the state of `num` hypotheses of the scan in ctx->query_ptr (count in
+// ctx's FrameResult) in ctx->hyp_buf, their step descriptors (ProjSeq) and done flags in ctx->batch_buf.  Returns their
+// FrameResults and 16 words each, for hypotheses_begin_kernel.
+void projmap_hypotheses_begin(pls_context* ctx, int num, cudaStream_t st, FrameResult** frs, uint32_t** words) {
+    PLS_REQUIRE(ctx->pm.valid, "projective map: search before any update");
+    const HypLayout L = hyp_layout(ctx, num);
+    ctx->last_sharded = false;
+    ctx->hyp_buf.reserve(L.total, st);
+    char* base = ctx->hyp_buf.as<char>();
+    *frs = reinterpret_cast<FrameResult*>(base + L.fr_off);
+    *words = reinterpret_cast<uint32_t*>(base + L.words_off);
+    std::vector<ProjSeq> seqs((size_t)num);
+    for (int h = 0; h < num; ++h) {
+        ProjSeq& s = seqs[(size_t)h];
+        memset(&s, 0, sizeof(s));
+        s.model_v = ctx->pm.model_v.as<float>();
+        s.model_n = ctx->pm.model_n.as<float4>();
+        s.queries = ctx->query_ptr;
+        s.fr = *frs + h;
+        s.zbuf = reinterpret_cast<unsigned long long*>(base + L.zbuf_off) + (size_t)h * L.hw;
+        s.tgt = L.plan.use_tma ? reinterpret_cast<float4*>(base + L.tgt_off) + (size_t)h * L.hw : nullptr;
+        s.partials = reinterpret_cast<double*>(base + L.part_off) + (size_t)h * L.plan.blocks * NACC;
+        s.K = ctx->pm.K;
+        s.kcap = ctx->cfg.local_map_size;
+        s.scheme = ctx->cfg.scheme;
+        s.sigma = ctx->cfg.sigma;
+        s.threshold_delta = ctx->cfg.threshold_delta_pose;
+        s.step_blocks = L.plan.blocks;
+        s.max_iters = ctx->cfg.max_num_alignments;
+    }
+    const size_t head = (num * sizeof(ProjSeq) + PLS_MAX_SEQUENCES * sizeof(int) + 255) / 256 * 256;
+    ctx->batch_buf.reserve(head, st);
+    PLS_CUDA(cudaMemcpyAsync(ctx->batch_buf.p, seqs.data(), seqs.size() * sizeof(ProjSeq), cudaMemcpyHostToDevice, st));
+}
+
+// ICP iterations [first, last) of the hypotheses projmap_hypotheses_begin described, on st.  TMA path: one z-buffer,
+// one resolve, one proj_icp_tma_hyp_kernel and one step launch per iteration, whatever num.  Off it, each hypothesis
+// runs proj_icp_iter_kernel in its own launch, as projmap_icp_iteration does; the z-buffer and step launches are shared.
+void projmap_hypotheses_iterations(pls_context* ctx, int64_t query_bound, int num, cudaStream_t st, int first, int last) {
+    const HypLayout L = hyp_layout(ctx, num);
+    const ProjPlan& plan = L.plan;
+    char* base = ctx->hyp_buf.as<char>();
+    const FrameResult* frs = reinterpret_cast<const FrameResult*>(base + L.fr_off);
+    unsigned long long* zbufs = reinterpret_cast<unsigned long long*>(base + L.zbuf_off);
+    float4* tgts = reinterpret_cast<float4*>(base + L.tgt_off);
+    double* parts = reinterpret_cast<double*>(base + L.part_off);
+    const size_t part_rows = (size_t)plan.blocks * NACC;
+    const ProjConst pc = make_proj_const(ctx->cfg.height, ctx->cfg.width, ctx->cfg.up_fov_deg, ctx->cfg.down_fov_deg);
+    const uint32_t* nq_dev = reinterpret_cast<const uint32_t*>(&frame_result_dev(ctx)->counts[1]);
+    const int K = ctx->pm.K, kcap = ctx->cfg.local_map_size;
+    int resident_mb = 16;
+    resident_mb_env(&resident_mb);
+    const int64_t resident_end = resident_end_tile(ctx, 0, (int64_t)resident_mb << 20);
+    static bool attr_set = false;
+    if (!attr_set) {
+        PLS_CUDA(cudaFuncSetAttribute(proj_icp_tma_hyp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+        attr_set = true;
+    }
+    for (int it = first; it < last; ++it) {
+        // the single call clears its z-buffer before every iteration off the TMA path, before the first on it (the
+        // resolve kernel leaves it clear)
+        if (!plan.use_tma || it == 0)
+            PLS_CUDA(cudaMemsetAsync(zbufs, 0xff, (size_t)num * L.hw * sizeof(unsigned long long), st));
+        query_zbuf_hyp_kernel<<<grid_for(query_bound, 256), 256, 0, st>>>(ctx->query_ptr, nq_dev, frs, num, pc, L.hw, zbufs);
+        PLS_CHECK_LAUNCH();
+        if (plan.use_tma) {
+            query_resolve_hyp_kernel<<<dim3(grid_for(L.hw, 256), num), 256, 0, st>>>(zbufs, ctx->query_ptr, frs, L.hw, tgts);
+            PLS_CHECK_LAUNCH();
+            const int64_t tiles = L.hw / PT_TILE;
+            proj_icp_tma_hyp_kernel<<<(unsigned)(plan.blocks * num), PT_TILE, plan.smem, st>>>(
+                ctx->pm.model_v.as<float>(), ctx->pm.model_n.as<float4>(), K, kcap, tgts, L.hw, frs, num, plan.blocks,
+                tiles, ctx->cfg.scheme, ctx->cfg.sigma, plan.stages, plan.ktma, resident_end, parts, (int64_t)part_rows);
+            PLS_CHECK_LAUNCH();
+        } else {
+            for (int h = 0; h < num; ++h) {
+                proj_icp_iter_kernel<<<plan.blocks, PJ_THREADS, 0, st>>>(ctx->pm.model_v.as<float>(), ctx->pm.model_n.as<float4>(), K,
+                                                                         kcap, zbufs + (size_t)h * L.hw, ctx->query_ptr, frs + h,
+                                                                         0, L.hw, ctx->cfg.scheme, ctx->cfg.sigma,
+                                                                         parts + (size_t)h * part_rows);
+                PLS_CHECK_LAUNCH();
+            }
+        }
+        icp_step_batch_kernel<<<dim3(1, num), 256, 0, st>>>(ctx->batch_buf.as<ProjSeq>(), it);
+        PLS_CHECK_LAUNCH();
+    }
+}
+
+// Hypothesis h's FrameResult (all but the counts) into ctx's own, and ctx's query z-buffer as the single call leaves it:
+// pls_last_icp_sums and a following frame then see ctx as if pls_register_frame had run that hypothesis last.
+void projmap_hypothesis_adopt(pls_context* ctx, int h, cudaStream_t st) {
+    const HypLayout L = hyp_layout(ctx, h + 1);
+    const FrameResult* fr = reinterpret_cast<const FrameResult*>(ctx->hyp_buf.as<char>() + L.fr_off) + h;
+    PLS_CUDA(cudaMemcpyAsync(frame_result_dev(ctx), fr, offsetof(FrameResult, counts), cudaMemcpyDeviceToDevice, st));
+    PLS_CUDA(cudaMemsetAsync(scalar_u32(ctx, SC_KD_COUNTERS), 0, 16 * sizeof(uint32_t), st));  // frame_begin clears them
+    ctx->tmp[3].reserve((size_t)L.hw * sizeof(unsigned long long), st);
+    if (L.plan.use_tma) PLS_CUDA(cudaMemsetAsync(ctx->tmp[3].p, 0xff, (size_t)L.hw * sizeof(unsigned long long), st));
+    ctx->pm.zbuf_clean = L.plan.use_tma;
 }
 
 }  // namespace pls

@@ -806,10 +806,12 @@ class ICPFrameToModel(OdometryAlgorithm):
         """register_new_frame for B initial estimates [B,4,4] of one scan [n,3], in one call (pls_register_hypotheses;
         no reference counterpart): relocalisation in a prior map registers a scan from many guesses -- a yaw sweep, a
         grid of positions, place-recognition candidates -- and keeps the best converged result.  Registers against the
-        map this odometry's context holds (a KdTreeLocalMap built with ctx=self.ctx, e.g. after set_map_pointcloud)
-        and leaves it unchanged.  Returns (params [B,6], T [B,4,4], losses: B lists, iterations [B]); hypothesis b's are
-        what register_new_frame(target_points, initial_estimates[b]) returns, bit for bit.  A singular hypothesis does
-        not stop the others: it is logged, and last_hypotheses_status[b] holds each one's status (PLS_OK,
+        map this odometry's context holds and leaves it unchanged: a KdTreeLocalMap built with ctx=self.ctx (e.g.
+        after set_map_pointcloud), or the odometry's own projective local map, where a sweep of yaw and offset guesses
+        recovers a scan that projective association, converging only from a close pose, lost after a fast turn.
+        Returns (params [B,6], T [B,4,4], losses: B lists, iterations [B]); hypothesis b's are what
+        register_new_frame(target_points, initial_estimates[b]) returns, bit for bit.  A singular hypothesis does not
+        stop the others: it is logged, and last_hypotheses_status[b] holds each one's status (PLS_OK,
         PLS_W_TINY_RESIDUAL or PLS_E_SINGULAR)."""
         _check_given_normals(self.ctx)
         check_tensor(target_points, [-1, 3])
