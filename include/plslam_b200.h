@@ -268,6 +268,20 @@ PLS_API int pls_register_frame(pls_context* ctx, const float* points, int64_t n,
  * an update, gn_max_iters == 1, no communicator, B > 0 and n > 0. */
 PLS_API int pls_register_hypotheses(pls_context* ctx, const float* points, int64_t n, const float* T0s, int B,
                                     float* out_T, float* out_params, float* out_losses, int* out_iters, int* out_status);
+/* S scans registered from B initial estimates against the kd map ctx holds, in one call (no reference counterpart: a
+ * localisation server registers many vehicles' scans on one map, offline map matching a recorded drive's scans).
+ * scans[s]: [n[s],3] float32, host or device, n[s] > 0.  scan_of [B]: the scan registration b uses (NULL: b -> b,
+ * which needs B == S).  T0s [B,16].  Outputs as pls_register_hypotheses: out_T [B,16], out_params [B,6],
+ * out_losses [B,max_num_alignments], out_iters [B], out_status [B] (nullable, same rule for raising).
+ * Registration b gives the bits pls_register_frame(scans[scan_of[b]], T0s[b]) gives on the same context.  The map is
+ * not updated, its index not rebuilt; afterwards the last registration is the context's last search
+ * (pls_kdmap_last_correspondences, pls_last_icp_sums), as if pls_register_frame had run it last.  One launch packs
+ * every scan; every kernel of an ICP iteration is one launch for up to PLS_MAX_SEQUENCES registrations, larger B runs
+ * in chunks of that many.  PLS_E_INVALID before any work, the context unchanged: a projective map, gn_max_iters != 1,
+ * a communicator, a map that has had no update, S or B <= 0, an n[s] <= 0 or a scan_of entry outside [0, S). */
+PLS_API int pls_register_scans(pls_context* ctx, const float* const* scans, const int64_t* n, int S,
+                               const int* scan_of, const float* T0s, int B, float* out_T, float* out_params,
+                               float* out_losses, int* out_iters, int* out_status);
 /* ICPFrameToModel.do_process_next_frame (icp_odometry.py:157-246): `data` is [n,3] points
  * (PLS_INPUT_NDARRAY / PLS_INPUT_TENSOR: float; the _F64 variants: double) or a float [3,H,W] vertex map
  * (PLS_INPUT_VERTEX_MAP, n ignored).  init_pose [16] or NULL (identity).  On frame 0 the map is initialised and

@@ -408,12 +408,29 @@ void kdmap_batch_begin(pls_context* lead, pls_context* const* ctxs, const int64_
                        int* grid);
 void kdmap_batch_iterations(pls_context* lead, int num, cudaStream_t st, const int* grid, int first, int last);
 void kdmap_batch_done(pls_context* lead, int num, cudaStream_t st, int* out);
-// pls_register_hypotheses: `num` <= PLS_MAX_SEQUENCES hypotheses of the scan in ctx->query_ptr on ctx's map, driven by
-// kdmap_batch_iterations / kdmap_batch_done with lead = ctx.  begin returns their FrameResults and 16 counter and
-// work-list words each (for the caller to initialise, as frame_begin does); adopt makes hypothesis h ctx's last search.
-void kdmap_hypotheses_begin(pls_context* ctx, int64_t query_bound, int num, cudaStream_t st, int* grid, FrameResult** frs,
+// The scan one registration of pls_register_hypotheses / pls_register_scans reads: its packed float4 queries, their
+// count on the device (u32) and the query bound of its single pls_register_frame call (the scan's row count).
+struct KdScan {
+    const float4* queries;
+    const uint32_t* nq_dev;
+    int64_t bound;
+};
+// pls_register_hypotheses / pls_register_scans: `num` <= PLS_MAX_SEQUENCES registrations on ctx's map, registration h of
+// scans[h], driven by kdmap_batch_iterations / kdmap_batch_done with lead = ctx.  begin returns their FrameResults and
+// 16 counter and work-list words each (for the caller to initialise, as frame_begin does); adopt makes registration h,
+// of scan `scan`, ctx's last search: its matches, search states, FrameResult, query count and queries.
+void kdmap_hypotheses_begin(pls_context* ctx, const KdScan* scans, int num, cudaStream_t st, int* grid, FrameResult** frs,
                             uint32_t** words);
-void kdmap_hypothesis_adopt(pls_context* ctx, int64_t query_bound, int h, cudaStream_t st);
+void kdmap_hypothesis_adopt(pls_context* ctx, const KdScan& scan, int h, cudaStream_t st);
+// pls_register_scans: one scan to pack, its device rows [n,3] (n > 0) and where its valid rows and their count go.
+struct KdScanRows {
+    const float* rows;
+    int64_t n;
+    float4* out;
+    uint32_t* count;
+};
+// One launch packs every scan, each as pack_valid_rows packs it alone.
+void pack_valid_scans(pls_context* ctx, const std::vector<KdScanRows>& scans);
 // ICP iteration `it` of the frame over ctx->query_ptr; returns the number of partial rows written
 // it == 0: no previous matches; fuse_threshold >= 0: finish the iteration (sum + solve + pose update) in the last
 // block of the reduction kernel (*solved tells).  bound_dev (nullable, unsharded frames only): a device-side count that

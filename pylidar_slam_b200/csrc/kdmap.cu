@@ -104,6 +104,57 @@ __global__ void kd_pack_rows_kernel(const T* __restrict__ pts, int64_t n, const 
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
         if (flags[i]) out[pos[i]] = make_float4((float)pts[3 * i], (float)pts[3 * i + 1], (float)pts[3 * i + 2], 0.f);
 }
+// pls_register_scans: block s packs scans[s] into its own slice of the query buffer, with the rows and the count
+// pack_valid_rows gives for that scan alone: the rows without a NaN coordinate (kd_valid_rows_kernel's test), in input
+// order (the positions of the exclusive scan).  The block walks its scan in tiles of KD_PACK_ROWS rows per thread.
+constexpr int KD_PACK_THREADS = 1024, KD_PACK_ROWS = 4;
+__global__ void __launch_bounds__(KD_PACK_THREADS) kd_pack_scans_kernel(const KdScanRows* __restrict__ scans) {
+    __shared__ uint32_t s_warp[KD_PACK_ROWS][32];  // per sub-tile: valid rows of the warps before, then of the sub-tile
+    __shared__ uint32_t s_sub[KD_PACK_ROWS];
+    const KdScanRows sc = scans[blockIdx.x];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const uint32_t below = (1u << lane) - 1u;
+    uint32_t base = 0;
+    for (int64_t t0 = 0; t0 < sc.n; t0 += (int64_t)KD_PACK_THREADS * KD_PACK_ROWS) {
+        float4 v[KD_PACK_ROWS];
+        bool ok[KD_PACK_ROWS];
+        uint32_t rank[KD_PACK_ROWS];
+#pragma unroll
+        for (int j = 0; j < KD_PACK_ROWS; ++j) {
+            const int64_t i = t0 + (int64_t)j * KD_PACK_THREADS + threadIdx.x;
+            ok[j] = false;
+            if (i < sc.n) {
+                const float x = sc.rows[3 * i], y = sc.rows[3 * i + 1], z = sc.rows[3 * i + 2];
+                ok[j] = x == x && y == y && z == z;
+                v[j] = make_float4(x, y, z, 0.f);
+            }
+            const unsigned b = __ballot_sync(0xffffffffu, ok[j]);
+            rank[j] = __popc(b & below);
+            if (lane == 0) s_warp[j][warp] = __popc(b);
+        }
+        __syncthreads();
+        if (warp < KD_PACK_ROWS) {  // warp j: exclusive prefix over the 32 warps of sub-tile j
+            const uint32_t c = s_warp[warp][lane];
+            uint32_t inc = c;
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) {
+                const uint32_t u = __shfl_up_sync(0xffffffffu, inc, o);
+                if (lane >= o) inc += u;
+            }
+            s_warp[warp][lane] = inc - c;
+            if (lane == 31) s_sub[warp] = inc;
+        }
+        __syncthreads();
+#pragma unroll
+        for (int j = 0; j < KD_PACK_ROWS; ++j) {
+            if (ok[j]) sc.out[base + s_warp[j][warp] + rank[j]] = v[j];
+            base += s_sub[j];
+        }
+        __syncthreads();  // s_warp and s_sub are rewritten by the next tile
+    }
+    if (threadIdx.x == 0) *sc.count = base;
+}
+
 // pls_kdmap_set_points: counts the rows with a NaN or an infinite coordinate once rounded to float32.
 template <typename T>
 __global__ void kd_nonfinite_rows_kernel(const T* __restrict__ pts, int64_t n, uint32_t* __restrict__ count) {
@@ -1094,6 +1145,15 @@ void pack_valid_rows_f64(pls_context* ctx, const double* pts_dev, int64_t n, flo
     pack_valid_rows_impl<double>(ctx, pts_dev, n, out, count_dev);
 }
 
+void pack_valid_scans(pls_context* ctx, const std::vector<KdScanRows>& scans) {
+    cudaStream_t st = ctx->stream;
+    const size_t bytes = scans.size() * sizeof(KdScanRows);
+    ctx->stage_in[2].reserve(bytes, st);
+    PLS_CUDA(cudaMemcpyAsync(ctx->stage_in[2].p, scans.data(), bytes, cudaMemcpyHostToDevice, st));
+    kd_pack_scans_kernel<<<(unsigned)scans.size(), KD_PACK_THREADS, 0, st>>>(ctx->stage_in[2].as<KdScanRows>());
+    PLS_CHECK_LAUNCH();
+}
+
 void pack_valid_pixels(pls_context* ctx, const float* vmap_dev, int64_t hw, float min_norm, float4* out,
                        uint32_t* count_dev) {
     cudaStream_t st = ctx->stream;
@@ -1330,13 +1390,14 @@ int kdmap_icp_iteration(pls_context* ctx, int64_t query_bound, const uint32_t* b
     return blocks;
 }
 
-// The descriptor of one sequence's (or one hypothesis's) ICP on ctx's map, with its per-query and per-block state at the
-// given addresses; fr is its FrameResult, nq_dev its query count.
-static KdSeq make_seq(pls_context* ctx, const KdPlan& plan, FrameResult* fr, const uint32_t* nq_dev, int* match,
-                      float4* nn_state, int* worklist, uint32_t* words, double* partials, int share_nn, int share_kn) {
+// The descriptor of one sequence's (or one registration's) ICP on ctx's map, with its per-query and per-block state at
+// the given addresses; fr is its FrameResult, queries and nq_dev its queries and their count.
+static KdSeq make_seq(pls_context* ctx, const KdPlan& plan, const float4* queries, FrameResult* fr, const uint32_t* nq_dev,
+                      int* match, float4* nn_state, int* worklist, uint32_t* words, double* partials, int share_nn,
+                      int share_kn) {
     KdSeq s;
     s.ix = make_index(ctx);
-    s.queries = ctx->query_ptr;
+    s.queries = queries;
     s.nq_dev = nq_dev;
     s.fr = fr;
     s.match = match;
@@ -1398,7 +1459,7 @@ void kdmap_batch_begin(pls_context* lead, pls_context* const* ctxs, const int64_
         ctx->last_sharded = false;
         record_search(ctx->kd, true, false, true, 0);
         FrameResult* fr = frame_result_dev(ctx);
-        seqs.push_back(make_seq(ctx, plan, fr, reinterpret_cast<const uint32_t*>(&fr->counts[1]), ctx->nn_prev.as<int>(),
+        seqs.push_back(make_seq(ctx, plan, ctx->query_ptr, fr, reinterpret_cast<const uint32_t*>(&fr->counts[1]), ctx->nn_prev.as<int>(),
                                 ctx->kd_nn_state.as<float4>(), ctx->kd_worklist.as<int>(), scalar_u32(ctx, SC_KD_COUNTERS),
                                 ctx->partials.as<double>(), share_nn, share_kn));
     }
@@ -1437,50 +1498,63 @@ void kdmap_batch_iterations(pls_context* lead, int num, cudaStream_t st, const i
     }
 }
 
-// pls_register_hypotheses: the ICP state of `num` hypotheses of one scan (ctx->query_ptr, count in ctx's FrameResult) on
-// ctx's map, each a slice of ctx->hyp_buf laid out as pls_register_frame's own buffers; their descriptors into
-// ctx->batch_buf.  Returns the hypotheses' FrameResults (contiguous) and their 16 counter and work-list words each, for
-// the caller to initialise before the first iteration; grid as kdmap_batch_begin.
-void kdmap_hypotheses_begin(pls_context* ctx, int64_t query_bound, int num, cudaStream_t st, int* grid, FrameResult** frs,
+// pls_register_hypotheses / pls_register_scans: the ICP state of `num` registrations on ctx's map, registration h of
+// scans[h], each a slice of ctx->hyp_buf laid out as pls_register_frame's own buffers for that scan's query bound; their
+// descriptors into ctx->batch_buf.  Returns the registrations' FrameResults (contiguous) and their 16 counter and
+// work-list words each, for the caller to initialise before the first iteration; grid as kdmap_batch_begin.
+void kdmap_hypotheses_begin(pls_context* ctx, const KdScan* scans, int num, cudaStream_t st, int* grid, FrameResult** frs,
                             uint32_t** words) {
     PLS_REQUIRE(ctx->kd.valid, "kd map: search before any update");
     static const int resident_nn = resident_blocks((const void*)kd_nn_warp_batch_kernel);
     static const int resident_kn = resident_blocks((const void*)kd_normals_warp_batch_kernel);
-    const KdPlan plan = plan_kd_iteration(ctx, query_bound, 1);  // ctx's own buffers: the last hypothesis is copied there
     ctx->last_sharded = false;
     record_search(ctx->kd, true, false, true, 0);
     auto up = [](size_t b) { return (b + 255) & ~(size_t)255; };
     const size_t fr_bytes = up((size_t)num * sizeof(FrameResult)), word_bytes = up((size_t)num * 16 * sizeof(uint32_t));
-    const size_t match_b = up((size_t)query_bound * sizeof(int)), state_b = up(plan.slots * sizeof(float4)),
-                 list_b = up(2 * plan.slots * sizeof(int)), part_b = up((size_t)plan.blocks * NACC * sizeof(double));
-    const size_t per = match_b + state_b + list_b + part_b;
-    ctx->hyp_buf.reserve(fr_bytes + word_bytes + (size_t)num * per, st);
+    // each plan also reserves ctx's own buffers for its bound: the last registration is copied there
+    std::vector<KdPlan> plans;
+    std::vector<size_t> offs;
+    size_t total = fr_bytes + word_bytes;
+    for (int h = 0; h < num; ++h) {
+        plans.push_back(plan_kd_iteration(ctx, scans[h].bound, 1));
+        const KdPlan& p = plans.back();
+        offs.push_back(total);
+        total += up((size_t)scans[h].bound * sizeof(int)) + up(p.slots * sizeof(float4)) + up(2 * p.slots * sizeof(int)) +
+                 up((size_t)p.blocks * NACC * sizeof(double));
+    }
+    ctx->hyp_buf.reserve(total, st);
     char* base = ctx->hyp_buf.as<char>();
     *frs = reinterpret_cast<FrameResult*>(base);
     *words = reinterpret_cast<uint32_t*>(base + fr_bytes);
-    const FrameResult* fr_ctx = frame_result_dev(ctx);
-    const uint32_t* nq_dev = reinterpret_cast<const uint32_t*>(&fr_ctx->counts[1]);  // one packed scan for all
     const int share_nn = (resident_nn + num - 1) / num, share_kn = (resident_kn + num - 1) / num;
     std::vector<KdSeq> seqs;
     for (int h = 0; h < num; ++h) {
-        char* p = base + fr_bytes + word_bytes + (size_t)h * per;
-        seqs.push_back(make_seq(ctx, plan, *frs + h, nq_dev, reinterpret_cast<int*>(p), reinterpret_cast<float4*>(p + match_b),
-                                reinterpret_cast<int*>(p + match_b + state_b), *words + 16 * h,
-                                reinterpret_cast<double*>(p + match_b + state_b + list_b), share_nn, share_kn));
+        const KdPlan& p = plans[(size_t)h];
+        char* match = base + offs[(size_t)h];
+        char* state = match + up((size_t)scans[h].bound * sizeof(int));
+        char* list = state + up(p.slots * sizeof(float4));
+        char* part = list + up(2 * p.slots * sizeof(int));
+        seqs.push_back(make_seq(ctx, p, scans[h].queries, *frs + h, scans[h].nq_dev, reinterpret_cast<int*>(match),
+                                reinterpret_cast<float4*>(state), reinterpret_cast<int*>(list), *words + 16 * h,
+                                reinterpret_cast<double*>(part), share_nn, share_kn));
     }
     upload_seqs(ctx, seqs, st, grid);
 }
 
-// Hypothesis h's matches, search states and FrameResult (all but the counts) into ctx's own: pls_kdmap_last_correspondences
-// and pls_last_icp_sums then read that hypothesis as the last search.
-void kdmap_hypothesis_adopt(pls_context* ctx, int64_t query_bound, int h, cudaStream_t st) {
+// Registration h's matches, search states and FrameResult (all but the counts) into ctx's own, and its scan's query
+// count and queries: pls_kdmap_last_correspondences and pls_last_icp_sums then read that registration as the last search.
+void kdmap_hypothesis_adopt(pls_context* ctx, const KdScan& scan, int h, cudaStream_t st) {
     KdSeq s;
     PLS_CUDA(cudaMemcpyAsync(&s, ctx->batch_buf.as<KdSeq>() + h, sizeof(KdSeq), cudaMemcpyDeviceToHost, st));
     PLS_CUDA(cudaStreamSynchronize(st));
-    PLS_CUDA(cudaMemcpyAsync(ctx->nn_prev.p, s.match, (size_t)query_bound * sizeof(int), cudaMemcpyDeviceToDevice, st));
-    PLS_CUDA(cudaMemcpyAsync(ctx->kd_nn_state.p, s.nn_state, (size_t)query_bound * sizeof(float4), cudaMemcpyDeviceToDevice,
+    PLS_CUDA(cudaMemcpyAsync(ctx->nn_prev.p, s.match, (size_t)scan.bound * sizeof(int), cudaMemcpyDeviceToDevice, st));
+    PLS_CUDA(cudaMemcpyAsync(ctx->kd_nn_state.p, s.nn_state, (size_t)scan.bound * sizeof(float4), cudaMemcpyDeviceToDevice,
                              st));
-    PLS_CUDA(cudaMemcpyAsync(frame_result_dev(ctx), s.fr, offsetof(FrameResult, counts), cudaMemcpyDeviceToDevice, st));
+    FrameResult* fr = frame_result_dev(ctx);
+    PLS_CUDA(cudaMemcpyAsync(fr, s.fr, offsetof(FrameResult, counts), cudaMemcpyDeviceToDevice, st));
+    uint32_t* nq = reinterpret_cast<uint32_t*>(&fr->counts[1]);
+    if (scan.nq_dev != nq) PLS_CUDA(cudaMemcpyAsync(nq, scan.nq_dev, sizeof(uint32_t), cudaMemcpyDeviceToDevice, st));
+    ctx->query_ptr = scan.queries;
 }
 
 // The done flag of every sequence of the batch: one gather launch, one copy, one synchronisation.

@@ -811,6 +811,67 @@ void odometry_reset(pls_context* ctx) {
     for (int i = 0; i < 16; ++i) ctx->delta_since_update[i] = (i % 5 == 0) ? 1.f : 0.f;
 }
 
+// The B registrations of pls_register_hypotheses / pls_register_scans from T0_dev [B,16] on ctx's map, whose queries are
+// packed, in chunks of PLS_MAX_SEQUENCES.  kd map: registration b reads scans[b].  Projective map: every registration
+// reads the scan in ctx->query_ptr, bound n.  Outputs and status as pls_register_hypotheses; afterwards the last
+// registration is ctx's last search and last ICP result, as if pls_register_frame had run it last.
+static void register_batch(pls_context* ctx, const KdScan* scans, int64_t n, const float* T0_dev, int B, float* out_T,
+                           float* out_params, float* out_losses, int* out_iters, int* out_status) {
+    const bool kd = ctx->cfg.local_map_type == PLS_MAP_KDTREE;
+    cudaStream_t st = ctx->stream;
+    const int M = ctx->cfg.max_num_alignments;
+    std::vector<FrameResult> h((size_t)PLS_MAX_SEQUENCES);
+    std::vector<float> T((size_t)B * 16), params((size_t)B * 6), losses((size_t)B * M);
+    std::vector<int> iters((size_t)B), status((size_t)B);
+    int first_error = PLS_OK, last = 0;
+    for (int c0 = 0; c0 < B; c0 += PLS_MAX_SEQUENCES) {  // chunks of at most PLS_MAX_SEQUENCES registrations
+        const int num = B - c0 < PLS_MAX_SEQUENCES ? B - c0 : PLS_MAX_SEQUENCES;
+        int grid[KD_BATCH_GRID];
+        FrameResult* frs = nullptr;
+        uint32_t* words = nullptr;
+        if (kd) kdmap_hypotheses_begin(ctx, scans + c0, num, st, grid, &frs, &words);
+        else projmap_hypotheses_begin(ctx, num, st, &frs, &words);
+        hypotheses_begin_kernel<<<num, kMaxAlign, 0, st>>>(frs, T0_dev + 16 * (size_t)c0, words);
+        PLS_CHECK_LAUNCH();
+        // every registration has ctx's settings: icp_rounds sees num copies of ctx
+        std::vector<pls_context*> same((size_t)num, ctx);
+        if (kd)
+            icp_rounds(same.data(), num, [&](int a, int b) { kdmap_batch_iterations(ctx, num, st, grid, a, b); },
+                       [&](int* done) { kdmap_batch_done(ctx, num, st, done); });
+        else
+            icp_rounds(same.data(), num, [&](int a, int b) { projmap_hypotheses_iterations(ctx, n, num, st, a, b); },
+                       [&](int* done) { projmap_batch_done(ctx, num, st, done); });
+        PLS_CUDA(cudaMemcpyAsync(h.data(), frs, (size_t)num * sizeof(FrameResult), cudaMemcpyDeviceToHost, st));
+        PLS_CUDA(cudaStreamSynchronize(st));
+        for (int j = 0; j < num; ++j) {
+            const FrameResult& r = h[(size_t)j];
+            const size_t b = (size_t)(c0 + j);
+            memcpy(&T[16 * b], r.T, 16 * sizeof(float));
+            memcpy(&params[6 * b], r.params, 6 * sizeof(float));
+            memcpy(&losses[(size_t)M * b], r.losses, (size_t)M * sizeof(float));
+            iters[b] = r.iters;
+            status[b] = r.status;
+            if (first_error == PLS_OK && (r.status == PLS_E_SINGULAR || r.status == PLS_E_COMM)) first_error = r.status;
+        }
+        last = num - 1;
+    }
+    if (kd) kdmap_hypothesis_adopt(ctx, scans[B - 1], last, st);
+    else projmap_hypothesis_adopt(ctx, last, st);
+    fetch_result(ctx);
+    ctx->icp_result = true;
+    auto put = [&](void* dst, const void* src, size_t bytes) {  // host or device outputs, as pls_register_frame
+        if (!dst) return;
+        if (is_device_ptr(dst)) PLS_CUDA(cudaMemcpy(dst, src, bytes, cudaMemcpyHostToDevice));
+        else memcpy(dst, src, bytes);
+    };
+    put(out_T, T.data(), T.size() * sizeof(float));
+    put(out_params, params.data(), params.size() * sizeof(float));
+    put(out_losses, losses.data(), losses.size() * sizeof(float));
+    put(out_iters, iters.data(), iters.size() * sizeof(int));
+    put(out_status, status.data(), status.size() * sizeof(int));
+    if (!out_status) raise_status(ctx, first_error);
+}
+
 }  // namespace pls
 
 using namespace pls;
@@ -903,58 +964,61 @@ int pls_register_hypotheses(pls_context* ctx, const float* points, int64_t n, co
     ctx->queries.reserve((size_t)n * sizeof(float4), st);
     pack_valid_rows(ctx, d, n, ctx->queries.as<float4>(), count_slot(ctx, 1));
     ctx->query_ptr = ctx->queries.as<float4>();
-    const int M = ctx->cfg.max_num_alignments;
-    std::vector<FrameResult> h((size_t)PLS_MAX_SEQUENCES);
-    std::vector<float> T((size_t)B * 16), params((size_t)B * 6), losses((size_t)B * M);
-    std::vector<int> iters((size_t)B), status((size_t)B);
-    int first_error = PLS_OK, last = 0;
-    for (int c0 = 0; c0 < B; c0 += PLS_MAX_SEQUENCES) {  // chunks of at most PLS_MAX_SEQUENCES hypotheses
-        const int num = B - c0 < PLS_MAX_SEQUENCES ? B - c0 : PLS_MAX_SEQUENCES;
-        int grid[KD_BATCH_GRID];
-        FrameResult* frs = nullptr;
-        uint32_t* words = nullptr;
-        if (kd) kdmap_hypotheses_begin(ctx, n, num, st, grid, &frs, &words);
-        else projmap_hypotheses_begin(ctx, num, st, &frs, &words);
-        hypotheses_begin_kernel<<<num, kMaxAlign, 0, st>>>(frs, T0_dev + 16 * (size_t)c0, words);
-        PLS_CHECK_LAUNCH();
-        // every hypothesis has ctx's settings: icp_rounds sees num copies of ctx
-        std::vector<pls_context*> same((size_t)num, ctx);
-        if (kd)
-            icp_rounds(same.data(), num, [&](int a, int b) { kdmap_batch_iterations(ctx, num, st, grid, a, b); },
-                       [&](int* done) { kdmap_batch_done(ctx, num, st, done); });
-        else
-            icp_rounds(same.data(), num, [&](int a, int b) { projmap_hypotheses_iterations(ctx, n, num, st, a, b); },
-                       [&](int* done) { projmap_batch_done(ctx, num, st, done); });
-        PLS_CUDA(cudaMemcpyAsync(h.data(), frs, (size_t)num * sizeof(FrameResult), cudaMemcpyDeviceToHost, st));
-        PLS_CUDA(cudaStreamSynchronize(st));
-        for (int j = 0; j < num; ++j) {
-            const FrameResult& r = h[(size_t)j];
-            const size_t b = (size_t)(c0 + j);
-            memcpy(&T[16 * b], r.T, 16 * sizeof(float));
-            memcpy(&params[6 * b], r.params, 6 * sizeof(float));
-            memcpy(&losses[(size_t)M * b], r.losses, (size_t)M * sizeof(float));
-            iters[b] = r.iters;
-            status[b] = r.status;
-            if (first_error == PLS_OK && (r.status == PLS_E_SINGULAR || r.status == PLS_E_COMM)) first_error = r.status;
+    // on a kd map: pls_register_scans's registrations, S = 1, every hypothesis on the one scan
+    const std::vector<KdScan> scans(kd ? (size_t)B : 0, KdScan{ctx->query_ptr, count_slot(ctx, 1), n});
+    register_batch(ctx, scans.data(), n, T0_dev, B, out_T, out_params, out_losses, out_iters, out_status);
+    PLS_API_END(ctx)
+}
+
+int pls_register_scans(pls_context* ctx, const float* const* scans, const int64_t* n, int S, const int* scan_of,
+                       const float* T0s, int B, float* out_T, float* out_params, float* out_losses, int* out_iters,
+                       int* out_status) {
+    PLS_API_BEGIN(ctx)
+    // every argument is checked before anything is enqueued: a refused call changes nothing
+    PLS_REQUIRE(ctx->cfg.local_map_type == PLS_MAP_KDTREE, "pls_register_scans: needs a kd-tree local map");
+    PLS_REQUIRE(ctx->cfg.gn_max_iters == 1, "fused ICP path supports gauss_newton_config.max_iters == 1");
+    PLS_REQUIRE(!ctx->comm, "pls_register_scans: a context with a multi-GPU communicator is not supported");
+    PLS_REQUIRE(ctx->kd.valid, "kd map: search before any update");
+    PLS_REQUIRE(scans && n && S > 0, "pls_register_scans: scans and n must hold S > 0 scans");
+    PLS_REQUIRE(T0s && B > 0, "pls_register_scans: T0s must be [B,16] with B > 0");
+    PLS_REQUIRE(scan_of || B == S, "pls_register_scans: without scan_of, B must equal S");
+    for (int s = 0; s < S; ++s) PLS_REQUIRE(scans[s] && n[s] > 0, "pls_register_scans: every scan must be [n,3] with n > 0");
+    for (int b = 0; scan_of && b < B; ++b)
+        PLS_REQUIRE(scan_of[b] >= 0 && scan_of[b] < S, "pls_register_scans: scan_of entries must lie in [0, S)");
+    cudaStream_t st = ctx->stream;
+    map_stream_wait(ctx);
+    // host scans are staged back to back, as to_device stages one
+    size_t host_rows = 0;
+    for (int s = 0; s < S; ++s)
+        if (!is_device_ptr(scans[s])) host_rows += (size_t)n[s];
+    if (host_rows) ctx->stage_in[0].reserve(host_rows * 3 * sizeof(float), st);
+    // scan s's packed rows go to ctx->queries at the sum of the earlier scans' row counts, the S counts behind them
+    size_t rows = 0;
+    for (int s = 0; s < S; ++s) rows += (size_t)n[s];
+    ctx->queries.reserve(rows * sizeof(float4) + (size_t)S * sizeof(uint32_t), st);
+    float4* q = ctx->queries.as<float4>();
+    uint32_t* counts = reinterpret_cast<uint32_t*>(q + rows);
+    std::vector<KdScanRows> pack((size_t)S);
+    std::vector<KdScan> packed((size_t)S);
+    float* staged = ctx->stage_in[0].as<float>();
+    for (int s = 0; s < S; ++s) {
+        const float* d = scans[s];
+        if (!is_device_ptr(d)) {
+            PLS_CUDA(cudaMemcpyAsync(staged, d, (size_t)n[s] * 3 * sizeof(float), cudaMemcpyHostToDevice, st));
+            d = staged;
+            staged += (size_t)n[s] * 3;
         }
-        last = num - 1;
+        pack[(size_t)s] = KdScanRows{d, n[s], q, counts + s};
+        packed[(size_t)s] = KdScan{q, counts + s, n[s]};
+        q += n[s];
     }
-    // the last hypothesis is this context's last search and last ICP result, as if pls_register_frame had run it last
-    if (kd) kdmap_hypothesis_adopt(ctx, n, last, st);
-    else projmap_hypothesis_adopt(ctx, last, st);
-    fetch_result(ctx);
-    ctx->icp_result = true;
-    auto put = [&](void* dst, const void* src, size_t bytes) {  // host or device outputs, as pls_register_frame
-        if (!dst) return;
-        if (is_device_ptr(dst)) PLS_CUDA(cudaMemcpy(dst, src, bytes, cudaMemcpyHostToDevice));
-        else memcpy(dst, src, bytes);
-    };
-    put(out_T, T.data(), T.size() * sizeof(float));
-    put(out_params, params.data(), params.size() * sizeof(float));
-    put(out_losses, losses.data(), losses.size() * sizeof(float));
-    put(out_iters, iters.data(), iters.size() * sizeof(int));
-    put(out_status, status.data(), status.size() * sizeof(int));
-    if (!out_status) raise_status(ctx, first_error);
+    const float* T0_dev = (const float*)to_device(ctx, T0s, (size_t)B * 16 * sizeof(float), ctx->stage_in[1]);
+    FrameResult* fr = frame_result_dev(ctx);
+    PLS_CUDA(cudaMemsetAsync(fr->counts, 0, sizeof(fr->counts), st));
+    pack_valid_scans(ctx, pack);
+    std::vector<KdScan> regs((size_t)B);
+    for (int b = 0; b < B; ++b) regs[(size_t)b] = packed[(size_t)(scan_of ? scan_of[b] : b)];
+    register_batch(ctx, regs.data(), 0, T0_dev, B, out_T, out_params, out_losses, out_iters, out_status);
     PLS_API_END(ctx)
 }
 

@@ -834,6 +834,48 @@ class ICPFrameToModel(OdometryAlgorithm):
                           f"(hypotheses {singular.tolist()})")
         return params, T, [list(losses[b, :iters[b]]) for b in range(B)], iters
 
+    def register_new_frames(self, scans, initial_estimates, scan_indices=None):
+        """register_new_frame for many scans against the one map this odometry's context holds, in one call
+        (pls_register_scans; no reference counterpart): a localisation server registers many vehicles' scans on one
+        city map, offline map matching registers a recorded drive's scans on a prior map.  `scans` is a list of S
+        [n_i,3] arrays or tensors, `initial_estimates` [B,4,4], and registration b registers scans[scan_indices[b]]
+        from initial_estimates[b] (scan_indices None: scan b, which needs B == S).  The map is a kd map, e.g. one loaded
+        with KdTreeLocalMap(ctx=self.ctx).set_map_pointcloud; it is left unchanged.
+        Returns (params [B,6], T [B,4,4], losses: B lists, iterations [B]); registration b's are what
+        register_new_frame(scans[scan_indices[b]], initial_estimates[b]) returns, bit for bit.  A singular registration
+        does not stop the others: it is logged, and last_registrations_status[b] holds each one's status (PLS_OK,
+        PLS_W_TINY_RESIDUAL or PLS_E_SINGULAR)."""
+        _check_given_normals(self.ctx)
+        pts = []
+        for scan in scans:
+            check_tensor(scan, [-1, 3])
+            pts.append(_f32c(scan))
+        if isinstance(initial_estimates, torch.Tensor):
+            initial_estimates = initial_estimates.detach().cpu().numpy()
+        check_tensor(initial_estimates, [-1, 4, 4])
+        T0 = np.ascontiguousarray(initial_estimates, dtype=np.float32)
+        B, S, M = T0.shape[0], len(pts), int(self.config.max_num_alignments)
+        index = None
+        if scan_indices is not None:
+            if isinstance(scan_indices, torch.Tensor):
+                scan_indices = scan_indices.detach().cpu().numpy()
+            index = np.ascontiguousarray(scan_indices, dtype=np.int32).reshape(-1)
+            assert_debug(index.shape[0] == B, f"scan_indices must hold one scan index per initial estimate ({B})")
+        addresses = np.array([_lib.ptr(p) for p in pts], dtype=np.uint64)
+        rows = np.array([p.shape[0] for p in pts], dtype=np.int64)
+        T, params = np.zeros((B, 4, 4), np.float32), np.zeros((B, 6), np.float32)
+        losses = np.zeros((B, M), np.float32)
+        iters, status = np.zeros(B, np.int32), np.zeros(B, np.int32)
+        self.ctx.call("pls_register_scans", _lib.ptr(addresses), _lib.ptr(rows), S, _lib.ptr(index), _lib.ptr(T0), B,
+                      _lib.ptr(T), _lib.ptr(params), _lib.ptr(losses), _lib.ptr(iters), _lib.ptr(status))
+        self.last_registrations_status = status
+        singular = np.flatnonzero(status == _lib.PLS_E_SINGULAR)
+        if singular.size:
+            import logging
+            logging.error(f"Invalid Jacobian in Gauss Newton minimization, the hessian is not invertible "
+                          f"(registrations {singular.tolist()})")
+        return params, T, [list(losses[b, :iters[b]]) for b in range(B)], iters
+
 
 class ICPFrameToModelBatch:
     """Advances several independent ICPFrameToModel sequences by one frame each in ONE `pls_process_frames` call (no
