@@ -320,7 +320,7 @@ int pls_destroy(pls_context* ctx) {
     ctx->scan.status.release();
     ctx->sel[0].status.release(); ctx->sel[1].status.release(); ctx->input_zbuf.release();
     for (auto& b : ctx->kd.store) b.release();
-    ctx->kd.morton.release(); ctx->kd.order.release(); ctx->kd.sorted.release(); ctx->kd.normals.release();
+    ctx->kd.morton.release(); ctx->kd.order.release(); ctx->kd.sorted.release(); ctx->kd.sorted_prev.release(); ctx->kd.normals.release();
     ctx->kd.bbox.release(); ctx->kd.grid_hdr.release(); ctx->kd.cells.release(); ctx->kd.stats.release();
     ctx->kd_worklist.release(); ctx->kd_nn_state.release();
     ctx->pm.vmaps.release(); ctx->pm.nmaps.release(); ctx->pm.poses.release();
@@ -335,6 +335,7 @@ int pls_destroy(pls_context* ctx) {
     if (ctx->ev_map_done) cudaEventDestroy(ctx->ev_map_done);
     if (ctx->ev_inputs) cudaEventDestroy(ctx->ev_inputs);
     if (ctx->ev_batch) cudaEventDestroy(ctx->ev_batch);
+    if (ctx->ev_icp_done) cudaEventDestroy(ctx->ev_icp_done);
     ctx->gs_host_xyz.release(); ctx->gs_host_idx.release();
     if (ctx->stream_map) cudaStreamDestroy(ctx->stream_map);
     if (ctx->own_stream) cudaStreamDestroy(ctx->stream_main);

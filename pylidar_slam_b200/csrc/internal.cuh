@@ -130,6 +130,8 @@ struct KdMap {
     // search index
     DBuf morton, order;     // u64 cell keys, u32 original index (sorted)
     DBuf sorted;            // float4 (x,y,z, bitcast original index), level-0 cell order
+    DBuf sorted_prev;       // a device-decided update builds into the other buffer: the sorted points of generation
+    uint32_t prev_gen = 0;  // prev_gen (0: none), which the last frame's search ran on, stay exportable
     DBuf normals;           // float4 (nx,ny,nz, state word) in sorted order; states carry the build generation
     DBuf bbox;              // 6 ordered-int words
     bool bbox_clean = false; // the header kernel of the last build left the box empty
@@ -183,6 +185,22 @@ struct Comm;  // NCCL glue (comm.cu)
 
 static_assert(sizeof(FrameResult) <= kScalarOffset, "FrameResult must fit before the scalar slots");
 
+// The kd map update of a frame as its device-side decision (kd_update_decision_kernel, odometry.cu) leaves it for the
+// update's launches, in the scalar block behind the FrameResult, so that the frame's one result copy brings it back.
+struct KdUpdateWords {
+    float X[12];          // the move inverse(T): R row-major, then t
+    float delta[16];      // _delta_since_map_update after the frame
+    uint32_t gate;        // 1: the update runs -- the frame's ICP is complete and succeeded on a valid grid sample
+    uint32_t insert;      // the frame is a key frame
+    uint32_t skip;        // points of the evicted frame, at the front of the store
+    uint32_t kept;        // points moved
+    uint32_t num_new;     // points appended
+    uint32_t total;       // map points after the update (kept + num_new; 0 while the gate is closed)
+    uint32_t pad[2];
+};
+constexpr size_t kUpdateOffset = kScalarOffset - 256;
+static_assert(sizeof(FrameResult) <= kUpdateOffset && sizeof(KdUpdateWords) <= 256, "KdUpdateWords after FrameResult");
+
 }  // namespace pls
 
 struct pls_context {
@@ -226,8 +244,9 @@ struct pls_context {
     pls::DBuf frame_vmap_buf[2];        // [3][H][W] of the current frame (double-buffered: the previous one may
     pls::DBuf frame_pts_buf[2];         // still be read by the map-update stream); float4 packed valid points
     int frame_slot = 0;
-    // the local-map update of the last frame, decided but not yet enqueued: the next call enqueues it once its own
-    // first kernels are in flight (flush_map_update), so its launches leave the critical path of both calls
+    // the local-map update of the last frame, decided by the host but not yet enqueued: the next call enqueues it first
+    // (flush_map_update).  A kd map's update on one GPU is decided on the device and enqueued with its frame instead
+    // (odometry.cu: enqueue_device_map_update), and none is left pending
     bool upd_pending = false, upd_insert = false;
     float upd_T[16];
     int upd_slot = 0;
@@ -241,6 +260,7 @@ struct pls_context {
     pls::DBuf batch_buf;                // pls_process_frames led by this context: sequence descriptors, then done flags
     pls::DBuf hyp_buf;                  // pls_register_hypotheses: FrameResults and per-query state of the hypotheses
     cudaEvent_t ev_batch = nullptr;     // pls_process_frames: this context's input stage, before the batched ICP
+    cudaEvent_t ev_icp_done = nullptr;  // a frame's ICP launches and its map-update decision, before the map stream's update
     pls::DBuf gs_keys, gs_vals, gs_out_xyz, gs_out_idx;
     uint32_t gs_seq = 0;                // stamp of the last compact-key grid sample (overflow detection)
     pls::HBuf gs_host_xyz, gs_host_idx; // pinned + mapped staging the grid sample's gather writes directly (host callers)
@@ -309,6 +329,12 @@ inline uint32_t* scalar_u32(pls_context* ctx, int i) {
 }
 inline FrameResult* frame_result_dev(pls_context* ctx) { return reinterpret_cast<FrameResult*>(ctx->scalars.p); }
 inline FrameResult* frame_result_host(pls_context* ctx) { return reinterpret_cast<FrameResult*>(ctx->pinned.p); }
+inline KdUpdateWords* kd_update_words_dev(pls_context* ctx) {
+    return reinterpret_cast<KdUpdateWords*>(reinterpret_cast<char*>(ctx->scalars.p) + kUpdateOffset);
+}
+inline const KdUpdateWords* kd_update_words_host(pls_context* ctx) {
+    return reinterpret_cast<const KdUpdateWords*>(reinterpret_cast<const char*>(ctx->pinned.p) + kUpdateOffset);
+}
 
 // The asynchronous map-update scope: kernels enqueued inside run on stream_map with its own sort scratch.
 void map_stream_begin(pls_context* ctx);
@@ -342,8 +368,9 @@ inline void profile_credit(pls_context* ctx, int which, int64_t launches, double
 // pointers stored in DEVICE memory (the plan), and also returned on the host when the number of
 // executed passes is statically known (no skipping), which is how it is used here.
 // cap_n >= n: the scratch is sized for cap_n elements (callers whose n grows towards a known bound pass the bound).
+// n_dev (nullable): the element count on the device, read by the kernels; n is then a bound of it that sizes the launches.
 void radix_sort_pairs(pls_context* ctx, uint64_t* keys, uint32_t* vals, int64_t n, int num_passes,
-                      uint64_t** keys_out, uint32_t** vals_out, int64_t cap_n = 0);
+                      uint64_t** keys_out, uint32_t** vals_out, int64_t cap_n = 0, const uint32_t* n_dev = nullptr);
 
 // Exclusive scan / stream compaction with a single-pass decoupled look-back.
 // flags[i] in {0,1}; pos_out[i] = number of set flags before i; *total_dev = number set.
@@ -398,6 +425,16 @@ void kdmap_reset(pls_context* ctx);
 void kdmap_update(pls_context* ctx, const float* rel_pose_host, const float* pts_dev, int64_t n,
                   const float* vmap_dev, int H, int W, int64_t known_count);
 // insertion of already packed float4 points (nullable) whose count the host knows
+// The update as the device decided it (*upd, written on the map stream's side of an event before the launches run).
+// kdmap_device_update_bound: the point count the launches are sized for -- the map's count + new_bound new points,
+// clamped to the capacity already planned -- or 0 when the update has to stay on the host's path (a first insertion, a
+// generation restart).  The device closes the update's gate when the new count exceeds the bound, and the host then
+// decides and enqueues that update itself, re-planning the capacity as it always did: capacity and index geometry come
+// out as a host-decided update plans them.  kdmap_settle_device_update: the host mirror (counts, the per-frame counts,
+// the index size) once *upd is back on the host with the gate open.
+int64_t kdmap_device_update_bound(const pls_context* ctx, int64_t new_bound);
+void kdmap_update_on_device(pls_context* ctx, const float4* fresh_dev, int64_t bound, const KdUpdateWords* upd);
+void kdmap_settle_device_update(pls_context* ctx, const KdUpdateWords& w, int local_map_size);
 void kdmap_update_packed(pls_context* ctx, const float* rel_pose_host, const float4* fresh_dev, int64_t num_new,
                          bool has_new);
 // pls_process_frames: the ICP of `num` sequences (distinct kd-map contexts, no communicator) in batched launches on st.

@@ -41,12 +41,22 @@ struct Rigid {
 };
 
 // dst[k] = R src[k + skip] + t for k < kept;  dst[kept + j] = fresh[j] for j < num_new (from a
-// device count);  bounding box of everything written.
+// device count);  bounding box of everything written.  upd: the device decided the update (kd_update_decision_kernel):
+// skip, kept, num_new and the move come from it (all counts 0 when its gate is closed).
 __global__ void __launch_bounds__(256)
 kd_move_append_kernel(const float4* __restrict__ src, int64_t skip, int64_t kept, Rigid X,
                       const float4* __restrict__ fresh, const uint32_t* __restrict__ num_new_dev, int64_t num_new_cap,
-                      float4* __restrict__ dst, int* __restrict__ bbox) {
-    const int64_t num_new = num_new_dev ? (int64_t)*num_new_dev : num_new_cap;
+                      float4* __restrict__ dst, int* __restrict__ bbox, const KdUpdateWords* __restrict__ upd) {
+    int64_t num_new = num_new_dev ? (int64_t)*num_new_dev : num_new_cap;
+    if (upd) {
+        skip = upd->skip;
+        kept = upd->kept;
+        num_new = upd->num_new;
+#pragma unroll
+        for (int i = 0; i < 9; ++i) X.R[i] = upd->X[i];
+#pragma unroll
+        for (int i = 0; i < 3; ++i) X.t[i] = upd->X[9 + i];
+    }
     const int64_t total = kept + num_new;
     float mn[3] = {FLT_MAX, FLT_MAX, FLT_MAX}, mx[3] = {-FLT_MAX, -FLT_MAX, -FLT_MAX};
     for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < total; k += (int64_t)gridDim.x * blockDim.x) {
@@ -182,8 +192,10 @@ __global__ void kd_pack_pixels_kernel(const float* __restrict__ vmap, int64_t hw
 // Morton-interleaved) fits 30 bits and the sort needs four 8-bit passes whatever the extent; the unit is chosen so
 // that the cell side equals the target -- or, for maps wider than 1024 cells, so that the 13-bit range just covers the
 // extent (coarser cells).  The coarsest level (top = 10) is a single cell.
-__global__ void kd_grid_header_kernel(int* __restrict__ bbox, KdGridHeader* __restrict__ hdr, float cell_target) {
-    if (threadIdx.x != 0) return;
+// gate (nullable): a device-decided update whose gate is closed leaves the header (which the ICP reads) as it is.
+__global__ void kd_grid_header_kernel(int* __restrict__ bbox, KdGridHeader* __restrict__ hdr, float cell_target,
+                                      const uint32_t* __restrict__ gate) {
+    if (threadIdx.x != 0 || (gate && !*gate)) return;
     const float mnx = ordered_to_float(bbox[0]), mny = ordered_to_float(bbox[1]), mnz = ordered_to_float(bbox[2]);
     const float ex = ordered_to_float(bbox[3]) - mnx, ey = ordered_to_float(bbox[4]) - mny,
                 ez = ordered_to_float(bbox[5]) - mnz;
@@ -203,9 +215,11 @@ __global__ void kd_grid_header_kernel(int* __restrict__ bbox, KdGridHeader* __re
 
 // Sort key of a map point = the Morton id of its level-0 cell (<= 30 bits); the order inside a cell is the
 // insertion order (stable sort), nothing finer is needed: every level's cell is a prefix of this id.
+// n_dev (nullable): the point count on the device, n a bound of it.
 __global__ void kd_cell_key_kernel(const float4* __restrict__ pts, int64_t n, const KdGridHeader* __restrict__ hdr,
-                                   uint64_t* __restrict__ keys, uint32_t* __restrict__ vals) {
+                                   uint64_t* __restrict__ keys, uint32_t* __restrict__ vals, const uint32_t* __restrict__ n_dev) {
     pls_grid_dependency_wait();
+    if (n_dev) n = *n_dev;
     const float mnx = hdr->mn[0], mny = hdr->mn[1], mnz = hdr->mn[2];
     const float scale = hdr->scale;
     const int b0 = hdr->b0;
@@ -249,8 +263,10 @@ __device__ __forceinline__ int cell_claim(uint4* table, uint32_t mask, uint32_t 
 // `first`, tails store `last` into the slot they find-or-claim.
 __global__ void __launch_bounds__(256)
 kd_finalize_kernel(const float4* __restrict__ pts, const uint64_t* __restrict__ keys, const uint32_t* __restrict__ order,
-                   int64_t n, CellTables T, KdGridHeader* hdr, uint32_t gen, float4* __restrict__ sorted) {
+                   int64_t n, CellTables T, KdGridHeader* hdr, uint32_t gen, float4* __restrict__ sorted,
+                   const uint32_t* __restrict__ n_dev) {
     pls_grid_dependency_wait();
+    if (n_dev) n = *n_dev;
     const int top = hdr->top;
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
         const uint32_t src = order[i];
@@ -1065,14 +1081,17 @@ KdIndex make_index(pls_context* ctx) {
 
 // The per-frame index build (stands in for the KDTree rebuild of local_map.py:365-369): header, cell keys, four
 // radix passes, one finishing pass.  Nothing is cleared: tables and normal states carry the build's generation.
-void build_index(pls_context* ctx) {
+// upd (nullable): kd.count is a bound of the point count, which the device holds in upd->total (the launches are sized
+// for the bound and read the count; the caller settles kd.indexed / kd.valid and the profile credit once it is known).
+void build_index(pls_context* ctx, const KdUpdateWords* upd) {
     KdMap& kd = ctx->kd;
     cudaStream_t st = ctx->stream;
     const int64_t M = kd.count;
     kd.indexed = M;
     kd.valid = M > 0;
     if (M <= 0) return;
-    ProfileScope ps(ctx, 3, (double)M * 32.0);
+    ProfileScope ps(ctx, 3, (double)M * 32.0, upd == nullptr);
+    const uint32_t* n_dev = upd ? &upd->total : nullptr;
     PLS_REQUIRE(M < (1ll << 30), "kd map: too many points");
     kd_reserve_capacity(ctx, M);
     kd.gen += 1;
@@ -1084,14 +1103,15 @@ void build_index(pls_context* ctx) {
     const float4* pts = kd.store[kd.cur].as<float4>();
     kd.grid_hdr.reserve(sizeof(KdGridHeader), st);
     static const float cell_target = getenv("PLS_KD_CELL") ? (float)atof(getenv("PLS_KD_CELL")) : KD_CELL_TARGET;
-    kd_grid_header_kernel<<<1, 32, 0, st>>>(kd.bbox.as<int>(), kd.grid_hdr.as<KdGridHeader>(), cell_target);
+    kd_grid_header_kernel<<<1, 32, 0, st>>>(kd.bbox.as<int>(), kd.grid_hdr.as<KdGridHeader>(), cell_target,
+                                            upd ? &upd->gate : nullptr);
     PLS_CHECK_LAUNCH();
     kd.bbox_clean = true;
     launch_dependent(kd_cell_key_kernel, grid_for(M, 256, 8 * kNumSMs), 256, st, pts, M, kd.grid_hdr.as<KdGridHeader>(),
-                     kd.morton.as<uint64_t>(), kd.order.as<uint32_t>());
+                     kd.morton.as<uint64_t>(), kd.order.as<uint32_t>(), n_dev);
     uint64_t* sk;
     uint32_t* sv;
-    radix_sort_pairs(ctx, kd.morton.as<uint64_t>(), kd.order.as<uint32_t>(), M, 4, &sk, &sv, kd.cap_points);
+    radix_sort_pairs(ctx, kd.morton.as<uint64_t>(), kd.order.as<uint32_t>(), M, 4, &sk, &sv, kd.cap_points, n_dev);
     // table geometry follows the capacity, not M: it only changes when the buffers are re-planned
     cell_table_bytes(kd.cap_points, kd.table_mask, kd.table_offset);
     CellTables T;
@@ -1100,7 +1120,7 @@ void build_index(pls_context* ctx) {
         T.mask[l] = kd.table_mask[l];
     }
     launch_dependent(kd_finalize_kernel, grid_for(M, 256, 8 * kNumSMs), 256, st, pts, sk, sv, M, T, kd.grid_hdr.as<KdGridHeader>(),
-                     kd.gen, kd.sorted.as<float4>());
+                     kd.gen, kd.sorted.as<float4>(), n_dev);
 }
 
 }  // namespace
@@ -1167,12 +1187,42 @@ void pack_valid_pixels(pls_context* ctx, const float* vmap_dev, int64_t hw, floa
     PLS_CHECK_LAUNCH();
 }
 
+namespace {
+
+// The device side of a map update: move + append + evict into the other store, then the index rebuild.  total is the
+// new point count, or with upd a bound of it (see build_index).
+void move_and_rebuild(pls_context* ctx, int64_t skip, int64_t kept, const Rigid& X, const float4* fresh_dev,
+                      int64_t num_new, int64_t total, const KdUpdateWords* upd) {
+    KdMap& kd = ctx->kd;
+    cudaStream_t st = ctx->stream;
+    kd_reserve_capacity(ctx, total > 0 ? total : 1);
+    const int dst = kd.cur ^ 1;
+    kd.bbox.reserve(8 * sizeof(int), st);
+    if (!kd.bbox_clean) {
+        kd_bbox_init_kernel<<<1, 32, 0, st>>>(kd.bbox.as<int>());
+        PLS_CHECK_LAUNCH();
+    }
+    kd.bbox_clean = false;
+    if (total > 0) {
+        kd_move_append_kernel<<<grid_for(total, 256, 8 * kNumSMs), 256, 0, st>>>(
+            kd.store[kd.cur].as<float4>(), skip, kept, X, fresh_dev, nullptr, num_new, kd.store[dst].as<float4>(),
+            kd.bbox.as<int>(), upd);
+        PLS_CHECK_LAUNCH();
+    }
+    kd.cur = dst;
+    kd.count = total;
+    // a device-decided update leaves the searched generation's sorted points in sorted_prev (its caller swapped)
+    kd.prev_gen = upd ? kd.gen : 0;
+    build_index(ctx, upd);
+}
+
+}  // namespace
+
 // Move the map by inverse(rel_pose), append `num_new` packed points, evict, rebuild the index
 // (local_map.py:330-369).
 void kdmap_update_packed(pls_context* ctx, const float* rel_pose_host, const float4* fresh_dev, int64_t num_new,
                          bool has_new) {
     KdMap& kd = ctx->kd;
-    cudaStream_t st = ctx->stream;
     Rigid X;
     int64_t skip = 0;
     const bool first = kd.frame_counts.empty() && kd.count == 0;
@@ -1199,23 +1249,41 @@ void kdmap_update_packed(pls_context* ctx, const float* rel_pose_host, const flo
     const int64_t kept = kd.count - skip;
     const int64_t total = kept + num_new;
     if (num_new > kd.max_frame) kd.max_frame = num_new;
-    kd_reserve_capacity(ctx, total > 0 ? total : 1);
-    const int dst = kd.cur ^ 1;
-    kd.bbox.reserve(8 * sizeof(int), st);
-    if (!kd.bbox_clean) {
-        kd_bbox_init_kernel<<<1, 32, 0, st>>>(kd.bbox.as<int>());
-        PLS_CHECK_LAUNCH();
+    move_and_rebuild(ctx, skip, kept, X, fresh_dev, num_new, total, nullptr);
+}
+
+int64_t kdmap_device_update_bound(const pls_context* ctx, int64_t new_bound) {
+    const KdMap& kd = ctx->kd;
+    if (kd.frame_counts.empty() || kd.gen + 1 >= 0x7ffffff0u) return 0;
+    int64_t bound = kd.count + new_bound;
+    if (bound > kd.cap_points) bound = kd.cap_points;
+    if (bound > (1ll << 30) - 1) bound = (1ll << 30) - 1;
+    return bound;
+}
+
+void kdmap_update_on_device(pls_context* ctx, const float4* fresh_dev, int64_t bound, const KdUpdateWords* upd) {
+    KdMap& kd = ctx->kd;
+    PLS_REQUIRE(bound > 0 && bound >= kd.count && bound <= kd.cap_points,
+                "kd map: a device-decided update needs a bound within the planned capacity");
+    // the host enqueues this before it has seen the frame's result, whose last correspondences
+    // (pls_kdmap_last_correspondences) read the sorted points of the index the frame searched: the build writes the
+    // other buffer
+    std::swap(kd.sorted, kd.sorted_prev);
+    kd.sorted.reserve_exact((size_t)kd.cap_points * sizeof(float4), ctx->stream);
+    move_and_rebuild(ctx, 0, bound, Rigid{}, fresh_dev, bound - kd.count, bound, upd);
+}
+
+void kdmap_settle_device_update(pls_context* ctx, const KdUpdateWords& w, int local_map_size) {
+    KdMap& kd = ctx->kd;
+    if (w.insert) {
+        kd.frame_counts.push_back((int64_t)w.num_new);
+        if ((int)kd.frame_counts.size() > local_map_size) kd.frame_counts.pop_front();
+        if ((int64_t)w.num_new > kd.max_frame) kd.max_frame = (int64_t)w.num_new;
     }
-    kd.bbox_clean = false;
-    if (total > 0) {
-        kd_move_append_kernel<<<grid_for(total, 256, 8 * kNumSMs), 256, 0, st>>>(
-            kd.store[kd.cur].as<float4>(), skip, kept, X, fresh_dev, nullptr, num_new, kd.store[dst].as<float4>(),
-            kd.bbox.as<int>());
-        PLS_CHECK_LAUNCH();
-    }
-    kd.cur = dst;
-    kd.count = total;
-    build_index(ctx);
+    kd.count = (int64_t)w.total;
+    kd.indexed = kd.count;
+    kd.valid = kd.count > 0;
+    if (kd.count > 0) profile_credit(ctx, 3, 1, (double)kd.count * 32.0);
 }
 
 void kdmap_update(pls_context* ctx, const float* rel_pose_host, const float* pts_dev, int64_t n,
@@ -1758,7 +1826,11 @@ int pls_kdmap_last_correspondences(pls_context* ctx, int64_t n, int64_t* out_idx
     PLS_API_BEGIN_FRAME(ctx)
     const KdMap& kd = ctx->kd;
     if (!kd.searched) throw pls::Error{PLS_E_STATE, "pls_kdmap_last_correspondences: no kd search has run"};
-    if (!kd.valid || kd.searched_gen != kd.gen)
+    // the search ran on the current index, or on the one the frame's own device-decided update has since replaced
+    // (its sorted points are kept in sorted_prev; the normals are only rewritten by the next search)
+    const bool current = kd.valid && kd.searched_gen == kd.gen;
+    const bool replaced = kd.prev_gen != 0 && kd.searched_gen == kd.prev_gen;
+    if (!current && !replaced)
         throw pls::Error{PLS_E_STATE, "pls_kdmap_last_correspondences: the map was rebuilt since the last search"};
     if (kd.searched_sharded)
         throw pls::Error{PLS_E_STATE, "pls_kdmap_last_correspondences: the last ICP split its queries over the ranks"};
@@ -1780,8 +1852,10 @@ int pls_kdmap_last_correspondences(pls_context* ctx, int64_t n, int64_t* out_idx
             ctx->stage_out[3].reserve((size_t)n * 3 * sizeof(float), st);
             nb = ctx->stage_out[3].as<float>();
         }
+        KdIndex ix = make_index(ctx);
+        if (!current) ix.sorted = kd.sorted_prev.as<float4>();
         kd_search_export_kernel<<<grid_for(n, 256, 8 * kNumSMs), 256, 0, st>>>(
-            make_index(ctx), ctx->nn_prev.as<int>(), n, nb, kd.searched_normals ? (float*)onr.dev : nullptr,
+            ix, ctx->nn_prev.as<int>(), n, nb, kd.searched_normals ? (float*)onr.dev : nullptr,
             (long long*)oix.dev);
         PLS_CHECK_LAUNCH();
         if (onr.dev && !kd.searched_normals)  // the search computed no normals: NaN

@@ -8,6 +8,8 @@
 #include <stdlib.h>
 
 #include <chrono>
+#include <functional>
+#include <optional>
 #include <utility>
 #include <vector>
 
@@ -301,14 +303,98 @@ int enqueue_icp_iterations(pls_context* ctx, int64_t query_bound, const uint32_t
     return last_blocks;
 }
 
-// PLS_HOST_TRACE=1: host-side time of the phases of a frame (enqueue up to the ICP, the wait for the pose, the
-// map-update enqueue), averaged and printed every 64 frames -- a development aid for the end-to-end path.
+// __update_map's key-frame decision (keyframe_decision) and the move of the map (kdmap_update_packed) on the device,
+// one thread, behind a frame's ICP launches: the map update can then be enqueued before the host has seen the pose.
+// The float and double arithmetic is that of the host code, rounded operation by operation (__fmul_rn & co.: no
+// contraction into FMAs, which the host build does not do either), so that the move X and the new delta are the host's
+// bits.  The decision also goes through atan2f, whose device result may differ from glibc's by a few ulp (CUDA documents
+// a 3-ulp bound): a decision can only differ from the host's when the rotation angle lies within a few ulp of
+// threshold_rot.
+// The gate opens when the frame needs no further ICP launches (done, or max_num_alignments iterations), its ICP did not
+// fail, its grid sample's compact keys did not overflow (gs_overflow: the stamp word, or null), and the new map count
+// fits total_limit, the count the update's launches are sized for; while it is closed every count is 0 and the update's
+// launches do nothing.
+__device__ __forceinline__ void mat4_mul_rn(const float* A, const float* B, float* C) {
+    for (int i = 0; i < 4; ++i)
+        for (int j = 0; j < 4; ++j) {
+            float s = 0.f;
+            for (int k = 0; k < 4; ++k) s = __fadd_rn(s, __fmul_rn(A[i * 4 + k], B[k * 4 + j]));
+            C[i * 4 + j] = s;
+        }
+}
+
+__device__ __forceinline__ float norm3_rn(float a, float b, float c) {
+    return __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(a, a), __fmul_rn(b, b)), __fmul_rn(c, c)));
+}
+
+__global__ void kd_update_decision_kernel(const FrameResult* __restrict__ fr, KdUpdateWords* __restrict__ w, Pose16 delta,
+                                          float threshold_trans, float threshold_rot, int max_num_alignments,
+                                          uint32_t map_count, uint32_t evict_count, uint32_t total_limit,
+                                          const uint32_t* __restrict__ gs_overflow, uint32_t gs_seq) {
+    const bool failed = fr->status == PLS_E_SINGULAR || fr->status == PLS_E_COMM;
+    const bool ready = (fr->done || fr->iters >= max_num_alignments) && !failed && !(gs_overflow && *gs_overflow == gs_seq);
+    float T[16];
+    for (int i = 0; i < 16; ++i) T[i] = fr->T[i];
+    // keyframe_decision: the accumulated motion nd = delta T, its translation and Euler-angle norms
+    float nd[16];
+    mat4_mul_rn(delta.m, T, nd);
+    float sy = __fsqrt_rn(__fadd_rn(__fmul_rn(nd[0], nd[0]), __fmul_rn(nd[4], nd[4])));
+    float e[3];  // mat_to_euler
+    if (!(sy < 1e-6f)) {
+        e[0] = atan2f(nd[9], nd[10]);
+        e[1] = atan2f(-nd[8], sy);
+        e[2] = atan2f(nd[4], nd[0]);
+    } else {
+        e[0] = atan2f(-nd[6], nd[5]);
+        e[1] = atan2f(-nd[8], sy);
+        e[2] = 0.f;
+    }
+    const float tn = norm3_rn(nd[3], nd[7], nd[11]);
+    const float rn = norm3_rn(e[0], e[1], e[2]);
+    bool insert = ready && (tn > threshold_trans ||
+                            __fdiv_rn(__fmul_rn(rn, 180.0f), 3.14159265358979323846f) > threshold_rot);
+    // the new count: kdmap_update_packed's kept + num_new (a larger one is left to the host, which re-plans the capacity)
+    const bool gate = ready && map_count - (insert ? evict_count : 0u) + (insert ? (uint32_t)fr->counts[2] : 0u) <= total_limit;
+    insert = insert && gate;
+    // rigid_inverse(T): (R^T, -R^T t) in double
+    const double R[9] = {T[0], T[1], T[2], T[4], T[5], T[6], T[8], T[9], T[10]};
+    const double t[3] = {T[3], T[7], T[11]};
+    for (int i = 0; i < 3; ++i) {
+        for (int j = 0; j < 3; ++j) w->X[3 * i + j] = (float)R[j * 3 + i];
+        w->X[9 + i] = __double2float_rn(
+            -__dadd_rn(__dadd_rn(__dmul_rn(R[i], t[0]), __dmul_rn(R[3 + i], t[1])), __dmul_rn(R[6 + i], t[2])));
+    }
+    for (int i = 0; i < 16; ++i) w->delta[i] = !gate ? delta.m[i] : (insert ? ((i % 5 == 0) ? 1.f : 0.f) : nd[i]);
+    const uint32_t num_new = insert ? (uint32_t)fr->counts[2] : 0u;
+    const uint32_t skip = insert ? evict_count : 0u;
+    w->gate = gate ? 1u : 0u;
+    w->insert = insert ? 1u : 0u;
+    w->skip = gate ? skip : 0u;
+    w->kept = gate ? map_count - skip : 0u;
+    w->num_new = num_new;
+    w->total = gate ? map_count - skip + num_new : 0u;
+}
+
+// PLS_HOST_TRACE=1: host-side time of the phases of a frame (the grid-sampled call's prologue: a deferred map-update
+// enqueue, then the grid-sample enqueue; the enqueue of the input stage and the ICP, the wait for the pose, the map
+// update: its enqueue behind the ICP when the device decides it, else the host's decision), averaged and printed every
+// 64 frames -- a development aid for the end-to-end path.
 struct HostTrace {
     bool on = getenv("PLS_HOST_TRACE") != nullptr;
-    double acc[4] = {0, 0, 0, 0};
+    bool in_call = false;  // begin_call() ran: process_frame_device closes the prologue lap instead of starting afresh
+    double acc[6] = {0, 0, 0, 0, 0, 0};
     int frames = 0, extra_rounds = 0;
     std::chrono::steady_clock::time_point t;
     void start() { if (on) t = std::chrono::steady_clock::now(); }
+    void begin_call() {
+        start();
+        in_call = on;
+    }
+    void frame_start() {  // the start of process_frame_device
+        if (in_call) lap(5);
+        else start();
+        in_call = false;
+    }
     void lap(int k) {
         if (!on) return;
         const auto now = std::chrono::steady_clock::now();
@@ -317,12 +403,14 @@ struct HostTrace {
     }
     void end_frame() {
         if (!on || ++frames < 64) return;
-        fprintf(stderr, "[plslam_b200 host trace] per frame: enqueue input+ICP %.1f us, wait for the pose %.1f us, "
-                        "map-update enqueue %.1f us, rest %.1f us; %d of %d frames needed a second round of ICP launches\n",
-                acc[0] / frames, acc[1] / frames, acc[2] / frames, acc[3] / frames, extra_rounds, frames);
+        fprintf(stderr, "[plslam_b200 host trace] per frame: call prologue: map-update flush %.1f us, grid-sample "
+                        "enqueue %.1f us; enqueue input+ICP %.1f us, wait for the pose %.1f us, map update %.1f us, "
+                        "rest %.1f us; %d of %d frames needed a second round of ICP launches\n",
+                acc[4] / frames, acc[5] / frames, acc[0] / frames, acc[1] / frames, acc[2] / frames, acc[3] / frames,
+                extra_rounds, frames);
         frames = 0;
         extra_rounds = 0;
-        acc[0] = acc[1] = acc[2] = acc[3] = 0;
+        for (double& a : acc) a = 0;
     }
 };
 HostTrace g_trace;
@@ -418,28 +506,6 @@ int icp_rounds(pls_context* const* ctxs, int num, Enqueue enqueue, ReadDone read
     return extra;
 }
 
-// The ICP loop of one frame over ctx->query_ptr / counts[1], on ctx->stream.  Returns the launched block count of the
-// correspondence kernel.
-int run_icp(pls_context* ctx, int64_t query_bound, const uint32_t* bound_dev) {
-    cudaStream_t st = ctx->stream;
-    FrameResult* fr = frame_result_dev(ctx);
-    if (query_bound < 1) query_bound = 1;
-    ctx->pm.zbuf_clean = false;  // tmp[3] may have been used by the frame's own projection
-    int blocks = 0;
-    auto enqueue = [&](int first, int last) {
-        blocks = enqueue_icp_iterations(ctx, query_bound, bound_dev, first, last);
-        if (first == 0) g_trace.lap(0);
-    };
-    auto read_done = [&](int* done) {
-        int flags[3];  // iters, status, done
-        PLS_CUDA(cudaMemcpyAsync(flags, &fr->iters, sizeof(flags), cudaMemcpyDeviceToHost, st));
-        PLS_CUDA(cudaStreamSynchronize(st));
-        done[0] = flags[2];
-    };
-    g_trace.extra_rounds += icp_rounds(&ctx, 1, enqueue, read_done);
-    return blocks;
-}
-
 // The FrameResult and the u32 / u64 scalar slots behind it in one copy to the pinned host mirror, on st.
 void enqueue_result_copy(pls_context* ctx, cudaStream_t st) {
     PLS_CUDA(cudaMemcpyAsync(ctx->pinned.p, ctx->scalars.p, kScalarOffset + SC_NUM * sizeof(uint32_t), cudaMemcpyDeviceToHost,
@@ -449,6 +515,42 @@ void enqueue_result_copy(pls_context* ctx, cudaStream_t st) {
 void fetch_result(pls_context* ctx) {
     enqueue_result_copy(ctx, ctx->stream);
     PLS_CUDA(cudaStreamSynchronize(ctx->stream));
+}
+
+// The ICP loop of one frame over ctx->query_ptr / counts[1], on ctx->stream, up to the host copy of its result.
+// after_upfront (may be empty) is enqueued behind the up-front launches, before the host first waits.  Each look at the
+// done flag copies the whole result, so a frame that needs no second round of launches costs the host one wait.
+// Returns the launched block count of the correspondence kernel; *extra_rounds: the rounds of launches after the first.
+int run_icp(pls_context* ctx, int64_t query_bound, const uint32_t* bound_dev, const std::function<void()>& after_upfront,
+            int* extra_rounds) {
+    if (query_bound < 1) query_bound = 1;
+    ctx->pm.zbuf_clean = false;  // tmp[3] may have been used by the frame's own projection
+    int blocks = 0;
+    bool fresh = false;  // the host copy holds the result of every launch enqueued so far
+    auto enqueue = [&](int first, int last) {
+        blocks = enqueue_icp_iterations(ctx, query_bound, bound_dev, first, last);
+        fresh = false;
+        if (first == 0) {
+            g_trace.lap(0);
+            if (after_upfront) {
+                after_upfront();
+                g_trace.lap(2);
+            }
+        }
+    };
+    auto read_done = [&](int* done) {
+        fetch_result(ctx);
+        fresh = true;
+        done[0] = frame_result_host(ctx)->done;
+    };
+    *extra_rounds = icp_rounds(&ctx, 1, enqueue, read_done);
+    g_trace.extra_rounds += *extra_rounds;
+    if (*extra_rounds > 0 && after_upfront) {  // behind the last round: the update's gate opens this time
+        after_upfront();
+        fresh = false;
+    }
+    if (!fresh) fetch_result(ctx);
+    return blocks;
 }
 
 // Algorithmic bytes of the frame's executed ICP iterations, by SURVEY.md 8d's formulas.
@@ -531,6 +633,7 @@ struct FrameIn {
     int64_t pts_bound = 0;    // rows of the frame's own points, NaN rows included (a bound of them, with n_dev)
     int64_t query_bound = 0;  // bound of the query count
     const uint32_t* n_dev = nullptr;  // the row count on the device, when the host knows only the bound pts_bound
+    int64_t map_points = 0;   // points of the kd map the frame registers against (info[3])
 };
 
 // The caller's outputs of one frame, each nullable.
@@ -716,24 +819,33 @@ bool frame_input(pls_context* ctx, const void* data_void, int layout, int64_t n,
     // ---- register_new_frame
     flush_map_update(ctx);  // (already enqueued by the grid-sample call of this frame, if there was one)
     map_stream_wait(ctx);   // the ICP below reads the local map the previous frame's update is still building
+    in.map_points = ctx->kd.count;
     frame_begin(ctx, init_pose, nullptr, queries_are_rows);
     return true;
 }
 
 // The epilogue of a frame whose ICP result is in the host FrameResult: status, key-frame decision, the deferred map
 // update, outputs.  Throws on a failed ICP, leaving the frame unadvanced and no map update pending.
-void frame_epilogue(pls_context* ctx, const FrameIn& in, const FrameOut& out, bool trace) {
+// upd (nullable): the device decided and enqueued the kd map update (with its gate open); the host mirror follows it.
+void frame_epilogue(pls_context* ctx, const FrameIn& in, const FrameOut& out, bool trace, const KdUpdateWords* upd) {
     FrameResult* h = frame_result_host(ctx);
     ctx->last_icp_iters = h->iters;
     raise_status(ctx, h->status);
 
-    // ---- __update_map: decided now, enqueued (on the map stream, beside the NEXT frame's preprocessing) by the next call
-    const bool insert = keyframe_decision(ctx, h->T);
-    ctx->upd_pending = true;
-    ctx->upd_insert = insert;
-    memcpy(ctx->upd_T, h->T, sizeof(ctx->upd_T));
-    ctx->upd_slot = ctx->frame_slot;
-    ctx->upd_count = (long long)h->counts[2];
+    // ---- __update_map
+    bool insert;
+    if (upd) {
+        insert = upd->insert != 0;
+        memcpy(ctx->delta_since_update, upd->delta, sizeof(ctx->delta_since_update));
+        kdmap_settle_device_update(ctx, *upd, ctx->cfg.local_map_size);
+    } else {  // decided now, enqueued (on the map stream, beside the NEXT frame's preprocessing) by the next call
+        insert = keyframe_decision(ctx, h->T);
+        ctx->upd_pending = true;
+        ctx->upd_insert = insert;
+        memcpy(ctx->upd_T, h->T, sizeof(ctx->upd_T));
+        ctx->upd_slot = ctx->frame_slot;
+        ctx->upd_count = (long long)h->counts[2];
+    }
     if (trace) g_trace.lap(2);
     ctx->frame_index += 1;
     if (out.pose) memcpy(out.pose, h->T, 16 * sizeof(float));
@@ -743,7 +855,7 @@ void frame_epilogue(pls_context* ctx, const FrameIn& in, const FrameOut& out, bo
         out.info[0] = (double)h->iters;
         out.info[1] = h->iters > 0 ? (double)h->losses[h->iters - 1] : 0.0;
         out.info[2] = (double)h->counts[1];
-        out.info[3] = (double)ctx->kd.count;
+        out.info[3] = (double)in.map_points;
         out.info[4] = (double)h->counts[0];
         out.info[5] = (double)(in.pts_bound - (int64_t)h->counts[2]);
         out.info[6] = (double)h->status;
@@ -754,18 +866,93 @@ void frame_epilogue(pls_context* ctx, const FrameIn& in, const FrameOut& out, bo
     out.put_samples();
 }
 
+// What enqueueing a device-decided kd map update changes in the host mirror of the map.  The mirror goes back to the
+// state before it at once -- ICP launches of a second round still search the frame's map -- and takes the state after
+// it once the result shows the update's gate open (with it closed, the device left the map as it was).
+struct KdMirror {
+    int cur;
+    int64_t count, indexed;
+    bool valid, bbox_clean;
+    uint32_t gen, prev_gen;
+    const void* sorted;
+    explicit KdMirror(const pls_context* ctx)
+        : cur(ctx->kd.cur), count(ctx->kd.count), indexed(ctx->kd.indexed), valid(ctx->kd.valid),
+          bbox_clean(ctx->kd.bbox_clean), gen(ctx->kd.gen), prev_gen(ctx->kd.prev_gen), sorted(ctx->kd.sorted.p) {}
+    void restore(pls_context* ctx) const {
+        KdMap& kd = ctx->kd;
+        kd.cur = cur;
+        kd.count = count;
+        kd.indexed = indexed;
+        kd.valid = valid;
+        kd.bbox_clean = bbox_clean;
+        kd.gen = gen;
+        kd.prev_gen = prev_gen;
+        if (kd.sorted.p != sorted) std::swap(kd.sorted, kd.sorted_prev);
+    }
+};
+
+// The frame's kd map update, decided on the device behind the ICP launches enqueued so far and enqueued on the map
+// stream right away, so that its launches leave the host's path between this frame's ICP and the next frame.  Leaves
+// the host mirror of the map as the update's launches advanced it (see KdMirror); the counts are settled from the
+// result copy (kdmap_settle_device_update).
+void enqueue_device_map_update(pls_context* ctx, const FrameIn& in) {
+    KdMap& kd = ctx->kd;
+    const int64_t bound = kdmap_device_update_bound(ctx, in.pts_bound);
+    // the evicted frame's points if this frame is inserted (kdmap_update_packed's deque, one frame ahead)
+    const int64_t evict =
+        (int64_t)kd.frame_counts.size() + 1 > ctx->cfg.local_map_size ? kd.frame_counts.front() : 0;
+    Pose16 delta;
+    memcpy(delta.m, ctx->delta_since_update, sizeof(delta.m));
+    map_stream_wait(ctx);  // an earlier update of this frame (closed gate) still reads the words rewritten here
+    kd_update_decision_kernel<<<1, 1, 0, ctx->stream>>>(frame_result_dev(ctx), kd_update_words_dev(ctx), delta,
+                                                         ctx->cfg.threshold_trans, ctx->cfg.threshold_rot,
+                                                         ctx->cfg.max_num_alignments, (uint32_t)kd.count, (uint32_t)evict,
+                                                         (uint32_t)bound, in.n_dev ? scalar_u32(ctx, SC_GS_OVERFLOW) : nullptr, ctx->gs_seq);
+    PLS_CHECK_LAUNCH();
+    if (!ctx->ev_icp_done) PLS_CUDA(cudaEventCreateWithFlags(&ctx->ev_icp_done, cudaEventDisableTiming));
+    PLS_CUDA(cudaEventRecord(ctx->ev_icp_done, ctx->stream_main));
+    PLS_CUDA(cudaStreamWaitEvent(ctx->stream_map, ctx->ev_icp_done, 0));
+    map_stream_begin(ctx);
+    try {
+        kdmap_update_on_device(ctx, ctx->frame_pts_buf[ctx->frame_slot].as<float4>(), bound, kd_update_words_dev(ctx));
+    } catch (...) {
+        map_stream_end(ctx);
+        throw;
+    }
+    map_stream_end(ctx);
+}
+
 // One frame, enqueued in one go; the host waits once, for its result.  n_dev: see frame_input -- here it is the count of a
 // grid sample enqueued on compact keys, whose overflow stamp comes back with the result: if the keys overflowed, the
 // frame ran on a wrong sample, nothing is reported or advanced past the input stage, and false is returned for the
 // caller to roll back and replay.
+// On a kd map after its first insertion, on one GPU, the frame's map update is decided on the device and enqueued before
+// the host waits (enqueue_device_map_update); a frame that needs a second round of ICP launches enqueues it again behind
+// them.  Otherwise -- and when the new map count would exceed the capacity planned so far -- the update is decided by
+// the host after the wait and enqueued by the next call (flush_map_update).
 bool process_frame_device(pls_context* ctx, const void* data_void, int layout, int64_t n, const uint32_t* n_dev,
                           const float* init_pose, FrameOut out) {
-    g_trace.start();
+    g_trace.frame_start();
     FrameIn in;
     if (!frame_input(ctx, data_void, layout, n, n_dev, init_pose, in, out)) return true;
-    int icp_blocks = run_icp(ctx, in.query_bound, in.n_dev);
-    fetch_result(ctx);
+    const bool device_update = ctx->cfg.local_map_type == PLS_MAP_KDTREE && comm_size(ctx) == 1 &&
+                               kdmap_device_update_bound(ctx, in.pts_bound) > 0;
+    const KdMirror before(ctx);
+    std::optional<KdMirror> after;
+    std::function<void()> update;
+    if (device_update)
+        update = [&] {
+            enqueue_device_map_update(ctx, in);
+            after.emplace(ctx);
+            before.restore(ctx);
+        };
+    int extra_rounds = 0;
+    int icp_blocks = run_icp(ctx, in.query_bound, in.n_dev, update, &extra_rounds);
     g_trace.lap(1);
+    // a closed gate: the device left the map as it was.  An overflowed sample is replayed and a failed ICP reported
+    // below; a map grown beyond the planned capacity is updated by the host's path (frame_epilogue, flush_map_update)
+    const KdUpdateWords* upd = device_update && kd_update_words_host(ctx)->gate ? kd_update_words_host(ctx) : nullptr;
+    if (upd) after->restore(ctx);
     if (in.n_dev) {
         bool overflowed = false;
         const int64_t rows = grid_sample_host_count(ctx, &overflowed);
@@ -778,7 +965,7 @@ bool process_frame_device(pls_context* ctx, const void* data_void, int layout, i
     }
     ctx->icp_result = true;
     credit_icp_profile(ctx, frame_result_host(ctx), icp_blocks);
-    frame_epilogue(ctx, in, out, true);
+    frame_epilogue(ctx, in, out, true, upd);
     g_trace.lap(3);
     g_trace.end_frame();
     return true;
@@ -926,8 +1113,8 @@ int pls_register_frame(pls_context* ctx, const float* points, int64_t n, const f
         T0_dev = ctx->tmp[6].as<float>();
     }
     frame_begin(ctx, nullptr, T0_dev, false);
-    const int icp_blocks = run_icp(ctx, n, nullptr);
-    fetch_result(ctx);
+    int extra_rounds = 0;
+    const int icp_blocks = run_icp(ctx, n, nullptr, nullptr, &extra_rounds);
     ctx->icp_result = true;
     FrameResult* h = frame_result_host(ctx);
     credit_icp_profile(ctx, h, icp_blocks);
@@ -1036,9 +1223,12 @@ int pls_process_frame(pls_context* ctx, const void* data, int layout, int64_t n,
 int pls_process_frame_grid_sample(pls_context* ctx, const float* raw_points, int64_t n, double voxel, int layout,
                                   const float* init_pose, float* out_pose, float* out_params, int* out_has_pose,
                                   double* out_info) {
-    // (the pending map update is enqueued first here: with no host gap between the frames the next ICP would
-    // otherwise wait for an index build that started a subsample's worth of launches later)
+    // (a map update still pending -- one the host decided -- is enqueued first here: with no host gap between the frames
+    // the next ICP would otherwise wait for an index build that started a subsample's worth of launches later; an update
+    // the device decided was enqueued with the last frame)
+    g_trace.begin_call();
     PLS_API_BEGIN(ctx)
+    g_trace.lap(4);
     PLS_REQUIRE(raw_points && n > 0 && voxel > 0.0, "pls_process_frame_grid_sample: bad arguments");
     if (const char* why = frame_refusal(ctx, layout, n, voxel)) throw pls::Error{PLS_E_INVALID, why};
     const void* d = to_device(ctx, raw_points, (size_t)n * 3 * sizeof(float), ctx->stage_in[0]);
@@ -1054,7 +1244,8 @@ int pls_process_frame_grid_sample(pls_context* ctx, const float* raw_points, int
         grid_sample_enqueue(ctx, g, false);
         if (process_frame_device(ctx, ctx->gs_out_xyz.p, layout, n, scalar_u32(ctx, SC_GS_COUNT), init_pose, out)) return PLS_OK;
         // a hash overflowed the compact sort keys: the frame ran on a wrong sample and is run again from its entry state
-        // on the raw keys (this frame's map update is not enqueued yet; the cached normals stay valid for the index)
+        // on the raw keys (this frame's map update did nothing: its gate stayed closed; the cached normals stay valid for
+        // the index)
         entry.restore(ctx);
     } else {
         grid_sample_enqueue(ctx, g);
@@ -1228,7 +1419,7 @@ int pls_process_frames(pls_context* const* ctxs, int num, const void* const* dat
             const int i = icp_seq[j];
             cur = i;
             try {
-                frame_epilogue(icp[j], in[i], outputs(i), false);
+                frame_epilogue(icp[j], in[i], outputs(i), false, nullptr);
             } catch (const pls::Error& e) {
                 if (e.code != PLS_E_SINGULAR) throw;
                 icp[j]->err = e.msg;

@@ -31,14 +31,15 @@ __device__ __forceinline__ void st_volatile_u32(uint32_t* p, uint32_t v) {
 
 // Digit histograms of all passes in one read of the keys; the block that finishes last turns them into
 // exclusive bin offsets (one launch instead of histogram + scan).  Also clears the look-back words and tile counters
-// of the passes that follow (status_words of them).
+// of the passes that follow (status_words of them).  n_dev (nullable): the key count on the device, n a bound of it.
 __global__ void __launch_bounds__(256) sort_hist_kernel(const uint64_t* __restrict__ keys, int64_t n,
                                                         int num_passes, uint32_t* __restrict__ hist,
                                                         uint32_t* __restrict__ done_counter, uint32_t* __restrict__ status,
-                                                        int64_t status_words) {
+                                                        int64_t status_words, const uint32_t* __restrict__ n_dev) {
     __shared__ uint32_t sh[8 * RADIX];
     __shared__ int s_last;
     pls_grid_dependency_wait();
+    if (n_dev) n = *n_dev;
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < status_words; i += (int64_t)gridDim.x * blockDim.x)
         status[i] = 0u;
     for (int i = threadIdx.x; i < num_passes * RADIX; i += blockDim.x) sh[i] = 0;
@@ -74,10 +75,13 @@ __global__ void __launch_bounds__(256) sort_hist_kernel(const uint64_t* __restri
     }
 }
 
+// n_dev (nullable): the key count on the device, n a bound of it (the grid is sized for n).  Tiles are cut from 0 as
+// for a host count; a tile past the count exits before it publishes a look-back word, and since tiles take their
+// numbers in launch order, no tile within the count ever waits for one past it.
 __global__ void __launch_bounds__(SORT_THREADS)
 sort_pass_kernel(const uint64_t* __restrict__ kin, const uint32_t* __restrict__ vin, uint64_t* __restrict__ kout,
                  uint32_t* __restrict__ vout, int64_t n, int shift, const uint32_t* __restrict__ base,
-                 uint32_t* status, uint32_t* tile_counter) {
+                 uint32_t* status, uint32_t* tile_counter, const uint32_t* __restrict__ n_dev) {
     __shared__ uint32_t warp_hist[SORT_WARPS][RADIX];
     __shared__ uint32_t tile_offset[RADIX];
     __shared__ uint32_t s_tile;
@@ -91,6 +95,10 @@ sort_pass_kernel(const uint64_t* __restrict__ kin, const uint32_t* __restrict__ 
     for (int i = tid; i < SORT_WARPS * RADIX; i += SORT_THREADS) (&warp_hist[0][0])[i] = 0;
     __syncthreads();
     const uint32_t tile = s_tile;
+    if (n_dev) {
+        n = *n_dev;
+        if ((int64_t)tile * SORT_TILE >= n) return;  // block-uniform
+    }
     const int64_t seg = (int64_t)tile * SORT_TILE + (int64_t)warp * (32 * SORT_ITEMS);
     const uint32_t lt_mask = (1u << lane) - 1u;
 
@@ -279,7 +287,7 @@ scan_flags_kernel(const uint8_t* __restrict__ flags, int64_t n, uint32_t* __rest
 }  // namespace
 
 void radix_sort_pairs(pls_context* ctx, uint64_t* keys, uint32_t* vals, int64_t n, int num_passes,
-                      uint64_t** keys_out, uint32_t** vals_out, int64_t cap_n) {
+                      uint64_t** keys_out, uint32_t** vals_out, int64_t cap_n, const uint32_t* n_dev) {
     PLS_REQUIRE(num_passes >= 1 && num_passes <= 8, "radix_sort_pairs: 1..8 passes");
     PLS_REQUIRE(n < (1ll << 30), "radix_sort_pairs: n must be < 2^30");
     SortScratch& s = ctx->sort;
@@ -303,7 +311,7 @@ void radix_sort_pairs(pls_context* ctx, uint64_t* keys, uint32_t* vals, int64_t 
     int hist_blocks = (int)((n + 256 * 4 - 1) / (256 * 4));
     if (hist_blocks > kNumSMs) hist_blocks = kNumSMs;
     launch_dependent(sort_hist_kernel, hist_blocks, 256, st, keys, n, num_passes, s.hist.as<uint32_t>(),
-                     s.hist.as<uint32_t>() + 8 * RADIX, s.status.as<uint32_t>(), (int64_t)status_words);
+                     s.hist.as<uint32_t>() + 8 * RADIX, s.status.as<uint32_t>(), (int64_t)status_words, n_dev);
     uint64_t* kin = keys;
     uint32_t* vin = vals;
     uint64_t* kout = s.keys_alt.as<uint64_t>();
@@ -311,7 +319,8 @@ void radix_sort_pairs(pls_context* ctx, uint64_t* keys, uint32_t* vals, int64_t 
     uint32_t* counters = s.status.as<uint32_t>() + (size_t)num_passes * tiles * RADIX;
     for (int p = 0; p < num_passes; ++p) {
         launch_dependent(sort_pass_kernel, (unsigned)tiles, SORT_THREADS, st, kin, vin, kout, vout, n, 8 * p,
-                         s.hist.as<uint32_t>() + p * RADIX, s.status.as<uint32_t>() + (size_t)p * tiles * RADIX, counters + p);
+                         s.hist.as<uint32_t>() + p * RADIX, s.status.as<uint32_t>() + (size_t)p * tiles * RADIX, counters + p,
+                         n_dev);
         uint64_t* tk = kin; kin = kout; kout = tk;
         uint32_t* tv = vin; vin = vout; vout = tv;
     }
