@@ -234,6 +234,36 @@ PLS_API int pls_kdmap_set_points(pls_context* ctx, const void* xyz, int is_f64, 
 /* The point counts of the frames the kd map holds, oldest first: *out_num frames (at most local_map_size), out_counts
  * [local_map_size] or NULL.  Rows of the map before the first counted frame are a cloud set by pls_kdmap_set_points. */
 PLS_API int pls_kdmap_frames(pls_context* ctx, int64_t* out_counts, int* out_num);
+/* Correlative pose search on the kd map ctx holds (no reference counterpart: finding a scan's pose on a prior map
+ * without an initial estimate, at start-up or after odometry is lost).  Scores every pose of a dense (base, x, y) grid
+ * by how many scan points land in occupied map cells, and returns the best local maxima for an ICP to refine.
+ * scan [n,3] float32, host or device; rows with a non-finite coordinate are dropped, the valid rows are the multiset P.
+ * Occupancy O: the cells (rint(x/c), rint(y/c), rint(z/c)) of the map's current points, c = cell -- pls_voxel_hash's
+ * coordinates: float64 true division of the float32 value, round half to even.
+ * bases [A,16] row-major float64 (host or device), base a = (R_a, t_a).  The base cell of p is rint(q / c) per axis,
+ * with q_x = ((R00*x + R01*y) + R02*z) + t_x (likewise y, z), every product, sum and the division a separately rounded
+ * float64 operation (no fused multiply-add).
+ * score(a, i, j) = #{p in P : cell_a(p) + (i, j, 0) in O}, i in [-half_x, half_x], j in [-half_y, half_y].
+ * out_scores [A, 2*half_y+1, 2*half_x+1] int32 (nullable): every score, at L = (a*(2*half_y+1) + j+half_y)*(2*half_x+1)
+ * + i+half_x.  A pose's key is (score descending, L ascending).  A candidate has score > 0 and a key strictly better than
+ * every existing neighbour in its 3x3x3 block (a+-1 without wrap-around, i+-1, j+-1, clipped to the volume).
+ * *out_num = min(K, candidates); the candidates in key order: out_score [K] their scores, out_index [K] their L, out_T
+ * [K,16] float64 bases[a] with t_x += i*c and t_y += j*c.  K == 0 only fills out_scores (half_x = half_y = 0 then
+ * scores A arbitrary poses).  Outputs host or device.  A scan without a valid row gives all-zero scores, *out_num = 0.
+ * Touches neither the map, its index, its normal cache nor any ICP state.  The map is the whole kd map on every rank of
+ * a communicator.  PLS_E_INVALID, the context unchanged, for a projective map, a map that has had no update, a NULL scan
+ * or bases, n <= 0, A <= 0, half_x or half_y < 0, K outside [0, PLS_POSE_SEARCH_MAX_K], a cell that is not finite and
+ * > 0, a non-finite base, A*(2*half_x+1)*(2*half_y+1) >= 2^31, or an occupancy bit grid -- the range of the base cells
+ * widened by half_x and half_y, x rows padded to whole 32-bit words -- of more than PLS_POSE_SEARCH_MAX_BITS bits (256 MiB; the
+ * extent is in pls_last_error) or beyond +-2^40 cells. */
+#define PLS_POSE_SEARCH_MAX_BITS (1ll << 31)
+enum { PLS_POSE_SEARCH_MAX_K = 1024 };
+PLS_API int pls_kdmap_pose_search(pls_context* ctx, const float* scan, int64_t n,
+                                  const double* bases /* [A,16] row-major float64 */, int A,
+                                  double cell, int half_x, int half_y, int K,
+                                  int32_t* out_scores /* [A, 2*half_y+1, 2*half_x+1] or NULL */,
+                                  double* out_T /* [K,16] */, int32_t* out_score /* [K] */,
+                                  int64_t* out_index /* [K] */, int* out_num);
 /* ProjectiveLocalMap.update (local_map.py:126-202): rel_pose [16]; vertex_map [3,H,W] or NULL. */
 PLS_API int pls_projmap_update(pls_context* ctx, const float* rel_pose, const float* vertex_map);
 PLS_API int pls_projmap_num_frames(pls_context* ctx, int* num_frames);

@@ -31,9 +31,9 @@ __global__ void voxel_hash_kernel(const T* __restrict__ xyz, int64_t n, double v
     if (voxel_z < 0.0) voxel_z = voxel;
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
         double x = (double)xyz[3 * i], y = (double)xyz[3 * i + 1], z = (double)xyz[3 * i + 2];
-        long long cx = __double2ll_rn(x / voxel);
-        long long cy = __double2ll_rn(y / voxel_y);
-        long long cz = __double2ll_rn(z / voxel_z);
+        long long cx = voxel_coord(x, voxel);
+        long long cy = voxel_coord(y, voxel_y);
+        long long cz = voxel_coord(z, voxel_z);
         // modulo 2^64 like numba's int64 arithmetic: signed overflow would be undefined behaviour
         const long long h = (long long)((uint64_t)HX * (uint64_t)cx + (uint64_t)HY * (uint64_t)cy + (uint64_t)HZ * (uint64_t)cz);
         if (coords) {

@@ -397,6 +397,9 @@ __device__ __forceinline__ int float_to_ordered(float f) {
 __device__ __forceinline__ float ordered_to_float(int i) {
     return __int_as_float(i >= 0 ? i : i ^ 0x7fffffff);
 }
+// voxelise's coordinate rule (slam/common/pointcloud.py:13-23): int64(round_half_even(v / voxel)), true float64
+// division.  The voxel hash and the pose search's occupancy both use it, so a cell means the same in both.
+__device__ __forceinline__ long long voxel_coord(double v, double voxel) { return __double2ll_rn(v / voxel); }
 #endif
 
 // ---- module entry points used across translation units -----------------------------------------

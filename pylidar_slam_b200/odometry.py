@@ -138,6 +138,73 @@ def _check_given_normals(ctx):
         raise IndexError(_NORMALS_INDEX_ERROR)
 
 
+def _pose_search(ctx, scan, poses, cell_size, half_x, half_y, num_candidates, out_scores=None):
+    """pls_kdmap_pose_search on ctx's kd map: scan [n,3] (numpy or torch, host or CUDA), poses [A,4,4] (float64).
+    Returns (T [k,4,4] float64, scores [k] int32, index [k] int64)."""
+    check_tensor(scan, [-1, 3])
+    pts = _f32c(scan)
+    if isinstance(poses, torch.Tensor):
+        poses = poses.detach().cpu().numpy()
+    check_tensor(poses, [-1, 4, 4])
+    bases = np.ascontiguousarray(poses, dtype=np.float64)
+    K = int(num_candidates)
+    T, score = np.zeros((K, 4, 4), np.float64), np.zeros(K, np.int32)
+    index, num = np.zeros(K, np.int64), C.c_int(0)
+    ctx.call("pls_kdmap_pose_search", _lib.ptr(pts), pts.shape[0], _lib.ptr(bases), bases.shape[0], float(cell_size),
+             int(half_x), int(half_y), K, _lib.ptr(out_scores), _lib.ptr(T), _lib.ptr(score), _lib.ptr(index),
+             C.byref(num))
+    k = num.value
+    return T[:k], score[:k], index[:k]
+
+
+def _score_poses(ctx, scan, poses, cell_size) -> np.ndarray:
+    """The [A] int32 scores of exactly these poses: pls_kdmap_pose_search with a 1x1 window and no candidates."""
+    if isinstance(poses, torch.Tensor):
+        poses = poses.detach().cpu().numpy()
+    check_tensor(poses, [-1, 4, 4])
+    scores = np.zeros(poses.shape[0], np.int32)
+    _pose_search(ctx, scan, poses, cell_size, 0, 0, 0, out_scores=scores)
+    return scores
+
+
+def yaw_sweep(prior_pose, yaw_range: float = np.pi, yaw_step: float = np.deg2rad(5)) -> np.ndarray:
+    """The base poses of ICPFrameToModel.localize [A,4,4] float64: the prior turned by theta_a about the map's z axis
+    through the prior's own position (its roll, pitch, z and xy stay).  yaw_range >= pi: the full circle,
+    theta_a = 2 pi a / A with A = ceil(2 pi / yaw_step); otherwise theta_a = (a - m) yaw_step, a = 0..2m,
+    m = floor(yaw_range / yaw_step)."""
+    if isinstance(prior_pose, torch.Tensor):
+        prior_pose = prior_pose.detach().cpu().numpy()
+    prior = np.asarray(prior_pose, dtype=np.float64).reshape(4, 4)
+    assert_debug(yaw_step > 0 and np.isfinite(yaw_step), "yaw_step must be finite and > 0")
+    assert_debug(yaw_range >= 0, "yaw_range must be >= 0")
+    if yaw_range >= np.pi:
+        A = int(np.ceil(2 * np.pi / yaw_step))
+        theta = 2 * np.pi * np.arange(A) / A
+    else:
+        m = int(np.floor(yaw_range / yaw_step))
+        theta = (np.arange(2 * m + 1) - m) * yaw_step
+    c, s = np.cos(theta), np.sin(theta)
+    Rz = np.zeros((theta.shape[0], 3, 3))
+    Rz[:, 0, 0], Rz[:, 0, 1], Rz[:, 1, 0], Rz[:, 1, 1], Rz[:, 2, 2] = c, -s, s, c, 1.0
+    bases = np.tile(prior, (theta.shape[0], 1, 1))
+    bases[:, :3, :3] = Rz @ prior[:3, :3]
+    return bases
+
+
+@dataclass
+class PoseCandidate:
+    """One result of ICPFrameToModel.localize: the refined pose and its score, the search's pose and score it started
+    from, its rank in the search, and the refinement's iterations and status (PLS_OK, PLS_W_TINY_RESIDUAL or
+    PLS_E_SINGULAR)."""
+    T: np.ndarray
+    score: int
+    T0: np.ndarray
+    coarse_score: int
+    coarse_rank: int
+    iterations: int
+    status: int
+
+
 class KdTreeLocalMap(LocalMap):
     """KdTreeLocalMap (local_map.py:254-427) on the GPU: exact 1-NN over the hashed cell pyramid + lazily cached 10-NN normals.
 
@@ -173,6 +240,19 @@ class KdTreeLocalMap(LocalMap):
             if not isinstance(normals, np.ndarray):
                 raise TypeError(f"{type(normals).__module__}.{type(normals).__name__} is not an instance of numpy.ndarray")
             _set_given_normals(self.ctx, True)
+
+    def search_poses(self, scan, base_poses, cell_size: float, half_extent=(0, 0), num_candidates: int = 8):
+        """Correlative pose search (pls_kdmap_pose_search; no reference counterpart): scores every pose base_poses[a]
+        moved by whole cells (i, j) along the map's x and y, |i| <= half_extent[0], |j| <= half_extent[1], by how many
+        valid scan points land in map cells of size cell_size, and returns the best local maxima in the (a, i, j)
+        volume, best first: (T [k,4,4] float64, scores [k] int32, index [k] int64 into the volume).  scan [n,3] is
+        numpy or torch, host or CUDA; base_poses [A,4,4].  The map is left unchanged."""
+        hx, hy = half_extent
+        return _pose_search(self.ctx, scan, base_poses, cell_size, hx, hy, num_candidates)
+
+    def score_poses(self, scan, poses, cell_size: float) -> np.ndarray:
+        """The [A] int32 scores of exactly these poses [A,4,4] (search_poses' score, without shifts)."""
+        return _score_poses(self.ctx, scan, poses, cell_size)
 
     def frame_counts(self) -> list:
         """The point counts of the frames the map holds, oldest first (rows before them are a set cloud)."""
@@ -833,6 +913,35 @@ class ICPFrameToModel(OdometryAlgorithm):
             logging.error(f"Invalid Jacobian in Gauss Newton minimization, the hessian is not invertible "
                           f"(hypotheses {singular.tolist()})")
         return params, T, [list(losses[b, :iters[b]]) for b in range(B)], iters
+
+    def localize(self, scan, prior_pose, radius: float, cell_size: float, yaw_range: float = np.pi,
+                 yaw_step: float = np.deg2rad(5), num_candidates: int = 8):
+        """Finds the pose of `scan` [n,3] on the kd map this odometry's context holds (e.g. loaded with
+        KdTreeLocalMap(ctx=self.ctx).set_map_pointcloud) from a coarse prior: start-up on a stored map, recovery after
+        odometry is lost.  No reference counterpart.
+        1. bases = yaw_sweep(prior_pose, yaw_range, yaw_step);
+        2. a correlative search of those bases moved by up to ceil(radius / cell_size) cells along x and y
+           (KdTreeLocalMap.search_poses) keeps num_candidates local maxima;
+        3. one register_new_frame_hypotheses call refines them from their float32-rounded poses;
+        4. score_poses rescores the refined poses.
+        Returns every candidate as a PoseCandidate, ordered by status (singular last), then refined score
+        (descending), then search rank.  Needs what register_new_frame_hypotheses needs; IndexError while the map
+        carries given normals."""
+        _check_given_normals(self.ctx)
+        assert_debug(np.isfinite(radius) and radius >= 0, "radius must be finite and >= 0")
+        assert_debug(np.isfinite(cell_size) and cell_size > 0, "cell_size must be finite and > 0")
+        bases = yaw_sweep(prior_pose, yaw_range, yaw_step)
+        half = int(np.ceil(radius / cell_size))
+        T0, coarse, _ = _pose_search(self.ctx, scan, bases, cell_size, half, half, num_candidates)
+        if T0.shape[0] == 0:
+            return []
+        _, T, _, iters = self.register_new_frame_hypotheses(scan, T0.astype(np.float32))
+        status = self.last_hypotheses_status
+        scores = _score_poses(self.ctx, scan, T.astype(np.float64), cell_size)
+        singular = status == _lib.PLS_E_SINGULAR
+        order = np.lexsort((np.arange(T.shape[0]), -scores.astype(np.int64), singular))
+        return [PoseCandidate(T=T[r].astype(np.float64), score=int(scores[r]), T0=T0[r], coarse_score=int(coarse[r]),
+                              coarse_rank=int(r), iterations=int(iters[r]), status=int(status[r])) for r in order]
 
     def register_new_frames(self, scans, initial_estimates, scan_indices=None):
         """register_new_frame for many scans against the one map this odometry's context holds, in one call
