@@ -264,6 +264,38 @@ PLS_API int pls_kdmap_pose_search(pls_context* ctx, const float* scan, int64_t n
                                   int32_t* out_scores /* [A, 2*half_y+1, 2*half_x+1] or NULL */,
                                   double* out_T /* [K,16] */, int32_t* out_score /* [K] */,
                                   int64_t* out_index /* [K] */, int* out_num);
+/* The candidates of pls_kdmap_pose_search found by branch and bound instead of scoring every pose: for windows up to
+ * the whole map, where scoring every pose would take seconds.  For any call pls_kdmap_pose_search accepts with
+ * out_scores == NULL and K >= 1, the same out_T, out_score, out_index and *out_num, bit for bit: the scores, the cell
+ * rule, the key, the 3x3x3 candidate rule and T are the ones defined there.  L is int64.
+ * Method (exact): B_0 is the occupancy bit grid over the reachable box (the base cells' box widened by the window)
+ * clipped to the map's own cell box -- no map cell lies outside it, so a lookup outside reads 0 -- and B_k(X, Y, Z) is
+ * the OR of B_(k-1) at (X, Y), (X + 2^(k-1), Y), (X, Y + 2^(k-1)), (X + 2^(k-1), Y + 2^(k-1)).  A node (a, I, J, k)
+ * covers the shifts i + half_x in [I 2^k, (I+1) 2^k), j likewise; its bound #{p : B_k(cell_a(p) - (half_x, half_y, 0)
+ * + (I 2^k, J 2^k)) set} is >= the score of each pose under it.  A pass with threshold tau expands every node whose
+ * bound is >= tau down to level 0 and keeps E_tau, the poses scoring >= tau; a pose of E_tau is a candidate iff no
+ * neighbour in E_tau has a better key.  If K candidates score >= tau, or tau == 1, the first K in key order are the
+ * answer; otherwise tau drops to max(1, min(tau - 1, floor(3 tau / 4))).  The first tau is the largest root bound,
+ * which no score exceeds.  Roots are at the least level kmax with at most 16 x 16 roots per base.
+ * Inputs and outputs host or device, as pls_kdmap_pose_search.  A scan without a valid row, or no map cell in the
+ * reachable box, gives *out_num = 0.  Touches neither the map, its index, its normal cache nor any ICP state.
+ * PLS_E_INVALID, the context unchanged, for every refusal of pls_kdmap_pose_search except its volume and bit limits,
+ * and K < 1, out_T, out_score or out_index NULL, half_x or half_y >= 2^30, or A*(2*half_x+1)*(2*half_y+1) >= 2^62;
+ * or when the kmax + 1 levels of the clipped grid (x rows padded to whole 32-bit words) exceed
+ * PLS_POSE_SEARCH_PYRAMID_MAX_BITS bits (8 GiB, a tenth of an 80 GB H100; the extent is in pls_last_error), or
+ * when the cell of every (base, scan row), 24 bytes each and computed once for all levels, would take more than
+ * PLS_POSE_SEARCH_PYRAMID_MAX_CELL_BYTES (8 GiB: n * A < 2^33 / 24, e.g. 2 730 bases of a 131 072-row scan).  Also
+ * PLS_E_INVALID, after work was enqueued but with the context unchanged, when more than
+ * PLS_POSE_SEARCH_PYRAMID_MAX_NODES nodes survive at one level of one pass (the level and count are in
+ * pls_last_error): a map where most poses of the window score alike, or fewer than K candidates in a large volume. */
+#define PLS_POSE_SEARCH_PYRAMID_MAX_BITS (1ll << 36)
+#define PLS_POSE_SEARCH_PYRAMID_MAX_CELL_BYTES (1ll << 33)
+#define PLS_POSE_SEARCH_PYRAMID_MAX_NODES (1ll << 26)
+PLS_API int pls_kdmap_pose_search_pyramid(pls_context* ctx, const float* scan, int64_t n,
+                                          const double* bases /* [A,16] row-major float64 */, int A, double cell,
+                                          int half_x, int half_y, int K /* >= 1 */,
+                                          double* out_T /* [K,16] */, int32_t* out_score /* [K] */,
+                                          int64_t* out_index /* [K] */, int* out_num);
 /* ProjectiveLocalMap.update (local_map.py:126-202): rel_pose [16]; vertex_map [3,H,W] or NULL. */
 PLS_API int pls_projmap_update(pls_context* ctx, const float* rel_pose, const float* vertex_map);
 PLS_API int pls_projmap_num_frames(pls_context* ctx, int* num_frames);

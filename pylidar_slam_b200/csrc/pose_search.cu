@@ -1,4 +1,5 @@
-// Correlative pose search on the kd map (no reference counterpart): pls_kdmap_pose_search.
+// Correlative pose search on the kd map (no reference counterpart): pls_kdmap_pose_search, which scores every pose,
+// and pls_kdmap_pose_search_pyramid, which finds the same candidates by branch and bound (kernels further down).
 //
 //   ps_box_kernel    : the base cell of every (base, valid scan row), float64 with explicit roundings, reduced to the
 //                      min / max cell with 64-bit atomicMin / atomicMax (order-independent).  The host reads the box.
@@ -184,6 +185,214 @@ __global__ void ps_compact_kernel(const int32_t* __restrict__ s, const uint8_t* 
     }
 }
 
+// ---- pls_kdmap_pose_search_pyramid: the same candidates by branch and bound over max-pooled bit grids --------------
+//
+// A node (a, I, J) at level k covers the shifts ii in [I 2^k, (I+1) 2^k), jj likewise, of base a (ii = i + half_x).
+// Level k's grid B_k(X, Y, Z) is the OR of level 0 over [X, X + 2^k) x [Y, Y + 2^k), so #{p : B_k(cell_a(p) - half +
+// (I 2^k, J 2^k)) set} bounds the score of every pose under the node.  Work lists hold int4 (a, I, J, bound), sorted
+// by a: roots are made a-major and expansion keeps the parents' order.
+constexpr int PY_THREADS = 256;
+constexpr int PY_CHUNK = 512;  // staged cells per pass (24 B each)
+
+// A (base, row)'s cell relative to the clipped grid at shift (-half_x, -half_y): x, y; row = Z * e[1], or -1 when Z
+// lies outside the grid (the row then scores 0 at every shift) or the scan row is not finite.
+struct PyCell {
+    long long x, y, row;
+};
+
+// box[0..2] = min map cell, box[3..5] = max (pls_voxel_hash's coordinates; initialised to LLONG_MAX / LLONG_MIN)
+__global__ void __launch_bounds__(PS_THREADS) ps_map_box_kernel(const float4* __restrict__ pts, int64_t m, double c,
+                                                                long long* __restrict__ box) {
+    long long lo[3] = {LLONG_MAX, LLONG_MAX, LLONG_MAX}, hi[3] = {LLONG_MIN, LLONG_MIN, LLONG_MIN};
+    for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < m; k += (int64_t)gridDim.x * blockDim.x) {
+        const float4 p = pts[k];
+        const long long cell[3] = {voxel_coord((double)p.x, c), voxel_coord((double)p.y, c), voxel_coord((double)p.z, c)};
+#pragma unroll
+        for (int r = 0; r < 3; ++r) {
+            lo[r] = min(lo[r], cell[r]);
+            hi[r] = max(hi[r], cell[r]);
+        }
+    }
+#pragma unroll
+    for (int r = 0; r < 3; ++r) {
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            lo[r] = min(lo[r], __shfl_xor_sync(0xffffffffu, lo[r], o));
+            hi[r] = max(hi[r], __shfl_xor_sync(0xffffffffu, hi[r], o));
+        }
+    }
+    if ((threadIdx.x & 31) == 0 && lo[0] <= hi[0]) {
+#pragma unroll
+        for (int r = 0; r < 3; ++r) {
+            atomicMin(box + r, lo[r]);
+            atomicMax(box + 3 + r, hi[r]);
+        }
+    }
+}
+
+// dst = B_k from src = B_(k-1), s = 2^(k-1): each word ORs its own, its x + s bits (a funnel shift of the two words
+// s bits on), and the same two at row y + s.  Bits past the grid's edge read 0.
+__global__ void ps_pool_kernel(const uint32_t* __restrict__ src, uint32_t* __restrict__ dst, PsGrid g, long long s) {
+    const long long wx = g.wx, words = wx * g.e[1] * g.e[2];
+    const long long q = s >> 5;
+    const uint32_t r = (uint32_t)(s & 31);
+    for (long long w = (long long)blockIdx.x * blockDim.x + threadIdx.x; w < words; w += (long long)gridDim.x * blockDim.x) {
+        const long long xw = w % wx, row = w / wx, y = row % g.e[1];
+        auto pooled_x = [&](long long at) {  // the row's word xw | its bits x + s
+            const long long rb = at - xw;
+            const uint32_t lo = xw + q < wx ? src[rb + xw + q] : 0u;
+            const uint32_t hi = xw + q + 1 < wx ? src[rb + xw + q + 1] : 0u;
+            return src[at] | __funnelshift_r(lo, hi, r);
+        };
+        uint32_t v = pooled_x(w);
+        if (y + s < g.e[1]) v |= pooled_x(w + s * wx);
+        dst[w] = v;
+    }
+}
+
+// cells[a n + p] for every base and scan row, computed once for every level and pass
+__global__ void ps_pyr_cells_kernel(const float* __restrict__ scan, int64_t n, const double* __restrict__ bases, int A,
+                                    double c, PsGrid g, int half_x, int half_y, PyCell* __restrict__ cells) {
+    const int64_t total = n * (int64_t)A;
+    for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < total; k += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t a = k / n, p = k - a * n;
+        long long cx, cy, cz;
+        PyCell v = {0, 0, -1};
+        if (base_cell(bases + 16 * a, scan[3 * p], scan[3 * p + 1], scan[3 * p + 2], c, cx, cy, cz)) {
+            const long long Z = cz - g.o[2];
+            if (Z >= 0 && Z < g.e[2]) v = {cx - half_x - g.o[0], cy - half_y - g.o[1], Z * g.e[1]};
+        }
+        cells[k] = v;
+    }
+}
+
+// nodes[i].w = the node's bound at level k (its exact score at k = 0).  A block's lanes are 256 consecutive nodes;
+// for each base among them, that base's cells stream through shared memory and its lanes count in a register.
+// A block left or below the grid's edge that reaches into it reads B_k at the edge, which pools a superset: still a bound.
+__global__ void __launch_bounds__(PY_THREADS) ps_pyr_score_kernel(const PyCell* __restrict__ cells, int64_t n,
+                                                                  const uint32_t* __restrict__ bits, PsGrid g, int k,
+                                                                  int4* __restrict__ nodes, int64_t count) {
+    __shared__ PyCell staged[PY_CHUNK];
+    const int64_t first = (int64_t)blockIdx.x * PY_THREADS, i = first + threadIdx.x;
+    const int4 nd = i < count ? nodes[i] : make_int4(-1, 0, 0, 0);
+    const int a_lo = nodes[first].x, a_hi = nodes[min(first + PY_THREADS, count) - 1].x;
+    const long long span = 1ll << k, xs = (long long)nd.y << k, ys = (long long)nd.z << k;
+    const unsigned long long ex = (unsigned long long)g.e[0], ey = (unsigned long long)g.e[1];
+    int32_t ub = 0;
+    for (int a = a_lo; a <= a_hi; ++a) {
+        if (!__syncthreads_or(nd.x == a)) continue;
+        const PyCell* src = cells + (int64_t)a * n;
+        for (int64_t k0 = 0; k0 < n; k0 += PY_CHUNK) {
+            const int len = (int)min((int64_t)PY_CHUNK, n - k0);
+            __syncthreads();
+            for (int t = threadIdx.x; t < len; t += PY_THREADS) staged[t] = src[k0 + t];
+            __syncthreads();
+            if (nd.x != a) continue;
+#pragma unroll 4
+            for (int t = 0; t < len; ++t) {
+                const PyCell v = staged[t];
+                if (v.row < 0) continue;
+                long long X = v.x + xs, Y = v.y + ys;
+                if (X < 0) X = X + span > 0 ? 0 : -1;
+                if (Y < 0) Y = Y + span > 0 ? 0 : -1;
+                if ((unsigned long long)X < ex && (unsigned long long)Y < ey)
+                    ub += (int32_t)((__ldg(bits + (v.row + Y) * (long long)g.wx + (X >> 5)) >> (X & 31)) & 1u);
+            }
+        }
+    }
+    if (i < count) nodes[i].w = ub;
+}
+
+// flags[4 i + c] = 1 for child c = (dx, dy) = (c & 1, c >> 1) of node i at level k >= 1: bound >= tau and the child's
+// first shift inside the window
+__global__ void ps_pyr_branch_kernel(const int4* __restrict__ nodes, int64_t count, int k, int Wx, int Wy, int tau,
+                                     uint8_t* __restrict__ flags) {
+    for (int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; f < 4 * count; f += (int64_t)gridDim.x * blockDim.x) {
+        const int4 nd = nodes[f >> 2];
+        const long long I = 2ll * nd.y + (f & 1), J = 2ll * nd.z + ((f >> 1) & 1);
+        flags[f] = nd.w >= tau && (I << (k - 1)) < Wx && (J << (k - 1)) < Wy;
+    }
+}
+
+__global__ void ps_pyr_children_kernel(const int4* __restrict__ nodes, const uint8_t* __restrict__ flags,
+                                       const uint32_t* __restrict__ pos, int64_t count, int4* __restrict__ out) {
+    for (int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; f < 4 * count; f += (int64_t)gridDim.x * blockDim.x) {
+        if (!flags[f]) continue;
+        const int4 nd = nodes[f >> 2];
+        out[pos[f]] = make_int4(nd.x, 2 * nd.y + (int)(f & 1), 2 * nd.z + (int)((f >> 1) & 1), 0);
+    }
+}
+
+// E_tau at level 0: flags[i] = score >= tau
+__global__ void ps_pyr_keep_kernel(const int4* __restrict__ nodes, int64_t count, int tau, uint8_t* __restrict__ flags) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < count; i += (int64_t)gridDim.x * blockDim.x)
+        flags[i] = nodes[i].w >= tau;
+}
+
+__global__ void ps_pyr_exact_kernel(const int4* __restrict__ nodes, const uint8_t* __restrict__ flags,
+                                    const uint32_t* __restrict__ pos, int64_t count, int Wx, int Wy,
+                                    uint64_t* __restrict__ L, uint32_t* __restrict__ s) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < count; i += (int64_t)gridDim.x * blockDim.x) {
+        if (!flags[i]) continue;
+        const int4 nd = nodes[i];
+        L[pos[i]] = (uint64_t)(((int64_t)nd.x * Wy + nd.z) * Wx + nd.y);
+        s[pos[i]] = (uint32_t)nd.w;
+    }
+}
+
+// flags[e] = 1 for a candidate among E_tau sorted by L: no neighbour of its 3x3x3 block that is in E_tau has a better
+// key.  A neighbour outside E_tau scores below tau <= s[e], so it cannot beat it.
+__global__ void ps_pyr_peak_kernel(const uint64_t* __restrict__ L, const uint32_t* __restrict__ s, int64_t m, int A,
+                                   int Wy, int Wx, uint8_t* __restrict__ flags) {
+    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < m; e += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t Le = (int64_t)L[e];
+        const uint32_t se = s[e];
+        const int ii = (int)(Le % Wx);
+        const int64_t t = Le / Wx;
+        const int jj = (int)(t % Wy);
+        const int64_t a = t / Wy;
+        bool peak = true;
+        for (int da = -1; da <= 1 && peak; ++da) {
+            if (a + da < 0 || a + da >= A) continue;
+            for (int dj = -1; dj <= 1; ++dj) {
+                if (jj + dj < 0 || jj + dj >= Wy) continue;
+                for (int dx = -1; dx <= 1; ++dx) {
+                    if (ii + dx < 0 || ii + dx >= Wx || (da == 0 && dj == 0 && dx == 0)) continue;
+                    const uint64_t Ln = (uint64_t)(Le + ((int64_t)da * Wy + dj) * Wx + dx);
+                    int64_t lo = 0, hi = m;  // lower bound of Ln
+                    while (lo < hi) {
+                        const int64_t mid = (lo + hi) >> 1;
+                        if (L[mid] < Ln) lo = mid + 1;
+                        else hi = mid;
+                    }
+                    if (lo < m && L[lo] == Ln && (s[lo] > se || (s[lo] == se && Ln < (uint64_t)Le))) peak = false;
+                }
+            }
+        }
+        flags[e] = peak ? 1 : 0;
+    }
+}
+
+// keys[pos[e]] = (~score << 32) | e: sorted ascending, score descending, then e ascending, which is L ascending
+__global__ void ps_pyr_rank_kernel(const uint32_t* __restrict__ s, const uint8_t* __restrict__ flags,
+                                   const uint32_t* __restrict__ pos, int64_t m, uint64_t* __restrict__ keys,
+                                   uint32_t* __restrict__ vals) {
+    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < m; e += (int64_t)gridDim.x * blockDim.x) {
+        if (!flags[e]) continue;
+        keys[pos[e]] = ((uint64_t)(~s[e]) << 32) | (uint64_t)e;
+        vals[pos[e]] = (uint32_t)e;
+    }
+}
+
+// the first k candidates in key order: their L and score
+__global__ void ps_pyr_top_kernel(const uint64_t* __restrict__ keys, const uint64_t* __restrict__ L, int k,
+                                  int64_t* __restrict__ out_L, int32_t* __restrict__ out_s) {
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= k) return;
+    out_L[c] = (int64_t)L[keys[c] & 0xffffffffull];
+    out_s[c] = (int32_t)~(uint32_t)(keys[c] >> 32);
+}
+
 }  // namespace
 
 }  // namespace pls
@@ -340,6 +549,270 @@ extern "C" int pls_kdmap_pose_search(pls_context* ctx, const float* scan, int64_
     put(out_T, T.data(), T.size() * sizeof(double));
     put(out_score, sc.data(), sc.size() * sizeof(int32_t));
     put(out_index, idx.data(), idx.size() * sizeof(int64_t));
+    *out_num = k;
+    PLS_API_END(ctx)
+}
+
+namespace {
+
+constexpr int PY_ROOT_SIDE = 16;  // kmax: the least level with at most 16 x 16 roots per base
+
+// The next threshold of a pass that found fewer than K candidates: 3/4 of the last, at least one less, at least 1.
+int next_tau(int tau) { return std::max(1, std::min(tau - 1, (int)((3ll * tau) / 4))); }
+
+// Sub-arrays carved from one scratch buffer start on 256-byte boundaries, as whole allocations do.
+size_t aligned(int64_t bytes) { return ((size_t)bytes + 255) & ~(size_t)255; }
+
+// The radix passes that order L < V: whole bytes, an even count, so that the sorted keys land back in place.
+int l_passes(int64_t V) {
+    int bytes = 1;
+    while (bytes < 8 && (uint64_t)(V - 1) >> (8 * bytes)) ++bytes;
+    return std::min(8, bytes + (bytes & 1));
+}
+
+}  // namespace
+
+extern "C" int pls_kdmap_pose_search_pyramid(pls_context* ctx, const float* scan, int64_t n, const double* bases, int A,
+                                             double cell, int half_x, int half_y, int K, double* out_T,
+                                             int32_t* out_score, int64_t* out_index, int* out_num) {
+    PLS_API_BEGIN(ctx)
+    // every argument is checked before anything is enqueued: a refused call changes nothing
+    PLS_REQUIRE(ctx->cfg.local_map_type == PLS_MAP_KDTREE, "pls_kdmap_pose_search_pyramid: needs a kd-tree local map");
+    PLS_REQUIRE(ctx->kd.valid, "kd map: search before any update");
+    PLS_REQUIRE(scan && bases, "pls_kdmap_pose_search_pyramid: scan and bases must not be NULL");
+    PLS_REQUIRE(n > 0 && n <= INT32_MAX, "pls_kdmap_pose_search_pyramid: scan must be [n,3] with 0 < n < 2^31");
+    PLS_REQUIRE(A > 0, "pls_kdmap_pose_search_pyramid: bases must be [A,16] with A > 0");
+    PLS_REQUIRE(half_x >= 0 && half_y >= 0 && half_x < (1 << 30) && half_y < (1 << 30),
+                "pls_kdmap_pose_search_pyramid: half_x and half_y must lie in [0, 2^30)");
+    PLS_REQUIRE(K >= 1 && K <= PLS_POSE_SEARCH_MAX_K, "pls_kdmap_pose_search_pyramid: K must lie in [1, 1024]");
+    PLS_REQUIRE(std::isfinite(cell) && cell > 0.0, "pls_kdmap_pose_search_pyramid: cell must be finite and > 0");
+    PLS_REQUIRE(out_num && out_T && out_score && out_index,
+                "pls_kdmap_pose_search_pyramid: out_T, out_score, out_index and out_num must not be NULL");
+    const int Wx = 2 * half_x + 1, Wy = 2 * half_y + 1;
+    PLS_REQUIRE((unsigned __int128)A * (unsigned)Wx * (unsigned)Wy < ((unsigned __int128)1 << 62),
+                "pls_kdmap_pose_search_pyramid: A*(2*half_x+1)*(2*half_y+1) must be < 2^62");
+    const int64_t V = (int64_t)A * Wx * Wy;
+    if ((double)n * A * sizeof(PyCell) > (double)PLS_POSE_SEARCH_PYRAMID_MAX_CELL_BYTES) {
+        char msg[256];
+        snprintf(msg, sizeof(msg),
+                 "pls_kdmap_pose_search_pyramid: the cells of %lld rows x %d bases (%zu bytes each) exceed "
+                 "PLS_POSE_SEARCH_PYRAMID_MAX_CELL_BYTES (2^33); use fewer bases or a sparser scan",
+                 (long long)n, A, sizeof(PyCell));
+        throw pls::Error{PLS_E_INVALID, msg};
+    }
+    std::vector<double> Tb((size_t)A * 16);
+    if (is_device_ptr(bases)) PLS_CUDA(cudaMemcpy(Tb.data(), bases, Tb.size() * sizeof(double), cudaMemcpyDeviceToHost));
+    else memcpy(Tb.data(), bases, Tb.size() * sizeof(double));
+    for (double v : Tb) PLS_REQUIRE(std::isfinite(v), "pls_kdmap_pose_search_pyramid: every base must be finite");
+
+    cudaStream_t st = ctx->stream;
+    map_stream_wait(ctx);
+    // scratch of this stateless call: next_buf, never a buffer the map or an ICP keeps state in
+    DBuf* nb = ctx->next_buf;
+    const float* scan_dev = (const float*)to_device(ctx, scan, (size_t)n * 3 * sizeof(float), nb[0]);
+    const size_t tail = (size_t)A * 16 * sizeof(double) + 12 * sizeof(long long) + 8 * sizeof(uint32_t);
+    nb[1].reserve(tail + (size_t)PLS_POSE_SEARCH_MAX_K * (sizeof(int64_t) + sizeof(int32_t)), st);
+    double* bases_dev = nb[1].as<double>();
+    long long* box_dev = reinterpret_cast<long long*>(bases_dev + (size_t)A * 16);  // base box, then map box
+    uint32_t* total_dev = reinterpret_cast<uint32_t*>(box_dev + 12);
+    int64_t* top_L = reinterpret_cast<int64_t*>(nb[1].as<char>() + tail);
+    int32_t* top_s = reinterpret_cast<int32_t*>(top_L + PLS_POSE_SEARCH_MAX_K);
+    const long long box_init[12] = {LLONG_MAX, LLONG_MAX, LLONG_MAX, LLONG_MIN, LLONG_MIN, LLONG_MIN,
+                                    LLONG_MAX, LLONG_MAX, LLONG_MAX, LLONG_MIN, LLONG_MIN, LLONG_MIN};
+    PLS_CUDA(cudaMemcpyAsync(bases_dev, Tb.data(), Tb.size() * sizeof(double), cudaMemcpyHostToDevice, st));
+    PLS_CUDA(cudaMemcpyAsync(box_dev, box_init, sizeof(box_init), cudaMemcpyHostToDevice, st));
+    ps_box_kernel<<<blocks_for(n * (int64_t)A, PS_THREADS, 8 * kNumSMs), PS_THREADS, 0, st>>>(scan_dev, n, bases_dev, A,
+                                                                                              cell, box_dev);
+    PLS_CHECK_LAUNCH();
+    const int64_t M = ctx->kd.count;
+    const float4* map_pts = ctx->kd.store[ctx->kd.cur].as<float4>();
+    if (M > 0) {
+        ps_map_box_kernel<<<blocks_for(M, PS_THREADS, 8 * kNumSMs), PS_THREADS, 0, st>>>(map_pts, M, cell, box_dev + 6);
+        PLS_CHECK_LAUNCH();
+    }
+    long long box[12];
+    PLS_CUDA(cudaMemcpyAsync(box, box_dev, sizeof(box), cudaMemcpyDeviceToHost, st));
+    PLS_CUDA(cudaStreamSynchronize(st));
+    *out_num = 0;
+    if (box[0] > box[3]) return PLS_OK;  // no valid row: every score is 0, no candidate
+    for (int r = 0; r < 6; ++r)
+        PLS_REQUIRE(box[r] > -PS_MAX_CELL && box[r] < PS_MAX_CELL,
+                    "pls_kdmap_pose_search_pyramid: a base cell lies beyond +-2^40 cells of the origin");
+    // the grid: the reachable box (base cells widened by the window) clipped to the map's own cells
+    PsGrid g;
+    const long long half[3] = {half_x, half_y, 0};
+    for (int r = 0; r < 3; ++r) {
+        g.o[r] = std::max(box[r] - half[r], box[6 + r]);
+        g.e[r] = std::min(box[3 + r] + half[r], box[9 + r]) - g.o[r] + 1;
+        if (M == 0 || g.e[r] <= 0) return PLS_OK;  // no map cell is reachable: every score is 0
+    }
+    int kmax = 0;
+    while (((int64_t)std::max(Wx, Wy) + (1ll << kmax) - 1) >> kmax > PY_ROOT_SIDE) ++kmax;
+    const int levels = kmax + 1;
+    const double level_bits = 32.0 * (double)((g.e[0] + 31) / 32) * (double)g.e[1] * (double)g.e[2];
+    if (level_bits * levels > (double)PLS_POSE_SEARCH_PYRAMID_MAX_BITS) {
+        char msg[320];
+        snprintf(msg, sizeof(msg),
+                 "pls_kdmap_pose_search_pyramid: %d pooled levels of the clipped occupancy grid of %lld x %lld x %lld "
+                 "cells (%.0f bits with word-padded x rows) exceed PLS_POSE_SEARCH_PYRAMID_MAX_BITS (2^36); use a "
+                 "larger cell or a smaller window",
+                 levels, g.e[0], g.e[1], g.e[2], level_bits * levels);
+        throw pls::Error{PLS_E_INVALID, msg};
+    }
+    g.wx = (uint32_t)((g.e[0] + 31) / 32);
+    const size_t words = (size_t)g.wx * (size_t)g.e[1] * (size_t)g.e[2];
+
+    // B_0: occupancy of the map's cells inside the clipped grid; B_k pooled from B_(k-1), one launch per level
+    nb[2].reserve(words * levels * sizeof(uint32_t), st);
+    uint32_t* bits = nb[2].as<uint32_t>();
+    PLS_CUDA(cudaMemsetAsync(bits, 0, words * sizeof(uint32_t), st));
+    ps_occupy_kernel<<<blocks_for(M, 256, 16 * kNumSMs), 256, 0, st>>>(map_pts, M, cell, g, bits);
+    PLS_CHECK_LAUNCH();
+    for (int k = 1; k <= kmax; ++k) {
+        ps_pool_kernel<<<blocks_for((int64_t)words, 256, 16 * kNumSMs), 256, 0, st>>>(
+            bits + (k - 1) * words, bits + k * words, g, 1ll << (k - 1));
+        PLS_CHECK_LAUNCH();
+    }
+    nb[3].reserve((size_t)n * A * sizeof(PyCell), st);
+    PyCell* cells = nb[3].as<PyCell>();
+    ps_pyr_cells_kernel<<<blocks_for(n * (int64_t)A, 256, 16 * kNumSMs), 256, 0, st>>>(scan_dev, n, bases_dev, A, cell,
+                                                                                        g, half_x, half_y, cells);
+    PLS_CHECK_LAUNCH();
+
+    auto over_capacity = [&](int level, int64_t count) {
+        if (count <= PLS_POSE_SEARCH_PYRAMID_MAX_NODES) return;
+        char msg[256];
+        snprintf(msg, sizeof(msg),
+                 "pls_kdmap_pose_search_pyramid: %lld nodes survive at level %d, more than "
+                 "PLS_POSE_SEARCH_PYRAMID_MAX_NODES (2^26)",
+                 (long long)count, level);
+        throw pls::Error{PLS_E_INVALID, msg};
+    };
+    auto score = [&](int4* nodes, int64_t count, int k) {
+        ps_pyr_score_kernel<<<(unsigned)((count + PY_THREADS - 1) / PY_THREADS), PY_THREADS, 0, st>>>(
+            cells, n, bits + (size_t)k * words, g, k, nodes, count);
+        PLS_CHECK_LAUNCH();
+    };
+    auto read_total = [&]() {
+        uint32_t t = 0;
+        PLS_CUDA(cudaMemcpyAsync(&t, total_dev, sizeof(t), cudaMemcpyDeviceToHost, st));
+        PLS_CUDA(cudaStreamSynchronize(st));
+        return (int64_t)t;
+    };
+
+    // roots: every (a, I, J) at level kmax, a-major, scored once for every pass; their bounds come back for the first tau
+    const int rx = (int)(((int64_t)Wx + (1ll << kmax) - 1) >> kmax), ry = (int)(((int64_t)Wy + (1ll << kmax) - 1) >> kmax);
+    const int64_t R = (int64_t)A * rx * ry;
+    over_capacity(kmax, R);
+    std::vector<int4> roots((size_t)R);
+    for (int64_t r = 0; r < R; ++r)
+        roots[(size_t)r] = make_int4((int)(r / ((int64_t)rx * ry)), (int)(r % rx), (int)((r / rx) % ry), 0);
+    nb[4].reserve((size_t)R * sizeof(int4), st);
+    int4* roots_dev = nb[4].as<int4>();
+    PLS_CUDA(cudaMemcpyAsync(roots_dev, roots.data(), (size_t)R * sizeof(int4), cudaMemcpyHostToDevice, st));
+    score(roots_dev, R, kmax);
+    PLS_CUDA(cudaMemcpyAsync(roots.data(), roots_dev, (size_t)R * sizeof(int4), cudaMemcpyDeviceToHost, st));
+    PLS_CUDA(cudaStreamSynchronize(st));
+
+    DBuf* work[2] = {&nb[5], &nb[6]};
+    int top_bound = 1;
+    for (const int4& r : roots) top_bound = std::max(top_bound, r.w);
+
+    // threshold passes: tau from the largest root bound (no pose scores more) down by next_tau until K candidates
+    // score >= tau, or tau = 1.  A high tau prunes hard, so the early passes are cheap.
+    std::vector<int64_t> hL;
+    std::vector<int32_t> hs;
+    for (int tau = top_bound;; tau = next_tau(tau)) {
+        int4* cur = roots_dev;
+        int64_t count = R;
+        int wi = 0;  // the work buffer the next level goes to
+        for (int k = kmax; k > 0 && count > 0; --k) {
+            nb[7].reserve((size_t)count * 4 * (sizeof(uint32_t) + 1), st);
+            uint32_t* pos = nb[7].as<uint32_t>();
+            uint8_t* flags = reinterpret_cast<uint8_t*>(pos + (size_t)count * 4);
+            ps_pyr_branch_kernel<<<blocks_for(4 * count, 256, 16 * kNumSMs), 256, 0, st>>>(cur, count, k, Wx, Wy, tau,
+                                                                                            flags);
+            PLS_CHECK_LAUNCH();
+            exclusive_scan_flags(ctx, flags, 4 * count, pos, total_dev);
+            const int64_t next = read_total();
+            over_capacity(k - 1, next);
+            if (next > 0) {
+                work[wi]->reserve((size_t)next * sizeof(int4), st);
+                int4* out = work[wi]->as<int4>();
+                ps_pyr_children_kernel<<<blocks_for(4 * count, 256, 16 * kNumSMs), 256, 0, st>>>(cur, flags, pos, count,
+                                                                                                  out);
+                PLS_CHECK_LAUNCH();
+                score(out, next, k - 1);
+                cur = out;
+                wi ^= 1;
+            }
+            count = next;
+        }
+        int64_t num = 0;
+        if (count > 0) {
+            // E_tau, sorted by L, in the work buffer cur is not in; the candidates' keys in the other one
+            DBuf* eb = work[wi];
+            DBuf* cb = work[wi ^ 1];
+            nb[7].reserve((size_t)count * (sizeof(uint32_t) + 1), st);
+            uint32_t* pos = nb[7].as<uint32_t>();  // 4-byte words first: flags need no alignment
+            uint8_t* flags = reinterpret_cast<uint8_t*>(pos + count);
+            ps_pyr_keep_kernel<<<blocks_for(count, 256, 16 * kNumSMs), 256, 0, st>>>(cur, count, tau, flags);
+            PLS_CHECK_LAUNCH();
+            exclusive_scan_flags(ctx, flags, count, pos, total_dev);
+            const int64_t m = read_total();
+            if (m > 0) {
+                eb->reserve(aligned(m * sizeof(uint64_t)) + (size_t)m * sizeof(uint32_t), st);
+                uint64_t* L = eb->as<uint64_t>();
+                uint32_t* s = reinterpret_cast<uint32_t*>(eb->as<char>() + aligned(m * sizeof(uint64_t)));
+                ps_pyr_exact_kernel<<<blocks_for(count, 256, 16 * kNumSMs), 256, 0, st>>>(cur, flags, pos, count, Wx, Wy,
+                                                                                           L, s);
+                PLS_CHECK_LAUNCH();
+                uint64_t* ko = nullptr;
+                uint32_t* vo = nullptr;
+                radix_sort_pairs(ctx, L, s, m, l_passes(V), &ko, &vo);  // an even pass count: sorted in place
+                ps_pyr_peak_kernel<<<blocks_for(m, 256, 16 * kNumSMs), 256, 0, st>>>(L, s, m, A, Wy, Wx, flags);
+                PLS_CHECK_LAUNCH();
+                exclusive_scan_flags(ctx, flags, m, pos, total_dev);
+                num = read_total();
+                if (num > 0 && (num >= K || tau == 1)) {
+                    cb->reserve(aligned(num * sizeof(uint64_t)) + (size_t)num * sizeof(uint32_t), st);
+                    uint64_t* keys = cb->as<uint64_t>();
+                    uint32_t* vals = reinterpret_cast<uint32_t*>(cb->as<char>() + aligned(num * sizeof(uint64_t)));
+                    ps_pyr_rank_kernel<<<blocks_for(m, 256, 16 * kNumSMs), 256, 0, st>>>(s, flags, pos, m, keys, vals);
+                    PLS_CHECK_LAUNCH();
+                    radix_sort_pairs(ctx, keys, vals, num, 8, &ko, &vo);
+                    const int k = (int)std::min<int64_t>(K, num);
+                    ps_pyr_top_kernel<<<(k + 255) / 256, 256, 0, st>>>(keys, L, k, top_L, top_s);
+                    PLS_CHECK_LAUNCH();
+                    hL.resize((size_t)k);
+                    hs.resize((size_t)k);
+                    PLS_CUDA(cudaMemcpyAsync(hL.data(), top_L, k * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+                    PLS_CUDA(cudaMemcpyAsync(hs.data(), top_s, k * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+                    PLS_CUDA(cudaStreamSynchronize(st));
+                }
+            }
+        }
+        if (num >= K || tau == 1) break;
+    }
+
+    auto put = [&](void* dst, const void* src, size_t bytes) {  // host or device outputs
+        if (!bytes) return;
+        if (is_device_ptr(dst)) PLS_CUDA(cudaMemcpy(dst, src, bytes, cudaMemcpyHostToDevice));
+        else memcpy(dst, src, bytes);
+    };
+    const int k = (int)hL.size();
+    std::vector<double> T((size_t)k * 16);
+    for (int c = 0; c < k; ++c) {
+        const int64_t L = hL[(size_t)c];
+        const int i = (int)(L % Wx) - half_x, j = (int)((L / Wx) % Wy) - half_y;
+        const int64_t a = L / ((int64_t)Wx * Wy);
+        memcpy(&T[16 * (size_t)c], &Tb[16 * (size_t)a], 16 * sizeof(double));
+        T[16 * (size_t)c + 3] += (double)i * cell;
+        T[16 * (size_t)c + 7] += (double)j * cell;
+    }
+    put(out_T, T.data(), T.size() * sizeof(double));
+    put(out_score, hs.data(), hs.size() * sizeof(int32_t));
+    put(out_index, hL.data(), hL.size() * sizeof(int64_t));
     *out_num = k;
     PLS_API_END(ctx)
 }

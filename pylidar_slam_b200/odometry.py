@@ -138,9 +138,20 @@ def _check_given_normals(ctx):
         raise IndexError(_NORMALS_INDEX_ERROR)
 
 
+# Pose count A*(2*half_x+1)*(2*half_y+1) from which _pose_search takes pls_kdmap_pose_search_pyramid (branch and
+# bound) instead of scoring every pose with pls_kdmap_pose_search.  Measured on an H100 SXM at 700 W, K = 8, 72 yaws
+# (profiles/h100_pose_search_pyramid.json, DESIGN section 18): up to 30 M poses the exhaustive call is faster in all
+# but one measured case; at 46 M poses (+-200 m at 0.5 m) the pyramid is 1.6-3.7x faster on 4 of 6 map/scan pairs and
+# 4-5 % slower on 2; at 288 M and 1.15 G poses (+-1000 m on the 2 km map) it is 1.5-11.7x faster.
+POSE_SEARCH_PYRAMID_MIN_POSES = 1 << 27
+
+
 def _pose_search(ctx, scan, poses, cell_size, half_x, half_y, num_candidates, out_scores=None):
-    """pls_kdmap_pose_search on ctx's kd map: scan [n,3] (numpy or torch, host or CUDA), poses [A,4,4] (float64).
-    Returns (T [k,4,4] float64, scores [k] int32, index [k] int64)."""
+    """The correlative pose search on ctx's kd map: scan [n,3] (numpy or torch, host or CUDA), poses [A,4,4] (float64).
+    Returns (T [k,4,4] float64, scores [k] int32, index [k] int64).  Both calls return the same candidates bit for bit;
+    pls_kdmap_pose_search scores every pose and is taken for out_scores, K = 0 and fewer than
+    POSE_SEARCH_PYRAMID_MIN_POSES poses, pls_kdmap_pose_search_pyramid prunes and is taken otherwise, with the
+    exhaustive call answering any volume below 2^31 poses that the pyramid refuses."""
     check_tensor(scan, [-1, 3])
     pts = _f32c(scan)
     if isinstance(poses, torch.Tensor):
@@ -150,9 +161,21 @@ def _pose_search(ctx, scan, poses, cell_size, half_x, half_y, num_candidates, ou
     K = int(num_candidates)
     T, score = np.zeros((K, 4, 4), np.float64), np.zeros(K, np.int32)
     index, num = np.zeros(K, np.int64), C.c_int(0)
-    ctx.call("pls_kdmap_pose_search", _lib.ptr(pts), pts.shape[0], _lib.ptr(bases), bases.shape[0], float(cell_size),
-             int(half_x), int(half_y), K, _lib.ptr(out_scores), _lib.ptr(T), _lib.ptr(score), _lib.ptr(index),
-             C.byref(num))
+    args = (_lib.ptr(pts), pts.shape[0], _lib.ptr(bases), bases.shape[0], float(cell_size), int(half_x), int(half_y), K)
+    outs = (_lib.ptr(T), _lib.ptr(score), _lib.ptr(index), C.byref(num))
+    poses_in_volume = bases.shape[0] * (2 * int(half_x) + 1) * (2 * int(half_y) + 1)
+    if out_scores is not None or K < 1 or poses_in_volume < POSE_SEARCH_PYRAMID_MIN_POSES:
+        ctx.call("pls_kdmap_pose_search", *args, _lib.ptr(out_scores), *outs)
+    else:
+        try:
+            ctx.call("pls_kdmap_pose_search_pyramid", *args, *outs)
+        except AssertionError:
+            # The pyramid refuses when more nodes survive a level than its work lists hold (maps where most poses
+            # score alike) or when its per-(base, row) cells outgrow their limit.  Below 2^31 poses the exhaustive call
+            # still answers, so the volume gets the answer it always had; beyond that the refusal stands.
+            if poses_in_volume >= 1 << 31:
+                raise
+            ctx.call("pls_kdmap_pose_search", *args, None, *outs)
     k = num.value
     return T[:k], score[:k], index[:k]
 
@@ -246,7 +269,8 @@ class KdTreeLocalMap(LocalMap):
         moved by whole cells (i, j) along the map's x and y, |i| <= half_extent[0], |j| <= half_extent[1], by how many
         valid scan points land in map cells of size cell_size, and returns the best local maxima in the (a, i, j)
         volume, best first: (T [k,4,4] float64, scores [k] int32, index [k] int64 into the volume).  scan [n,3] is
-        numpy or torch, host or CUDA; base_poses [A,4,4].  The map is left unchanged."""
+        numpy or torch, host or CUDA; base_poses [A,4,4].  The map is left unchanged.  Large volumes are searched by
+        branch and bound (pls_kdmap_pose_search_pyramid) with the same result, so half_extent may span the whole map."""
         hx, hy = half_extent
         return _pose_search(self.ctx, scan, base_poses, cell_size, hx, hy, num_candidates)
 
@@ -924,6 +948,8 @@ class ICPFrameToModel(OdometryAlgorithm):
            (KdTreeLocalMap.search_poses) keeps num_candidates local maxima;
         3. one register_new_frame_hypotheses call refines them from their float32-rounded poses;
         4. score_poses rescores the refined poses.
+        The search in step 2 is exact at any radius, and a large one is searched by branch and bound, so `radius` may
+        span the whole map when the position is unknown.
         Returns every candidate as a PoseCandidate, ordered by status (singular last), then refined score
         (descending), then search rank.  Needs what register_new_frame_hypotheses needs; IndexError while the map
         carries given normals."""
