@@ -296,6 +296,24 @@ PLS_API int pls_kdmap_pose_search_pyramid(pls_context* ctx, const float* scan, i
                                           int half_x, int half_y, int K /* >= 1 */,
                                           double* out_T /* [K,16] */, int32_t* out_score /* [K] */,
                                           int64_t* out_index /* [K] */, int* out_num);
+/* pls_kdmap_pose_search for S scans in one call (a localisation server re-localising many vehicles' scans on one map,
+ * offline map matching a recorded drive's scans from their GNSS fixes).  scans[s] [n[s],3] float32, host or device;
+ * bases [sum A_s,16] row-major float64 (host or device), scan s's A_s = num_bases[s] bases after the earlier scans';
+ * one cell and one K, per-scan windows half_x[s], half_y[s].  For each scan s the outputs are, bit for bit, what
+ * pls_kdmap_pose_search(ctx, scans[s], n[s], bases of s, A_s, cell, half_x[s], half_y[s], K, ...) writes: its scores at
+ * offset sum_{r<s} V_r of out_scores [sum V_s] (nullable), V_s = A_s*(2*half_x[s]+1)*(2*half_y[s]+1); out_T [S,K,16],
+ * out_score [S,K], out_index [S,K] (L local to scan s's own volume) at row s, and out_num[s].  Entries past out_num[s]
+ * are not written.  Outputs host or device.  One occupancy grid serves every scan: the bounding box of the union of the
+ * scans' reachable boxes (each scan's base-cell box widened by its own window).  Touches neither the map, its index, its
+ * normal cache nor any ICP state.  PLS_E_INVALID, the context unchanged, for any refusal pls_kdmap_pose_search would
+ * give for some scan s (pls_last_error names s), S <= 0, a NULL array, sum V_s >= 2^31, or a shared grid of more than
+ * PLS_POSE_SEARCH_MAX_BITS bits (x rows padded to whole 32-bit words; the extent is in pls_last_error). */
+PLS_API int pls_kdmap_pose_search_scans(pls_context* ctx, const float* const* scans, const int64_t* n, int S,
+                                        const double* bases /* [sum A_s,16] */, const int* num_bases /* [S] */,
+                                        double cell, const int* half_x /* [S] */, const int* half_y /* [S] */, int K,
+                                        int32_t* out_scores /* [sum V_s] or NULL */, double* out_T /* [S,K,16] */,
+                                        int32_t* out_score /* [S,K] */, int64_t* out_index /* [S,K] */,
+                                        int* out_num /* [S] */);
 /* ProjectiveLocalMap.update (local_map.py:126-202): rel_pose [16]; vertex_map [3,H,W] or NULL. */
 PLS_API int pls_projmap_update(pls_context* ctx, const float* rel_pose, const float* vertex_map);
 PLS_API int pls_projmap_num_frames(pls_context* ctx, int* num_frames);

@@ -76,6 +76,7 @@ _SIGNATURES = {
     "pls_kdmap_frames": [_P, _P, C.POINTER(_I)],
     "pls_kdmap_pose_search": [_P, _P, _L, _P, _I, _D, _I, _I, _I, _P, _P, _P, _P, C.POINTER(_I)],
     "pls_kdmap_pose_search_pyramid": [_P, _P, _L, _P, _I, _D, _I, _I, _I, _P, _P, _P, C.POINTER(_I)],
+    "pls_kdmap_pose_search_scans": [_P, _P, _P, _I, _P, _P, _D, _P, _P, _I, _P, _P, _P, _P, _P],
     "pls_projmap_last_frame": [_P, _P],
     "pls_projmap_update": [_P, _P, _P],
     "pls_projmap_num_frames": [_P, C.POINTER(_I)],

@@ -816,3 +816,464 @@ extern "C" int pls_kdmap_pose_search_pyramid(pls_context* ctx, const float* scan
     *out_num = k;
     PLS_API_END(ctx)
 }
+
+// ---- pls_kdmap_pose_search_scans: pls_kdmap_pose_search for S scans in one call -------------------------------------
+//
+// One occupancy grid serves every scan: the bounding box of the union of the scans' reachable boxes, so that every
+// lookup of every scan lies inside it, as in the single call.  It is cleared once and filled by one ps_occupy_kernel
+// pass over the map.  The scans' rows are staged back to back, their volumes concatenated scan-major; every kernel finds
+// its scan by binary search over per-scan offsets.
+//   ps_scans_box_kernel     : ps_box_kernel per scan, blocks [blk[s], blk[s+1]) on scan s, atomics on box[6 s ..].
+//   ps_scans_score_kernel   : ps_score_kernel's tiling per (scan, base, tile); cells relative to the shared grid.
+//   ps_scans_peak_kernel    : ps_peak_kernel within each scan's volume: a neighbour never crosses a scan boundary.
+//   ps_scans_segment_kernel : the first compacted candidate of each scan, from the flag scan's positions.
+//   ps_scans_compact_kernel : keys (~score << 32) | L_local, vals = the scan.  radix_sort_pairs orders the keys, a
+//                             second, stable radix sort by scan brings each scan's candidates together in key order.
+//   ps_scans_top_kernel     : the first min(K, count) keys of each scan.
+namespace pls {
+namespace {
+
+struct PsScan {
+    int64_t row;   // first row in the staged scans
+    int64_t n;
+    int64_t base;  // first base in the concatenated bases
+    int A, Wx, Wy, tiles_x, tiles_y;
+};
+
+// the s with off[s] <= x < off[s + 1], off [S + 1] ascending (scans with no entries are skipped)
+__device__ __forceinline__ int ps_scan_of(const int64_t* __restrict__ off, int S, int64_t x) {
+    int lo = 0, hi = S - 1;
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (off[mid] <= x) lo = mid;
+        else hi = mid - 1;
+    }
+    return lo;
+}
+
+__global__ void __launch_bounds__(PS_THREADS) ps_scans_box_kernel(const float* __restrict__ rows,
+                                                                  const double* __restrict__ bases,
+                                                                  const PsScan* __restrict__ sd,
+                                                                  const int64_t* __restrict__ blk, int S, double c,
+                                                                  long long* __restrict__ box) {
+    const int s = ps_scan_of(blk, S, blockIdx.x);
+    const PsScan d = sd[s];
+    const float* scan = rows + 3 * d.row;
+    const double* B = bases + 16 * d.base;
+    const int64_t nblk = blk[s + 1] - blk[s], total = d.n * (int64_t)d.A;
+    long long lo[3] = {LLONG_MAX, LLONG_MAX, LLONG_MAX}, hi[3] = {LLONG_MIN, LLONG_MIN, LLONG_MIN};
+    for (int64_t k = (blockIdx.x - blk[s]) * PS_THREADS + threadIdx.x; k < total; k += nblk * PS_THREADS) {
+        const int64_t a = k / d.n, p = k - a * d.n;
+        long long cell[3];
+        if (!base_cell(B + 16 * a, scan[3 * p], scan[3 * p + 1], scan[3 * p + 2], c, cell[0], cell[1], cell[2])) continue;
+#pragma unroll
+        for (int r = 0; r < 3; ++r) {
+            lo[r] = min(lo[r], cell[r]);
+            hi[r] = max(hi[r], cell[r]);
+        }
+    }
+#pragma unroll
+    for (int r = 0; r < 3; ++r) {
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            lo[r] = min(lo[r], __shfl_xor_sync(0xffffffffu, lo[r], o));
+            hi[r] = max(hi[r], __shfl_xor_sync(0xffffffffu, hi[r], o));
+        }
+    }
+    if ((threadIdx.x & 31) == 0 && lo[0] <= hi[0]) {
+#pragma unroll
+        for (int r = 0; r < 3; ++r) {
+            atomicMin(box + 6 * s + r, lo[r]);
+            atomicMax(box + 6 * s + 3 + r, hi[r]);
+        }
+    }
+}
+
+// ps_score_kernel for block b of scan s (blocks [blk[s], blk[s+1])): base a, shift tile (it, jt).  Every scan's
+// reachable box lies inside the shared grid g, so the cells need no bounds test.
+__global__ void __launch_bounds__(PS_THREADS) ps_scans_score_kernel(const float* __restrict__ rows,
+                                                                    const double* __restrict__ bases,
+                                                                    const PsScan* __restrict__ sd,
+                                                                    const int64_t* __restrict__ blk,
+                                                                    const int64_t* __restrict__ vol, int S, double c,
+                                                                    PsGrid g, const uint32_t* __restrict__ bits,
+                                                                    int32_t* __restrict__ scores) {
+    __shared__ uint2 cells[PS_CHUNK];
+    __shared__ double T[16];
+    const int s = ps_scan_of(blk, S, blockIdx.x);
+    const PsScan d = sd[s];
+    const int64_t b = blockIdx.x - blk[s];
+    const int it = (int)(b % d.tiles_x);
+    const int jt = (int)((b / d.tiles_x) % d.tiles_y);
+    const int64_t a = b / ((int64_t)d.tiles_x * d.tiles_y);
+    if (threadIdx.x < 16) T[threadIdx.x] = bases[16 * (d.base + a) + threadIdx.x];
+    const float* scan = rows + 3 * d.row;
+    const int64_t n = d.n;
+    const int Wx = d.Wx, Wy = d.Wy;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int ii = it * 32 + lane, jj = jt * PS_ROWS + warp;
+    const bool active = ii < Wx && jj < Wy;
+    const uint32_t di = (uint32_t)min(ii, Wx - 1), dj_words = (uint32_t)min(jj, Wy - 1) * g.wx;
+    int32_t count = 0;
+    for (int64_t k0 = 0; k0 < n; k0 += PS_CHUNK) {
+        const int len = (int)min((int64_t)PS_CHUNK, n - k0);
+        __syncthreads();
+        for (int k = threadIdx.x; k < len; k += PS_THREADS) {
+            const int64_t p = k0 + k;
+            long long cx, cy, cz;
+            uint2 v = make_uint2(PS_SKIP, 0u);
+            if (base_cell(T, scan[3 * p], scan[3 * p + 1], scan[3 * p + 2], c, cx, cy, cz)) {
+                const uint32_t X = (uint32_t)(cx - g.o[0]) - (uint32_t)(Wx - 1) / 2u;
+                const uint32_t Y = (uint32_t)(cy - g.o[1]) - (uint32_t)(Wy - 1) / 2u;
+                const uint32_t Z = (uint32_t)(cz - g.o[2]);
+                v = make_uint2((Z * (uint32_t)g.e[1] + Y) * g.wx, X);
+            }
+            cells[k] = v;
+        }
+        __syncthreads();
+#pragma unroll 8
+        for (int k = 0; k < len; ++k) {
+            const uint2 v = cells[k];
+            if (v.x == PS_SKIP) continue;
+            const uint32_t X = v.y + di;
+            count += (int32_t)((__ldg(bits + v.x + dj_words + (X >> 5)) >> (X & 31)) & 1u);
+        }
+    }
+    if (active) scores[vol[s] + (a * Wy + jj) * (int64_t)Wx + ii] = count;
+}
+
+// ps_peak_kernel over the concatenated volumes, scan s's at [vol[s], vol[s+1])
+__global__ void ps_scans_peak_kernel(const int32_t* __restrict__ scores, const PsScan* __restrict__ sd,
+                                     const int64_t* __restrict__ vol, int S, uint8_t* __restrict__ flags) {
+    const int64_t V = vol[S];
+    for (int64_t G = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; G < V; G += (int64_t)gridDim.x * blockDim.x) {
+        const int s_ = ps_scan_of(vol, S, G);
+        const PsScan d = sd[s_];
+        const int32_t* s = scores + vol[s_];
+        const int64_t L = G - vol[s_];
+        const int A = d.A, Wy = d.Wy, Wx = d.Wx;
+        const int ii = (int)(L % Wx);
+        const int64_t t = L / Wx;
+        const int jj = (int)(t % Wy);
+        const int a = (int)(t / Wy);
+        const int32_t sc = s[L];
+        bool peak = sc > 0;
+        for (int da = -1; da <= 1 && peak; ++da) {
+            if (a + da < 0 || a + da >= A) continue;
+            for (int dj = -1; dj <= 1; ++dj) {
+                if (jj + dj < 0 || jj + dj >= Wy) continue;
+                for (int dx = -1; dx <= 1; ++dx) {
+                    if (ii + dx < 0 || ii + dx >= Wx || (da == 0 && dj == 0 && dx == 0)) continue;
+                    const int64_t Ln = L + ((int64_t)da * Wy + dj) * Wx + dx;
+                    const int32_t sn = s[Ln];
+                    if (sn > sc || (sn == sc && Ln < L)) peak = false;
+                }
+            }
+        }
+        flags[G] = peak ? 1 : 0;
+    }
+}
+
+// seg[s] = the candidates of the scans before s (seg[S] = all of them): the compacted position at vol[s]
+__global__ void ps_scans_segment_kernel(const uint32_t* __restrict__ pos, const uint32_t* __restrict__ chunk_totals,
+                                        int chunks, const int64_t* __restrict__ vol, int S, uint32_t* __restrict__ seg) {
+    for (int s = blockIdx.x * blockDim.x + threadIdx.x; s <= S; s += gridDim.x * blockDim.x) {
+        const int64_t L = vol[s];
+        const int64_t full = s < S ? L / PS_SCAN_CHUNK : chunks;
+        uint32_t at = s < S ? pos[L] : 0u;
+        for (int64_t ch = 0; ch < full; ++ch) at += chunk_totals[ch];
+        seg[s] = at;
+    }
+}
+
+// keys[at] = (~score << 32) | L_local, vals[at] = s for every flagged entry
+__global__ void ps_scans_compact_kernel(const int32_t* __restrict__ scores, const uint8_t* __restrict__ flags,
+                                        const uint32_t* __restrict__ pos, const uint32_t* __restrict__ chunk_totals,
+                                        const int64_t* __restrict__ vol, int S, uint64_t* __restrict__ keys,
+                                        uint32_t* __restrict__ vals) {
+    const int64_t V = vol[S];
+    for (int64_t G = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; G < V; G += (int64_t)gridDim.x * blockDim.x) {
+        if (!flags[G]) continue;
+        uint32_t at = pos[G];
+        for (int64_t ch = 0; ch < G / PS_SCAN_CHUNK; ++ch) at += chunk_totals[ch];
+        const int s = ps_scan_of(vol, S, G);
+        keys[at] = ((uint64_t)(~(uint32_t)scores[G]) << 32) | (uint64_t)(G - vol[s]);
+        vals[at] = (uint32_t)s;
+    }
+}
+
+// the second sort's input: key = the scan of the e-th candidate in key order, value = e
+__global__ void ps_scans_by_scan_kernel(const uint32_t* __restrict__ scan_of, int64_t num, uint64_t* __restrict__ keys,
+                                        uint32_t* __restrict__ vals) {
+    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < num; e += (int64_t)gridDim.x * blockDim.x) {
+        keys[e] = scan_of[e];
+        vals[e] = (uint32_t)e;
+    }
+}
+
+// top[s K + j] = the key of scan s's j-th candidate, j < min(K, seg[s+1] - seg[s])
+__global__ void ps_scans_top_kernel(const uint64_t* __restrict__ keys, const uint32_t* __restrict__ order,
+                                    const uint32_t* __restrict__ seg, int S, int K, uint64_t* __restrict__ top) {
+    for (int64_t c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; c < (int64_t)S * K;
+         c += (int64_t)gridDim.x * blockDim.x) {
+        const int s = (int)(c / K), j = (int)(c % K);
+        if (seg[s] + (uint32_t)j < seg[s + 1]) top[c] = keys[order[seg[s] + j]];
+    }
+}
+
+// the radix passes that order the scan ids 0..S-1
+int scan_passes(int S) {
+    int bytes = 1;
+    while (bytes < 4 && (uint32_t)(S - 1) >> (8 * bytes)) ++bytes;
+    return bytes;
+}
+
+}  // namespace
+}  // namespace pls
+
+extern "C" int pls_kdmap_pose_search_scans(pls_context* ctx, const float* const* scans, const int64_t* n, int S,
+                                           const double* bases, const int* num_bases, double cell, const int* half_x,
+                                           const int* half_y, int K, int32_t* out_scores, double* out_T,
+                                           int32_t* out_score, int64_t* out_index, int* out_num) {
+    PLS_API_BEGIN(ctx)
+    // every argument is checked before anything is enqueued: a refused call changes nothing
+    auto refuse = [](int s, const char* why) {
+        char msg[256];
+        snprintf(msg, sizeof(msg), "pls_kdmap_pose_search_scans: scan %d: %s", s, why);
+        throw pls::Error{PLS_E_INVALID, msg};
+    };
+    PLS_REQUIRE(ctx->cfg.local_map_type == PLS_MAP_KDTREE, "pls_kdmap_pose_search_scans: needs a kd-tree local map");
+    PLS_REQUIRE(ctx->kd.valid, "kd map: search before any update");
+    PLS_REQUIRE(S > 0, "pls_kdmap_pose_search_scans: S must be > 0");
+    PLS_REQUIRE(scans && n && bases && num_bases && half_x && half_y,
+                "pls_kdmap_pose_search_scans: scans, n, bases, num_bases, half_x and half_y must not be NULL");
+    PLS_REQUIRE(K >= 0 && K <= PLS_POSE_SEARCH_MAX_K, "pls_kdmap_pose_search_scans: K must lie in [0, 1024]");
+    PLS_REQUIRE(std::isfinite(cell) && cell > 0.0, "pls_kdmap_pose_search_scans: cell must be finite and > 0");
+    PLS_REQUIRE(out_num && (K == 0 || (out_T && out_score && out_index)),
+                "pls_kdmap_pose_search_scans: out_num, and for K > 0 out_T, out_score and out_index, must not be NULL");
+    std::vector<PsScan> sd((size_t)S);
+    std::vector<int64_t> off((size_t)3 * (S + 1));  // box blocks, score blocks, volumes: [S + 1] each
+    int64_t* box_blk = off.data();
+    int64_t* score_blk = box_blk + (S + 1);
+    int64_t* vol = score_blk + (S + 1);
+    int64_t rows = 0, A_total = 0;
+    for (int s = 0; s < S; ++s) {
+        if (!scans[s]) refuse(s, "the scan must not be NULL");
+        if (!(n[s] > 0 && n[s] <= INT32_MAX)) refuse(s, "the scan must be [n,3] with 0 < n < 2^31");
+        const int A = num_bases[s];
+        if (A <= 0) refuse(s, "its bases must be [A,16] with A > 0");
+        if (half_x[s] < 0 || half_y[s] < 0) refuse(s, "half_x and half_y must be >= 0");
+        if (!(half_x[s] < (1 << 30) && half_y[s] < (1 << 30) &&
+              (double)A * (2.0 * half_x[s] + 1) * (2.0 * half_y[s] + 1) < 2147483648.0))
+            refuse(s, "A*(2*half_x+1)*(2*half_y+1) must be < 2^31");
+        PsScan& d = sd[(size_t)s];
+        d.row = rows;
+        d.n = n[s];
+        d.base = A_total;
+        d.A = A;
+        d.Wx = 2 * half_x[s] + 1;
+        d.Wy = 2 * half_y[s] + 1;
+        d.tiles_x = (d.Wx + 31) / 32;
+        d.tiles_y = (d.Wy + PS_ROWS - 1) / PS_ROWS;
+        const int64_t triples = d.n * A;
+        box_blk[s + 1] = box_blk[s] + std::min<int64_t>((triples + 16 * PS_THREADS - 1) / (16 * PS_THREADS), 8 * kNumSMs);
+        score_blk[s + 1] = score_blk[s] + (int64_t)A * d.tiles_x * d.tiles_y;
+        vol[s + 1] = vol[s] + (int64_t)A * d.Wx * d.Wy;
+        rows += d.n;
+        A_total += A;
+    }
+    const int64_t V = vol[S];
+    PLS_REQUIRE(V < (1ll << 31), "pls_kdmap_pose_search_scans: the volumes together must hold fewer than 2^31 poses");
+    std::vector<double> Tb((size_t)A_total * 16);
+    if (is_device_ptr(bases)) PLS_CUDA(cudaMemcpy(Tb.data(), bases, Tb.size() * sizeof(double), cudaMemcpyDeviceToHost));
+    else memcpy(Tb.data(), bases, Tb.size() * sizeof(double));
+    for (int s = 0; s < S; ++s)
+        for (int64_t v = 16 * sd[(size_t)s].base; v < 16 * (sd[(size_t)s].base + sd[(size_t)s].A); ++v)
+            if (!std::isfinite(Tb[(size_t)v])) refuse(s, "every base must be finite");
+
+    cudaStream_t st = ctx->stream;
+    map_stream_wait(ctx);
+    // scratch of this stateless call: next_buf, never a buffer the map or an ICP keeps state in.  nb[1] holds, on
+    // 256-byte boundaries: bases, boxes [S,6], chunk totals [8], segments [S+1], descriptors, offsets, top keys [S,K].
+    DBuf* nb = ctx->next_buf;
+    size_t at = 0;
+    auto carve = [&](size_t bytes) { const size_t o = at; at += aligned((int64_t)bytes); return o; };
+    const size_t o_bases = carve(Tb.size() * sizeof(double)), o_box = carve((size_t)S * 6 * sizeof(long long));
+    const size_t o_tot = carve(8 * sizeof(uint32_t)), o_seg = carve((size_t)(S + 1) * sizeof(uint32_t));
+    const size_t o_sd = carve(sd.size() * sizeof(PsScan)), o_off = carve(off.size() * sizeof(int64_t));
+    const size_t o_top = carve((size_t)S * K * sizeof(uint64_t));
+    // the inputs of the first launch, laid out as on the device up to the top keys, copied in one go
+    std::vector<char> head(o_top);
+    memcpy(head.data() + o_bases, Tb.data(), Tb.size() * sizeof(double));
+    long long* box_init = reinterpret_cast<long long*>(head.data() + o_box);
+    for (int s = 0; s < S; ++s)
+        for (int r = 0; r < 3; ++r) box_init[6 * s + r] = LLONG_MAX, box_init[6 * s + 3 + r] = LLONG_MIN;
+    memcpy(head.data() + o_sd, sd.data(), sd.size() * sizeof(PsScan));
+    memcpy(head.data() + o_off, off.data(), off.size() * sizeof(int64_t));
+    nb[1].reserve(at, st);
+    char* blob = nb[1].as<char>();
+    PLS_CUDA(cudaMemcpyAsync(blob, head.data(), head.size(), cudaMemcpyHostToDevice, st));
+    const double* bases_dev = reinterpret_cast<const double*>(blob + o_bases);
+    long long* box_dev = reinterpret_cast<long long*>(blob + o_box);
+    uint32_t* totals_dev = reinterpret_cast<uint32_t*>(blob + o_tot);
+    uint32_t* seg_dev = reinterpret_cast<uint32_t*>(blob + o_seg);
+    const PsScan* sd_dev = reinterpret_cast<const PsScan*>(blob + o_sd);
+    const int64_t* box_blk_dev = reinterpret_cast<const int64_t*>(blob + o_off);
+    const int64_t* score_blk_dev = box_blk_dev + (S + 1);
+    const int64_t* vol_dev = score_blk_dev + (S + 1);
+    uint64_t* top_dev = reinterpret_cast<uint64_t*>(blob + o_top);
+    // every scan's rows, back to back
+    nb[0].reserve((size_t)rows * 3 * sizeof(float), st);
+    float* rows_dev = nb[0].as<float>();
+    for (int s = 0; s < S; ++s)
+        PLS_CUDA(cudaMemcpyAsync(rows_dev + 3 * sd[(size_t)s].row, scans[s], (size_t)n[s] * 3 * sizeof(float),
+                                 cudaMemcpyDefault, st));
+    ps_scans_box_kernel<<<(unsigned)box_blk[S], PS_THREADS, 0, st>>>(rows_dev, bases_dev, sd_dev, box_blk_dev, S, cell,
+                                                                      box_dev);
+    PLS_CHECK_LAUNCH();
+    std::vector<long long> box((size_t)S * 6);
+    PLS_CUDA(cudaMemcpyAsync(box.data(), box_dev, box.size() * sizeof(long long), cudaMemcpyDeviceToHost, st));
+    PLS_CUDA(cudaStreamSynchronize(st));
+
+    // the shared grid: the union of the reachable boxes of the scans with a valid row
+    PsGrid g;
+    bool any = false;
+    for (int s = 0; s < S; ++s) {
+        const long long* b = &box[(size_t)s * 6];
+        if (b[0] > b[3]) continue;  // no valid row: every score 0, no candidate
+        for (int r = 0; r < 6; ++r)
+            if (!(b[r] > -PS_MAX_CELL && b[r] < PS_MAX_CELL)) refuse(s, "a base cell lies beyond +-2^40 cells of the origin");
+        const long long half[3] = {half_x[s], half_y[s], 0};
+        long long lo[3], hi[3];
+        for (int r = 0; r < 3; ++r) lo[r] = b[r] - half[r], hi[r] = b[3 + r] + half[r];
+        if (32.0 * (double)((hi[0] - lo[0] + 1 + 31) / 32) * (double)(hi[1] - lo[1] + 1) * (double)(hi[2] - lo[2] + 1) >
+            (double)PLS_POSE_SEARCH_MAX_BITS)
+            refuse(s, "its occupancy box exceeds PLS_POSE_SEARCH_MAX_BITS (2^31); use a larger cell or a smaller window");
+        for (int r = 0; r < 3; ++r) {
+            g.o[r] = any ? std::min(g.o[r], lo[r]) : lo[r];
+            g.e[r] = any ? std::max(g.e[r], hi[r]) : hi[r];  // the max cell until the loop ends
+        }
+        any = true;
+    }
+    auto put = [&](void* dst, const void* src, size_t bytes) {  // host or device outputs
+        if (!bytes) return;
+        if (is_device_ptr(dst)) PLS_CUDA(cudaMemcpy(dst, src, bytes, cudaMemcpyHostToDevice));
+        else memcpy(dst, src, bytes);
+    };
+    if (!any) {
+        if (out_scores) {
+            if (is_device_ptr(out_scores)) PLS_CUDA(cudaMemset(out_scores, 0, (size_t)V * sizeof(int32_t)));
+            else memset(out_scores, 0, (size_t)V * sizeof(int32_t));
+        }
+        const std::vector<int> zeros((size_t)S, 0);
+        put(out_num, zeros.data(), zeros.size() * sizeof(int));
+        return PLS_OK;
+    }
+    for (int r = 0; r < 3; ++r) g.e[r] = g.e[r] - g.o[r] + 1;
+    const double grid_bits = 32.0 * (double)((g.e[0] + 31) / 32) * (double)g.e[1] * (double)g.e[2];
+    if (grid_bits > (double)PLS_POSE_SEARCH_MAX_BITS) {
+        char msg[320];
+        snprintf(msg, sizeof(msg),
+                 "pls_kdmap_pose_search_scans: the shared occupancy box of %lld x %lld x %lld cells (%.0f bits with "
+                 "word-padded x rows) exceeds PLS_POSE_SEARCH_MAX_BITS (2^31); search scans that lie far apart in "
+                 "separate calls",
+                 g.e[0], g.e[1], g.e[2], grid_bits);
+        throw pls::Error{PLS_E_INVALID, msg};
+    }
+    g.wx = (uint32_t)((g.e[0] + 31) / 32);
+    const size_t words = (size_t)g.wx * (size_t)g.e[1] * (size_t)g.e[2];
+
+    nb[2].reserve(words * sizeof(uint32_t), st);
+    uint32_t* bits = nb[2].as<uint32_t>();
+    PLS_CUDA(cudaMemsetAsync(bits, 0, words * sizeof(uint32_t), st));
+    const int64_t M = ctx->kd.count;
+    if (M > 0) {
+        ps_occupy_kernel<<<blocks_for(M, 256, 16 * kNumSMs), 256, 0, st>>>(ctx->kd.store[ctx->kd.cur].as<float4>(), M,
+                                                                           cell, g, bits);
+        PLS_CHECK_LAUNCH();
+    }
+    nb[3].reserve((size_t)V * sizeof(int32_t), st);
+    int32_t* scores = nb[3].as<int32_t>();
+    ps_scans_score_kernel<<<(unsigned)score_blk[S], PS_THREADS, 0, st>>>(rows_dev, bases_dev, sd_dev, score_blk_dev,
+                                                                          vol_dev, S, cell, g, bits, scores);
+    PLS_CHECK_LAUNCH();
+
+    std::vector<uint32_t> seg((size_t)S + 1, 0u);
+    std::vector<uint64_t> top;
+    if (K > 0) {
+        nb[4].reserve((size_t)V, st);
+        nb[5].reserve((size_t)V * sizeof(uint32_t), st);
+        uint8_t* flags = nb[4].as<uint8_t>();
+        uint32_t* pos = nb[5].as<uint32_t>();
+        ps_scans_peak_kernel<<<blocks_for(V, 256, 16 * kNumSMs), 256, 0, st>>>(scores, sd_dev, vol_dev, S, flags);
+        PLS_CHECK_LAUNCH();
+        const int chunks = (int)((V + PS_SCAN_CHUNK - 1) / PS_SCAN_CHUNK);
+        for (int ch = 0; ch < chunks; ++ch) {
+            const int64_t o = (int64_t)ch * PS_SCAN_CHUNK;
+            exclusive_scan_flags(ctx, flags + o, std::min(PS_SCAN_CHUNK, V - o), pos + o, totals_dev + ch);
+        }
+        ps_scans_segment_kernel<<<blocks_for(S + 1, 256, 16 * kNumSMs), 256, 0, st>>>(pos, totals_dev, chunks, vol_dev,
+                                                                                       S, seg_dev);
+        PLS_CHECK_LAUNCH();
+        PLS_CUDA(cudaMemcpyAsync(seg.data(), seg_dev, seg.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+        PLS_CUDA(cudaStreamSynchronize(st));
+        const int64_t num = seg[(size_t)S];
+        if (num > 0) {
+            nb[6].reserve((size_t)num * sizeof(uint64_t), st);
+            nb[7].reserve((size_t)num * sizeof(uint32_t), st);
+            uint64_t* keys = nb[6].as<uint64_t>();
+            uint32_t* vals = nb[7].as<uint32_t>();
+            ps_scans_compact_kernel<<<blocks_for(V, 256, 16 * kNumSMs), 256, 0, st>>>(scores, flags, pos, totals_dev,
+                                                                                      vol_dev, S, keys, vals);
+            PLS_CHECK_LAUNCH();
+            uint64_t* ko = nullptr;
+            uint32_t* vo = nullptr;
+            radix_sort_pairs(ctx, keys, vals, num, 8, &ko, &vo);  // eight passes: sorted back in keys, vals
+            // flags and pos are spent: the stable sort by scan takes their buffers
+            nb[4].reserve((size_t)num * sizeof(uint64_t), st);
+            uint64_t* by_scan = nb[4].as<uint64_t>();
+            uint32_t* order = nb[5].as<uint32_t>();
+            ps_scans_by_scan_kernel<<<blocks_for(num, 256, 16 * kNumSMs), 256, 0, st>>>(vals, num, by_scan, order);
+            PLS_CHECK_LAUNCH();
+            uint64_t* so = nullptr;
+            uint32_t* oo = nullptr;
+            radix_sort_pairs(ctx, by_scan, order, num, scan_passes(S), &so, &oo);
+            ps_scans_top_kernel<<<blocks_for((int64_t)S * K, 256, 16 * kNumSMs), 256, 0, st>>>(keys, oo, seg_dev, S, K,
+                                                                                               top_dev);
+            PLS_CHECK_LAUNCH();
+            top.resize((size_t)S * K);
+            PLS_CUDA(cudaMemcpyAsync(top.data(), top_dev, top.size() * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+        }
+    }
+    if (out_scores)
+        PLS_CUDA(cudaMemcpyAsync(out_scores, scores, (size_t)V * sizeof(int32_t), cudaMemcpyDefault, st));
+    PLS_CUDA(cudaStreamSynchronize(st));
+
+    std::vector<int> nums((size_t)S);
+    std::vector<double> T((size_t)K * 16);
+    std::vector<int32_t> sc((size_t)K);
+    std::vector<int64_t> idx((size_t)K);
+    for (int s = 0; s < S; ++s) {
+        const PsScan& d = sd[(size_t)s];
+        const int k = (int)std::min<int64_t>(K, (int64_t)seg[(size_t)s + 1] - seg[(size_t)s]);
+        for (int c = 0; c < k; ++c) {
+            const uint64_t key = top[(size_t)s * K + c];
+            const int64_t L = (int64_t)(key & 0xffffffffull);
+            sc[(size_t)c] = (int32_t)~(uint32_t)(key >> 32);
+            idx[(size_t)c] = L;
+            const int i = (int)(L % d.Wx) - half_x[s], j = (int)((L / d.Wx) % d.Wy) - half_y[s];
+            const int64_t a = L / ((int64_t)d.Wx * d.Wy);
+            memcpy(&T[16 * (size_t)c], &Tb[16 * (size_t)(d.base + a)], 16 * sizeof(double));
+            T[16 * (size_t)c + 3] += (double)i * cell;
+            T[16 * (size_t)c + 7] += (double)j * cell;
+        }
+        if (k) {
+            put(out_T + (size_t)s * K * 16, T.data(), (size_t)k * 16 * sizeof(double));
+            put(out_score + (size_t)s * K, sc.data(), (size_t)k * sizeof(int32_t));
+            put(out_index + (size_t)s * K, idx.data(), (size_t)k * sizeof(int64_t));
+        }
+        nums[(size_t)s] = k;
+    }
+    put(out_num, nums.data(), nums.size() * sizeof(int));
+    PLS_API_END(ctx)
+}

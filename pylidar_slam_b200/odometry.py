@@ -180,6 +180,96 @@ def _pose_search(ctx, scan, poses, cell_size, half_x, half_y, num_candidates, ou
     return T[:k], score[:k], index[:k]
 
 
+# pls_kdmap_pose_search_scans refuses batches whose volumes together hold 2^31 poses or more
+_POSE_SEARCH_SCANS_MAX_POSES = 1 << 31
+_SHARED_GRID_REFUSAL = "shared occupancy box"
+
+
+def _pose_search_scans(ctx, scans, bases_list, cell_size, halves, num_candidates, out_scores=None):
+    """_pose_search for S scans: scans [n_s,3] (numpy or torch, host or CUDA), bases_list S arrays [A_s,4,4], halves S
+    pairs (half_x, half_y).  Returns S tuples (T, scores, index), tuple s what _pose_search gives scan s; out_scores
+    [sum V_s] int32 (nullable) receives every volume, scan-major.  With K >= 1 and no out_scores, a scan of at least
+    POSE_SEARCH_PYRAMID_MIN_POSES poses goes to _pose_search (the pyramid, with its fallback); the others go to
+    pls_kdmap_pose_search_scans in consecutive chunks of fewer than 2^31 poses.  A chunk whose shared occupancy grid is
+    refused -- scans that lie far apart on a large map -- is sorted by its first base's x, halved and retried; a chunk
+    of one scan goes to _pose_search."""
+    S, K = len(scans), int(num_candidates)
+    assert_debug(len(bases_list) == S and len(halves) == S, "one base set and one window per scan")
+    pts, bases, vols = [], [], []
+    for s in range(S):
+        check_tensor(scans[s], [-1, 3])
+        pts.append(_f32c(scans[s]))
+        b = bases_list[s]
+        if isinstance(b, torch.Tensor):
+            b = b.detach().cpu().numpy()
+        check_tensor(b, [-1, 4, 4])
+        bases.append(np.ascontiguousarray(b, dtype=np.float64))
+        hx, hy = (int(h) for h in halves[s])
+        vols.append(bases[s].shape[0] * (2 * hx + 1) * (2 * hy + 1))
+    first = np.concatenate([[0], np.cumsum(vols, dtype=np.int64)])
+    results = [None] * S
+
+    def single(s):
+        hx, hy = halves[s]
+        view = None if out_scores is None else out_scores[first[s]:first[s + 1]]
+        results[s] = _pose_search(ctx, pts[s], bases[s], cell_size, hx, hy, K, out_scores=view)
+
+    def batched(idx):
+        if len(idx) == 1:
+            return single(idx[0])
+        S_c, Kc = len(idx), max(K, 1)
+        addresses = np.array([_lib.ptr(pts[s]) for s in idx], dtype=np.uint64)
+        rows = np.array([pts[s].shape[0] for s in idx], dtype=np.int64)
+        cat = np.ascontiguousarray(np.concatenate([bases[s] for s in idx]))
+        num_bases = np.array([bases[s].shape[0] for s in idx], dtype=np.int32)
+        hx = np.array([int(halves[s][0]) for s in idx], dtype=np.int32)
+        hy = np.array([int(halves[s][1]) for s in idx], dtype=np.int32)
+        vol = None if out_scores is None else np.empty(sum(vols[s] for s in idx), np.int32)
+        T, score = np.zeros((S_c, Kc, 4, 4), np.float64), np.zeros((S_c, Kc), np.int32)
+        index, num = np.zeros((S_c, Kc), np.int64), np.zeros(S_c, np.int32)
+        try:
+            ctx.call("pls_kdmap_pose_search_scans", _lib.ptr(addresses), _lib.ptr(rows), S_c, _lib.ptr(cat),
+                     _lib.ptr(num_bases), float(cell_size), _lib.ptr(hx), _lib.ptr(hy), K, _lib.ptr(vol), _lib.ptr(T),
+                     _lib.ptr(score), _lib.ptr(index), _lib.ptr(num))
+        except AssertionError as e:
+            if _SHARED_GRID_REFUSAL not in str(e):
+                raise
+            by_x = sorted(idx, key=lambda s: bases[s][0, 0, 3])
+            batched(by_x[:S_c // 2])
+            batched(by_x[S_c // 2:])
+            return
+        at = 0
+        for c, s in enumerate(idx):
+            k = int(num[c])
+            results[s] = (T[c, :k], score[c, :k], index[c, :k])
+            if vol is not None:
+                out_scores[first[s]:first[s + 1]] = vol[at:at + vols[s]]
+                at += vols[s]
+
+    chunk, poses = [], 0
+    for s in range(S):
+        if out_scores is None and K >= 1 and vols[s] >= POSE_SEARCH_PYRAMID_MIN_POSES:
+            single(s)
+            continue
+        if chunk and poses + vols[s] >= _POSE_SEARCH_SCANS_MAX_POSES:
+            batched(chunk)
+            chunk, poses = [], 0
+        chunk.append(s)
+        poses += vols[s]
+    if chunk:
+        batched(chunk)
+    return results
+
+
+def _per_scan_halves(half_extents, S):
+    """One (half_x, half_y) pair for each of S scans, from one shared pair or S pairs."""
+    h = np.asarray(half_extents, dtype=np.int64)
+    if h.shape == (2,):
+        return [(int(h[0]), int(h[1]))] * S
+    assert_debug(h.shape == (S, 2), "half_extents must be one (half_x, half_y) pair or one pair per scan")
+    return [(int(x), int(y)) for x, y in h]
+
+
 def _score_poses(ctx, scan, poses, cell_size) -> np.ndarray:
     """The [A] int32 scores of exactly these poses: pls_kdmap_pose_search with a 1x1 window and no candidates."""
     if isinstance(poses, torch.Tensor):
@@ -228,6 +318,16 @@ class PoseCandidate:
     status: int
 
 
+def _pose_candidates(T0, coarse, T, iters, status, scores) -> list:
+    """localize's result for one scan from its search candidates (T0 [k,4,4], coarse [k]) and their refinements (T,
+    iters, status, refined scores [k]): every candidate as a PoseCandidate, ordered by status (singular last), then
+    refined score (descending), then search rank."""
+    singular = status == _lib.PLS_E_SINGULAR
+    order = np.lexsort((np.arange(T.shape[0]), -scores.astype(np.int64), singular))
+    return [PoseCandidate(T=T[r].astype(np.float64), score=int(scores[r]), T0=T0[r], coarse_score=int(coarse[r]),
+                          coarse_rank=int(r), iterations=int(iters[r]), status=int(status[r])) for r in order]
+
+
 class KdTreeLocalMap(LocalMap):
     """KdTreeLocalMap (local_map.py:254-427) on the GPU: exact 1-NN over the hashed cell pyramid + lazily cached 10-NN normals.
 
@@ -273,6 +373,17 @@ class KdTreeLocalMap(LocalMap):
         branch and bound (pls_kdmap_pose_search_pyramid) with the same result, so half_extent may span the whole map."""
         hx, hy = half_extent
         return _pose_search(self.ctx, scan, base_poses, cell_size, hx, hy, num_candidates)
+
+    def search_poses_scans(self, scans, base_poses, cell_size: float, half_extents=(0, 0), num_candidates: int = 8):
+        """search_poses for S scans in one call (pls_kdmap_pose_search_scans; no reference counterpart): a localisation
+        server re-localising many vehicles' scans, offline map matching a recorded drive's scans.  scans: S [n_s,3]
+        arrays or tensors; base_poses: S arrays [A_s,4,4]; half_extents: one pair for every scan or one pair per scan.
+        Returns S tuples (T, scores, index); tuple s is what search_poses(scans[s], base_poses[s], cell_size,
+        half_extents[s], num_candidates) returns.  The map is left unchanged."""
+        S = len(scans)
+        assert_debug(len(base_poses) == S, "base_poses must hold one [A,4,4] array per scan")
+        return _pose_search_scans(self.ctx, scans, base_poses, cell_size, _per_scan_halves(half_extents, S),
+                                  num_candidates)
 
     def score_poses(self, scan, poses, cell_size: float) -> np.ndarray:
         """The [A] int32 scores of exactly these poses [A,4,4] (search_poses' score, without shifts)."""
@@ -964,10 +1075,47 @@ class ICPFrameToModel(OdometryAlgorithm):
         _, T, _, iters = self.register_new_frame_hypotheses(scan, T0.astype(np.float32))
         status = self.last_hypotheses_status
         scores = _score_poses(self.ctx, scan, T.astype(np.float64), cell_size)
-        singular = status == _lib.PLS_E_SINGULAR
-        order = np.lexsort((np.arange(T.shape[0]), -scores.astype(np.int64), singular))
-        return [PoseCandidate(T=T[r].astype(np.float64), score=int(scores[r]), T0=T0[r], coarse_score=int(coarse[r]),
-                              coarse_rank=int(r), iterations=int(iters[r]), status=int(status[r])) for r in order]
+        return _pose_candidates(T0, coarse, T, iters, status, scores)
+
+    def localize_scans(self, scans, prior_poses, radius, cell_size: float, yaw_range: float = np.pi,
+                       yaw_step: float = np.deg2rad(5), num_candidates: int = 8):
+        """localize for S scans on the one kd map this odometry's context holds (no reference counterpart): a
+        localisation server re-localising many vehicles' scans, offline map matching a recorded drive's scans from
+        GNSS fixes.  scans: S [n_s,3] arrays or tensors; prior_poses [S,4,4]; radius a scalar or [S].
+        One batched search over every scan's yaw_sweep bases (KdTreeLocalMap.search_poses_scans), one
+        register_new_frames call over every candidate, one batched rescoring of the refined poses.  Returns S lists of
+        PoseCandidate; list s equals localize(scans[s], prior_poses[s], radius[s], cell_size, yaw_range, yaw_step,
+        num_candidates), field for field."""
+        _check_given_normals(self.ctx)
+        S = len(scans)
+        if isinstance(prior_poses, torch.Tensor):
+            prior_poses = prior_poses.detach().cpu().numpy()
+        check_tensor(prior_poses, [S, 4, 4])
+        radii = np.broadcast_to(np.asarray(radius, dtype=np.float64), (S,))
+        assert_debug(bool(np.all(np.isfinite(radii) & (radii >= 0))), "radius must be finite and >= 0")
+        assert_debug(np.isfinite(cell_size) and cell_size > 0, "cell_size must be finite and > 0")
+        bases = [yaw_sweep(prior_poses[s], yaw_range, yaw_step) for s in range(S)]
+        halves = [(h, h) for h in (int(np.ceil(r / cell_size)) for r in radii)]
+        found = _pose_search_scans(self.ctx, scans, bases, cell_size, halves, num_candidates)
+        counts = [T0.shape[0] for T0, _, _ in found]
+        if sum(counts) == 0:
+            return [[] for _ in range(S)]
+        T0_all = np.concatenate([T0 for T0, _, _ in found])
+        _, T, _, iters = self.register_new_frames(scans, T0_all.astype(np.float32),
+                                                  np.repeat(np.arange(S, dtype=np.int32), counts))
+        status = self.last_registrations_status
+        hit = [s for s in range(S) if counts[s]]
+        first = np.concatenate([[0], np.cumsum(counts)])
+        scores = np.zeros(T.shape[0], np.int32)
+        _pose_search_scans(self.ctx, [scans[s] for s in hit],
+                           [T[first[s]:first[s + 1]].astype(np.float64) for s in hit], cell_size, [(0, 0)] * len(hit),
+                           0, out_scores=scores)
+        out = []
+        for s in range(S):
+            r = slice(first[s], first[s + 1])
+            out.append(_pose_candidates(found[s][0], found[s][1], T[r], iters[r], status[r], scores[r]) if counts[s]
+                       else [])
+        return out
 
     def register_new_frames(self, scans, initial_estimates, scan_indices=None):
         """register_new_frame for many scans against the one map this odometry's context holds, in one call
