@@ -153,6 +153,12 @@ void finish_out(pls_context* ctx, const OutArg& o, size_t bytes_used) {
     if (b) PLS_CUDA(cudaMemcpyAsync(o.host, o.dev, b, cudaMemcpyDeviceToHost, ctx->stream));
 }
 
+void put_out(void* dst, const void* src, size_t bytes) {
+    if (!dst || !bytes) return;
+    if (is_device_ptr(dst)) PLS_CUDA(cudaMemcpy(dst, src, bytes, cudaMemcpyHostToDevice));
+    else memcpy(dst, src, bytes);
+}
+
 ProfileScope::ProfileScope(pls_context* c, int w, double bytes, bool count) : ctx(c), which(w) {
     ProfileSlot& s = ctx->prof[which];
     if (!s.enabled) return;

@@ -323,6 +323,9 @@ struct OutArg {
 };
 OutArg out_arg(pls_context* ctx, void* p, size_t bytes, DBuf& stage);
 void finish_out(pls_context* ctx, const OutArg& o, size_t bytes_used = (size_t)-1);
+// Copies `bytes` of host memory to an output that may be host or device memory; nothing for a NULL dst or zero bytes.
+// Synchronous: the caller's host buffer may go once it returns.
+void put_out(void* dst, const void* src, size_t bytes);
 
 inline uint32_t* scalar_u32(pls_context* ctx, int i) {
     return reinterpret_cast<uint32_t*>(reinterpret_cast<char*>(ctx->scalars.p) + kScalarOffset) + i;

@@ -1046,16 +1046,11 @@ static void register_batch(pls_context* ctx, const KdScan* scans, int64_t n, con
     else projmap_hypothesis_adopt(ctx, last, st);
     fetch_result(ctx);
     ctx->icp_result = true;
-    auto put = [&](void* dst, const void* src, size_t bytes) {  // host or device outputs, as pls_register_frame
-        if (!dst) return;
-        if (is_device_ptr(dst)) PLS_CUDA(cudaMemcpy(dst, src, bytes, cudaMemcpyHostToDevice));
-        else memcpy(dst, src, bytes);
-    };
-    put(out_T, T.data(), T.size() * sizeof(float));
-    put(out_params, params.data(), params.size() * sizeof(float));
-    put(out_losses, losses.data(), losses.size() * sizeof(float));
-    put(out_iters, iters.data(), iters.size() * sizeof(int));
-    put(out_status, status.data(), status.size() * sizeof(int));
+    put_out(out_T, T.data(), T.size() * sizeof(float));
+    put_out(out_params, params.data(), params.size() * sizeof(float));
+    put_out(out_losses, losses.data(), losses.size() * sizeof(float));
+    put_out(out_iters, iters.data(), iters.size() * sizeof(int));
+    put_out(out_status, status.data(), status.size() * sizeof(int));
     if (!out_status) raise_status(ctx, first_error);
 }
 
@@ -1118,14 +1113,9 @@ int pls_register_frame(pls_context* ctx, const float* points, int64_t n, const f
     ctx->icp_result = true;
     FrameResult* h = frame_result_host(ctx);
     credit_icp_profile(ctx, h, icp_blocks);
-    auto put = [&](void* dst, const void* src, size_t bytes) {
-        if (!dst) return;
-        if (is_device_ptr(dst)) PLS_CUDA(cudaMemcpy(dst, src, bytes, cudaMemcpyHostToDevice));
-        else memcpy(dst, src, bytes);
-    };
-    put(out_T, h->T, 16 * sizeof(float));
-    put(out_params, h->params, 6 * sizeof(float));
-    put(out_losses, h->losses, (size_t)ctx->cfg.max_num_alignments * sizeof(float));
+    put_out(out_T, h->T, 16 * sizeof(float));
+    put_out(out_params, h->params, 6 * sizeof(float));
+    put_out(out_losses, h->losses, (size_t)ctx->cfg.max_num_alignments * sizeof(float));
     if (out_iters) *out_iters = h->iters;
     raise_status(ctx, h->status);
     PLS_API_END(ctx)

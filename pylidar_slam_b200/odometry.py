@@ -146,6 +146,14 @@ def _check_given_normals(ctx):
 POSE_SEARCH_PYRAMID_MIN_POSES = 1 << 27
 
 
+def _bases_f64(poses) -> np.ndarray:
+    """Pose-search bases [A,4,4] (numpy or torch, host or CUDA) as a contiguous float64 host array."""
+    if isinstance(poses, torch.Tensor):
+        poses = poses.detach().cpu().numpy()
+    check_tensor(poses, [-1, 4, 4])
+    return np.ascontiguousarray(poses, dtype=np.float64)
+
+
 def _pose_search(ctx, scan, poses, cell_size, half_x, half_y, num_candidates, out_scores=None):
     """The correlative pose search on ctx's kd map: scan [n,3] (numpy or torch, host or CUDA), poses [A,4,4] (float64).
     Returns (T [k,4,4] float64, scores [k] int32, index [k] int64).  Both calls return the same candidates bit for bit;
@@ -154,10 +162,7 @@ def _pose_search(ctx, scan, poses, cell_size, half_x, half_y, num_candidates, ou
     exhaustive call answering any volume below 2^31 poses that the pyramid refuses."""
     check_tensor(scan, [-1, 3])
     pts = _f32c(scan)
-    if isinstance(poses, torch.Tensor):
-        poses = poses.detach().cpu().numpy()
-    check_tensor(poses, [-1, 4, 4])
-    bases = np.ascontiguousarray(poses, dtype=np.float64)
+    bases = _bases_f64(poses)
     K = int(num_candidates)
     T, score = np.zeros((K, 4, 4), np.float64), np.zeros(K, np.int32)
     index, num = np.zeros(K, np.int64), C.c_int(0)
@@ -199,11 +204,7 @@ def _pose_search_scans(ctx, scans, bases_list, cell_size, halves, num_candidates
     for s in range(S):
         check_tensor(scans[s], [-1, 3])
         pts.append(_f32c(scans[s]))
-        b = bases_list[s]
-        if isinstance(b, torch.Tensor):
-            b = b.detach().cpu().numpy()
-        check_tensor(b, [-1, 4, 4])
-        bases.append(np.ascontiguousarray(b, dtype=np.float64))
+        bases.append(_bases_f64(bases_list[s]))
         hx, hy = (int(h) for h in halves[s])
         vols.append(bases[s].shape[0] * (2 * hx + 1) * (2 * hy + 1))
     first = np.concatenate([[0], np.cumsum(vols, dtype=np.int64)])
@@ -272,11 +273,9 @@ def _per_scan_halves(half_extents, S):
 
 def _score_poses(ctx, scan, poses, cell_size) -> np.ndarray:
     """The [A] int32 scores of exactly these poses: pls_kdmap_pose_search with a 1x1 window and no candidates."""
-    if isinstance(poses, torch.Tensor):
-        poses = poses.detach().cpu().numpy()
-    check_tensor(poses, [-1, 4, 4])
-    scores = np.zeros(poses.shape[0], np.int32)
-    _pose_search(ctx, scan, poses, cell_size, 0, 0, 0, out_scores=scores)
+    bases = _bases_f64(poses)
+    scores = np.zeros(bases.shape[0], np.int32)
+    _pose_search(ctx, scan, bases, cell_size, 0, 0, 0, out_scores=scores)
     return scores
 
 

@@ -1,6 +1,6 @@
 """pls_kdmap_pose_search_scans on the GPU against per-scan pls_kdmap_pose_search on the same context, bit for bit:
-volumes and candidates for S = 1, 2, 64 and 300, mixed bases, rows and windows (0 x 0, and the score kernel's word and
-tile edges), NaN rows and scans without a valid row, plateaus with K = 0, 1 and 1024, a batch crossing the 2^29 flag
+volumes and candidates for S = 1, 2, 64 and 300 (and, up to S = 64, every scan's volume against the float64 reference,
+since both calls run the same pipeline), mixed bases, rows and windows (0 x 0, and the score kernel's word and tile edges), NaN rows and scans without a valid row, plateaus with K = 0, 1 and 1024, a batch crossing the 2^29 flag
 chunk inside one scan's volume, scans far apart on the 2 km map, host, device and mixed pointers; every refusal, each
 leaving the outputs unwritten and the context unchanged; and ICPFrameToModel.localize_scans against a loop of
 localize on the scene and the 2 km map."""
@@ -19,6 +19,7 @@ sys.path.insert(0, os.path.join(ROOT, "tools"))
 import pylidar_slam_b200 as b200  # noqa: E402
 from pylidar_slam_b200 import _lib as lib  # noqa: E402
 from pylidar_slam_b200 import synthetic as syn  # noqa: E402
+from oracle import pose_search_reference as ref  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
@@ -79,9 +80,9 @@ def _raw(ctx, scans, bases, cell, hxs, hys, K, outs=None, S=None, cat=None, num_
     return st, o
 
 
-def _check(ctx, scans, bases, cell, hxs, hys, K, **kw):
+def _check(ctx, scans, bases, cell, hxs, hys, K, want_volumes=None, **kw):
     """The batched call equals the single call per scan, and writes nothing past out_num[s]; returns the candidate
-    counts."""
+    counts.  want_volumes: each scan's reference score volume, which its part of the batched volume must equal."""
     st, o = _raw(ctx, scans, bases, cell, hxs, hys, K, **kw)
     assert st == lib.PLS_OK, lib.load().pls_last_error(ctx.handle)
     o = _host(o)
@@ -91,6 +92,8 @@ def _check(ctx, scans, bases, cell, hxs, hys, K, **kw):
         b = bases[s].cpu().numpy() if isinstance(bases[s], torch.Tensor) else bases[s]
         vol, T, sc, ix = _single(ctx, scan, b, cell, int(hxs[s]), int(hys[s]), K)
         assert np.array_equal(o["vol"][at:at + vol.size], vol), s
+        if want_volumes is not None:
+            assert np.array_equal(o["vol"][at:at + vol.size], want_volumes[s].reshape(-1)), s
         at += vol.size
         k = int(o["num"][s])
         assert k == len(ix), s
@@ -131,7 +134,8 @@ WINDOWS = [(0, 0), (15, 3), (16, 4), (1, 1), (0, 5), (7, 0), (32, 2), (3, 16)]
 @pytest.mark.parametrize("S", [1, 2, 64, 300])
 def test_equals_the_single_call_per_scan(S):
     rng = np.random.RandomState(S)
-    ctx = _map_ctx(_scene_map(rng))
+    m = _scene_map(rng)
+    ctx = _map_ctx(m)
     scans, bases, hxs, hys = [], [], [], []
     for s in range(S):
         n = int(rng.choice([1, 7, 255, 256, 1025, 3000] if S <= 64 else [1, 31, 200]))
@@ -140,8 +144,10 @@ def test_equals_the_single_call_per_scan(S):
         hx, hy = WINDOWS[s % len(WINDOWS)]
         hxs.append(hx)
         hys.append(hy)
+    # both calls run the same code: for S <= 64 every scan's volume is also checked against the float64 reference
+    want = [ref.score_volume(scans[s], bases[s], 0.5, hxs[s], hys[s], m) for s in range(S)] if S <= 64 else None
     for K in (0, 1, 8, 1024):
-        nums = _check(ctx, scans, bases, 0.5, hxs, hys, K)
+        nums = _check(ctx, scans, bases, 0.5, hxs, hys, K, want_volumes=want)
         assert K == 0 or sum(nums) > 0
 
 
