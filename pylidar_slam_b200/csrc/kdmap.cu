@@ -20,6 +20,7 @@
 #include "icp_device.cuh"
 #include "kdmap_device.cuh"
 #include "pose_device.cuh"
+#include "projection_device.cuh"
 
 namespace pls {
 
@@ -395,13 +396,6 @@ __device__ __forceinline__ bool claim_normal(const KdIndex& ix, int pos) {
     return cur != valid && cur != claimed && atomicCAS(w, cur, claimed) == cur;
 }
 
-// p = T p0, T the first three rows of a row-major 4x4 pose.
-__device__ __forceinline__ void transform_query(const float* T, const float4& p0, float* p) {
-    p[0] = p0.x * T[0] + p0.y * T[1] + p0.z * T[2] + T[3];
-    p[1] = p0.x * T[4] + p0.y * T[5] + p0.z * T[6] + T[7];
-    p[2] = p0.x * T[8] + p0.y * T[9] + p0.z * T[10] + T[11];
-}
-
 // 1-NN of ICP iterations after a frame's first: VERIFY instead of searching.  The full search stored in `state` where
 // the query stood (xyz, its transformed position) and in .w a lower bound of the squared distance to every map point
 // other than its match.  If the query, now at p, has moved by eps since then and its match `pos` is now at distance d,
@@ -491,7 +485,7 @@ __device__ __forceinline__ void kd_nn_verify_body(const KdIndex& ix, const float
     const int64_t qi = q_begin + ((int64_t)block * KD_THREADS + threadIdx.x) * q_stride;
     if (qi < nq) {
         float p[3];
-        transform_query(sT, queries[qi], p);
+        transform_point(sT, queries[qi], p);
         if (!match_proven(ix, p, match[qi], nn_state[qi])) s_hard[atomicAdd(&s_nh, 1)] = (int)qi;
     }
     __syncthreads();
@@ -570,7 +564,7 @@ __device__ __forceinline__ void kd_nn_warp_body(const KdIndex& ix, const float4*
             if (hard) hn = match[qn];
         }
         float p[3];
-        transform_query(t, p0, p);
+        transform_point(t, p0, p);
         float second;
         const int pos = warp_nearest(ix, g, p[0], p[1], p[2], hint, lane, &cand, &second);
         if (lane == 0) {
@@ -695,7 +689,7 @@ __device__ __forceinline__ void kd_residual_body(const KdIndex& ix, const float4
         const int64_t qi = q_begin + s * q_stride;
         if (qi >= nq) break;
         float p[3];
-        transform_query(sT, queries[qi], p);
+        transform_point(sT, queries[qi], p);
         const int pos = match[qi];
         if (pos < 0) continue;
         accumulate_match(acc, ix, p, pos, scheme, sigma KD_SPLIT_PASS);
@@ -755,7 +749,7 @@ __device__ __forceinline__ void kd_icp_refine_body(const KdIndex& ix, const floa
         const int64_t qi = q_begin + (round + threadIdx.x) * q_stride;
         if (owner && qi < nq) {
             float p[3];
-            transform_query(sT, queries[qi], p);
+            transform_point(sT, queries[qi], p);
             if (!match_proven(ix, p, match[qi], nn_state[qi])) s_hard[atomicAdd(&s_nh, 1)] = threadIdx.x;
         }
         __syncthreads();
@@ -768,7 +762,7 @@ __device__ __forceinline__ void kd_icp_refine_body(const KdIndex& ix, const floa
             for (int e = warp; e < nh; e += KD_REFINE_WARPS) {
                 const int64_t q = q_begin + (round + s_hard[e]) * q_stride;
                 float p[3];
-                transform_query(sT, queries[q], p);
+                transform_point(sT, queries[q], p);
                 float second;
                 const int pos = warp_nearest(ix, g, p[0], p[1], p[2], match[q], lane, &cand_nn, &second);
                 if (lane == 0) {
@@ -805,7 +799,7 @@ __device__ __forceinline__ void kd_icp_refine_body(const KdIndex& ix, const floa
         const int pos = match[qi];
         if (pos < 0) continue;
         float p[3];
-        transform_query(sT, queries[qi], p);
+        transform_point(sT, queries[qi], p);
         accumulate_match(acc, ix, p, pos, scheme, sigma KD_SPLIT_PASS);
     }
     block_partial_and_finish<KD_REFINE_THREADS>(acc, fr, partials, fuse_threshold, block, grid KD_SPLIT_PASS);

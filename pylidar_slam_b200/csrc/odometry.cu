@@ -214,7 +214,8 @@ struct FrameInputSelect {
         if (zbuf) {
             int pix;
             float r;
-            if (project_to_pixel(s.x, s.y, s.z, pc, pix, r) &&
+            // zbuf_points_kernel's order: a range one ulp off would drop this query
+            if (project_to_pixel(s.x, s.y, s.z, pc, pix, r, RangeOrder::kYFirst) &&
                 zbuf[pix] == (((unsigned long long)__float_as_uint(r) << 32) | (unsigned long long)(uint32_t)i)) {
                 s.pix = pix;
                 f |= 2u;

@@ -21,7 +21,7 @@ __global__ void project_pixels_kernel(const float* __restrict__ xyz, int64_t n, 
                                       float* __restrict__ out) {
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
         float row, col, r;
-        project_point(xyz[3 * i], xyz[3 * i + 1], xyz[3 * i + 2], pc, row, col, r);
+        project_point(xyz[3 * i], xyz[3 * i + 1], xyz[3 * i + 2], pc, row, col, r, RangeOrder::kYFirst);
         out[2 * i] = row;
         out[2 * i + 1] = col;
     }
@@ -35,7 +35,7 @@ __global__ void zbuf_kernel(const float* __restrict__ xyz, int batch, int64_t n,
         int64_t b = g / n, i = g - b * n;
         int pix;
         float r;
-        if (project_to_pixel(xyz[3 * g], xyz[3 * g + 1], xyz[3 * g + 2], pc, pix, r)) {
+        if (project_to_pixel(xyz[3 * g], xyz[3 * g + 1], xyz[3 * g + 2], pc, pix, r, RangeOrder::kYFirst)) {
             unsigned long long key = ((unsigned long long)__float_as_uint(r) << 32) | (unsigned long long)(uint32_t)i;
             atomicMin(&zbuf[b * hw + pix], key);
         }
@@ -48,7 +48,8 @@ __global__ void zbuf_points_kernel(const float* __restrict__ xyz, int64_t n, con
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
         int pix;
         float r;
-        if (project_to_pixel(xyz[3 * i], xyz[3 * i + 1], xyz[3 * i + 2], pc, pix, r))
+        // the order FrameInputSelect::flags tests this z-buffer's winners with
+        if (project_to_pixel(xyz[3 * i], xyz[3 * i + 1], xyz[3 * i + 2], pc, pix, r, RangeOrder::kYFirst))
             atomicMin(&zbuf[pix], ((unsigned long long)__float_as_uint(r) << 32) | (unsigned long long)(uint32_t)i);
     }
 }
@@ -81,15 +82,13 @@ struct ProjConst64 {
 
 __device__ __forceinline__ bool project_to_pixel_f64(double x, double y, double z, const ProjConst64& pc, int& pix, double& r) {
     const double kPi = 3.141592653589793;  // np.pi
-    r = sqrt(x * x + y * y + z * z);
+    r = range_rn(x, y, z, RangeOrder::kYFirst);
     const bool null = (r == 0.0);
     const double rr = null ? 0.001 : r;
     const double theta = -atan2(y, x);
-    const double phi = asin(z / rr);
-    double c = 0.5 * (theta / kPi + 1.0);
-    double rw = 1.0 - (phi + pc.abs_down) / pc.fov;
-    c = c * pc.Wf;
-    rw = rw * pc.Hf;
+    const double phi = asin(div_rn(z, rr));
+    const double c = mul_rn(mul_rn(0.5, add_rn(div_rn(theta, kPi), 1.0)), pc.Wf);
+    const double rw = mul_rn(add_rn(1.0, -div_rn(add_rn(phi, pc.abs_down), pc.fov)), pc.Hf);
     const double pr = rint(null ? -1.0 : rw), pcn = rint(null ? -1.0 : c);
     const bool ok = (pr >= 0.0) && (pr <= (double)(pc.H - 1)) && (pcn >= 0.0) && (pcn <= (double)(pc.W - 1)) && (r > 0.0);
     if (!ok) return false;

@@ -135,9 +135,7 @@ __device__ __forceinline__ bool model_point(const float* __restrict__ vmaps, con
     const float x = vmaps[src], y = vmaps[hw + src], z = vmaps[2 * hw + src];
     // mask_not_null (geometry.py:157-177): any channel non-zero
     if (fmaxf(fmaxf(fabsf(x), fabsf(y)), fabsf(z)) > 0.f) {
-        p[0] = x * P[0] + y * P[1] + z * P[2] + P[3];
-        p[1] = x * P[4] + y * P[5] + z * P[6] + P[7];
-        p[2] = x * P[8] + y * P[9] + z * P[10] + P[11];
+        transform_point(P, make_float4(x, y, z, 0.f), p);
         return true;
     }
     return false;
@@ -154,7 +152,7 @@ __global__ void model_zbuf_kernel(const float* __restrict__ vmaps, const float* 
         if (!model_point(vmaps + (size_t)((head + k) % slots) * 3 * hw, poses + 16 * k, hw, src, p)) continue;
         int pix;
         float r;
-        if (project_to_pixel(p[0], p[1], p[2], pc, pix, r) && pix >= pix_lo && pix < pix_hi) {
+        if (project_to_pixel(p[0], p[1], p[2], pc, pix, r, RangeOrder::kYFirst) && pix >= pix_lo && pix < pix_hi) {
             unsigned long long key = ((unsigned long long)__float_as_uint(r) << 32) | (unsigned long long)(uint32_t)src;
             atomicMin(&zbuf[k * hw + pix], key);
         }
@@ -193,6 +191,21 @@ __device__ __forceinline__ void load_T(const float* __restrict__ T, float* sT) {
     __syncthreads();
 }
 
+// Query i, moved by the pose T (null: where it stands), into the closest-wins z-buffer of the pixels [pix_lo, pix_hi).
+// Every query z-buffer (single, batched and per hypothesis) is built here, so they all get the same winners.
+__device__ __forceinline__ void query_zbuf_insert(const float4& p0, int64_t i, const float* T, const ProjConst& pc, int pix_lo,
+                                                  int pix_hi, unsigned long long* __restrict__ zbuf) {
+    float p[3] = {p0.x, p0.y, p0.z};
+    if (T) transform_point(T, p0, p);
+    int pix;
+    float r;
+    // x first, unlike the other z-buffers: the order these z-buffers have always been built with
+    if (project_to_pixel(p[0], p[1], p[2], pc, pix, r, RangeOrder::kXFirst) && pix >= pix_lo && pix < pix_hi) {
+        unsigned long long key = ((unsigned long long)__float_as_uint(r) << 32) | (unsigned long long)(uint32_t)i;
+        atomicMin(&zbuf[pix], key);
+    }
+}
+
 // The kernels of an ICP iteration below are __device__ bodies with two entry points each: the kernel of one sequence,
 // which passes blockIdx.x / gridDim.x and its arguments, and the *_batch_kernel of pls_process_frames, whose blockIdx.y
 // picks a sequence's descriptor (ProjSeq) and which passes that sequence's own block count.  A body reads no blockIdx.x
@@ -205,21 +218,8 @@ __device__ __forceinline__ void query_zbuf_body(const float4* __restrict__ queri
     __shared__ float sT[12];
     if (T) load_T(T, sT);
     const int64_t nq = nq_dev ? (int64_t)*nq_dev : nq_host;
-    for (int64_t i = (int64_t)block * blockDim.x + threadIdx.x; i < nq; i += (int64_t)grid * blockDim.x) {
-        const float4 p0 = queries[i];
-        float p[3] = {p0.x, p0.y, p0.z};
-        if (T) {
-            p[0] = p0.x * sT[0] + p0.y * sT[1] + p0.z * sT[2] + sT[3];
-            p[1] = p0.x * sT[4] + p0.y * sT[5] + p0.z * sT[6] + sT[7];
-            p[2] = p0.x * sT[8] + p0.y * sT[9] + p0.z * sT[10] + sT[11];
-        }
-        int pix;
-        float r;
-        if (project_to_pixel(p[0], p[1], p[2], pc, pix, r) && pix >= pix_lo && pix < pix_hi) {
-            unsigned long long key = ((unsigned long long)__float_as_uint(r) << 32) | (unsigned long long)(uint32_t)i;
-            atomicMin(&zbuf[pix], key);
-        }
-    }
+    for (int64_t i = (int64_t)block * blockDim.x + threadIdx.x; i < nq; i += (int64_t)grid * blockDim.x)
+        query_zbuf_insert(queries[i], i, T ? sT : nullptr, pc, pix_lo, pix_hi, zbuf);
 }
 
 __global__ void query_zbuf_kernel(const float4* __restrict__ queries, const uint32_t* __restrict__ nq_dev, int64_t nq_host,
@@ -240,11 +240,9 @@ __device__ __forceinline__ void query_resolve_body(unsigned long long* __restric
         zbuf[pix] = ~0ull;  // leave the z-buffer cleared for the next iteration (no separate memset)
         float4 o = make_float4(0.f, 0.f, 0.f, 0.f);
         if (key != ~0ull) {
-            const float4 p0 = queries[(uint32_t)(key & 0xffffffffull)];
-            o.x = p0.x * sT[0] + p0.y * sT[1] + p0.z * sT[2] + sT[3];
-            o.y = p0.x * sT[4] + p0.y * sT[5] + p0.z * sT[6] + sT[7];
-            o.z = p0.x * sT[8] + p0.y * sT[9] + p0.z * sT[10] + sT[11];
-            o.w = 1.f;
+            float p[3];
+            transform_point(sT, queries[(uint32_t)(key & 0xffffffffull)], p);
+            o = make_float4(p[0], p[1], p[2], 1.f);
         }
         tgt[pix] = o;
     }
@@ -327,11 +325,8 @@ proj_icp_iter_kernel(const float* __restrict__ model_v, const float4* __restrict
          pix += (int64_t)gridDim.x * blockDim.x) {
         const unsigned long long key = zbuf[pix];
         if (key == ~0ull) continue;
-        const float4 p0 = queries[(uint32_t)(key & 0xffffffffull)];
         float p[3], q[3], n[3];
-        p[0] = p0.x * sT[0] + p0.y * sT[1] + p0.z * sT[2] + sT[3];
-        p[1] = p0.x * sT[4] + p0.y * sT[5] + p0.z * sT[6] + sT[7];
-        p[2] = p0.x * sT[8] + p0.y * sT[9] + p0.z * sT[10] + sT[11];
+        transform_point(sT, queries[(uint32_t)(key & 0xffffffffull)], p);
         if (!pixel_argmin(model_v, model_n, K, kcap, pix, p, q, n)) continue;
         float J[6];
         const float r = p2plane_residual_jacobian_identity(p, q, n, J);
@@ -568,35 +563,8 @@ proj_icp_tma_kernel(const float* __restrict__ model_v, const float4* __restrict_
 // target maps `tgts`, and the h-th `part_rows`-double range of the partial rows; the scan's queries and the model are
 // shared.  Every hypothesis's arithmetic is its single call's (projmap_icp_iteration), so it gets that call's bits.
 
-// project_to_pixel with the range rounded as query_zbuf_kernel's compiled code rounds it, sqrt(fma(z, z, fma(y, y, x x))):
-// a range one ulp off can change a z-buffer winner.  The compiler is free to contract x x + y y + z z either way, and does
-// so differently in different kernels, so the roundings here and in query_zbuf_hyp_kernel's transform are spelled out
-// from the SASS of query_zbuf_kernel as this compiler builds it.  CONDITION: they must stay equal to that kernel's.  If a
-// compiler contracts query_zbuf_kernel differently, these lines must follow it; nothing but the GPU bit-identity tests
-// of pls_register_hypotheses (tests/test_proj_hypotheses_gpu.py) would notice.
-__device__ __forceinline__ bool project_to_pixel_zbuf(float x, float y, float z, const ProjConst& pc, int& pix, float& r_out) {
-    const float kPi = 3.14159274101257324f;
-    const float r = __fsqrt_rn(__fmaf_rn(z, z, __fmaf_rn(y, y, __fmul_rn(x, x))));
-    r_out = r;
-    const bool null = (r == 0.0f);
-    const float rr = null ? 0.001f : r;
-    const float theta = -atan2f(y, x);
-    const float phi = asinf(__fdiv_rn(z, rr));
-    float c = __fmul_rn(0.5f, __fadd_rn(__fdiv_rn(theta, kPi), 1.0f));
-    float rw = __fsub_rn(1.0f, __fdiv_rn(__fadd_rn(phi, pc.abs_down), pc.fov));
-    c = __fmul_rn(c, pc.Wf);
-    rw = __fmul_rn(rw, pc.Hf);
-    const float row = null ? -1.0f : rw, col = null ? -1.0f : c;
-    const float pr = rintf(row), pcn = rintf(col);
-    const bool ok = (pr >= 0.0f) && (pr <= (float)(pc.H - 1)) && (pcn >= 0.0f) && (pcn <= (float)(pc.W - 1)) && (r > 0.0f);
-    if (!ok) return false;
-    pix = (int)pr * pc.W + (int)pcn;
-    return true;
-}
-
 // Each query is loaded once and z-buffered into the z-buffer of every live hypothesis, transformed by that hypothesis's
-// pose with query_zbuf_kernel's roundings (fma(z, T2, fma(x, T0, y T1)) + T3 per row, as its compiled code does; the
-// CONDITION above).  The 64-bit atomic-min keys make every z-buffer the one its single call builds, whatever the order.
+// pose.  The 64-bit atomic-min keys make every z-buffer the one its single call builds, whatever the order.
 __global__ void __launch_bounds__(256)
 query_zbuf_hyp_kernel(const float4* __restrict__ queries, const uint32_t* __restrict__ nq_dev,
                       const FrameResult* __restrict__ frs, int num, ProjConst pc, int64_t hw,
@@ -618,20 +586,7 @@ query_zbuf_hyp_kernel(const float4* __restrict__ queries, const uint32_t* __rest
     const int64_t nq = (int64_t)*nq_dev;
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < nq; i += (int64_t)gridDim.x * blockDim.x) {
         const float4 p0 = queries[i];
-        for (int j = 0; j < nl; ++j) {
-            const float* T = sT[j];
-            float p[3];
-#pragma unroll
-            for (int c = 0; c < 3; ++c)
-                p[c] = __fadd_rn(__fmaf_rn(p0.z, T[4 * c + 2], __fmaf_rn(p0.x, T[4 * c], __fmul_rn(p0.y, T[4 * c + 1]))),
-                                 T[4 * c + 3]);
-            int pix;
-            float r;
-            if (project_to_pixel_zbuf(p[0], p[1], p[2], pc, pix, r)) {
-                unsigned long long key = ((unsigned long long)__float_as_uint(r) << 32) | (unsigned long long)(uint32_t)i;
-                atomicMin(&zbufs[(size_t)live[j] * hw + pix], key);
-            }
-        }
+        for (int j = 0; j < nl; ++j) query_zbuf_insert(p0, i, sT[j], pc, 0, (int)hw, zbufs + (size_t)live[j] * hw);
     }
 }
 

@@ -40,9 +40,7 @@ __device__ __forceinline__ bool moved_point(const float* __restrict__ vm, int64_
     p[0] = vm[i]; p[1] = vm[hw + i]; p[2] = vm[2 * hw + i];
     // mask_vm = (|p| != 0); the null point stays null after the transform (loss_modules.py:79-83)
     if (p[0] == 0.f && p[1] == 0.f && p[2] == 0.f) return false;
-    pm[0] = p[0] * sT[0] + p[1] * sT[1] + p[2] * sT[2] + sT[3];
-    pm[1] = p[0] * sT[4] + p[1] * sT[5] + p[2] * sT[6] + sT[7];
-    pm[2] = p[0] * sT[8] + p[1] * sT[9] + p[2] * sT[10] + sT[11];
+    transform_point(sT, make_float4(p[0], p[1], p[2], 0.f), pm);
     return true;
 }
 
@@ -58,7 +56,8 @@ loss_zbuf_kernel(const float* __restrict__ vm_target, const float* __restrict__ 
         if (!moved_point(vm, hw, i, sT, p, pm)) continue;
         int pix;
         float r;
-        if (project_to_pixel(pm[0], pm[1], pm[2], pc, pix, r))
+        // the order loss_accumulate_kernel finds each pixel's winner with
+        if (project_to_pixel(pm[0], pm[1], pm[2], pc, pix, r, RangeOrder::kYFirst))
             atomicMin(&zbuf[hw * (size_t)b + pix], ((unsigned long long)__float_as_uint(r) << 32) | (unsigned long long)(uint32_t)i);
     }
 }
@@ -81,7 +80,7 @@ loss_accumulate_kernel(const float* __restrict__ vm_target, const float* __restr
         if (!moved_point(vm, hw, i, sT, p, pm)) continue;
         int pix;
         float r;
-        if (!project_to_pixel(pm[0], pm[1], pm[2], pc, pix, r)) continue;
+        if (!project_to_pixel(pm[0], pm[1], pm[2], pc, pix, r, RangeOrder::kYFirst)) continue;  // loss_zbuf_kernel's order
         const uint32_t win = (uint32_t)(zbuf[hw * (size_t)b + pix] & 0xffffffffull);
         float pw[3] = {pm[0], pm[1], pm[2]};
         if (win != (uint32_t)i) {
