@@ -362,6 +362,34 @@ PLS_API int pls_register_hypotheses(pls_context* ctx, const float* points, int64
 PLS_API int pls_register_scans(pls_context* ctx, const float* const* scans, const int64_t* n, int S,
                                const int* scan_of, const float* T0s, int B, float* out_T, float* out_params,
                                float* out_losses, int* out_iters, int* out_status);
+/* The quality of B registrations on the kd map ctx holds, in one call (no reference counterpart: a localiser that feeds
+ * a filter or a pose graph needs each registration's inlier fraction, inlier RMSE and information matrix, and a
+ * re-ranking of pose candidates needs more than an occupancy score).  Arguments, staging and pointer rules are those
+ * of pls_register_scans: scans[s] [n[s],3] float32, host or device; scan_of [B] (NULL: b -> b, which needs B == S);
+ * T [B,16] the poses, host or device.  For pose b and scan s = scan_of[b]:
+ *   P         the valid rows of scan s (those pack_valid_rows keeps: no NaN coordinate);
+ *   p'        transform_point(T_b, p) for p in P; q its exact 1-NN in the map and n_q q's cached normal -- the match and
+ *             normal of the first ICP iteration of pls_register_frame(scan s, T_b);
+ *   r, J, w   the residual, Jacobian [n, p' x n] and weight of that iteration (the context's scheme and sigma);
+ *   d^2       ((dx dx + dy dy) + dz dz) in float64, dx = (double)p'_x - (double)q_x (likewise y, z), every operation
+ *             rounded on its own: numpy's element-wise float64 expressions give the same bits;
+ *   inlier    a matched query with d^2 <= max_distance * max_distance (float64); max_distance = +inf admits every match.
+ * out_stats [B,PLS_EVAL_STATS] (host or device), row b: [0..29] the accumulators of pls_kdmap_last_correspondences's
+ * layout (21 JtJ upper, 6 Jtr, sum (w r)^2, sum r^2, count) over the inliers only; [30] sum d^2 over the inliers;
+ * [31] |P|.  With max_distance = +inf, [0..29] are bit for bit the out_sums pls_kdmap_last_correspondences reports
+ * after pls_register_frame(scan s, T_b) with max_num_alignments = 1 on the same map.  Row b does not depend on B, on
+ * b's place in the batch or on the other scans: a batch equals B single-pose calls bit for bit.
+ * Nothing is solved.  The map, its index, its frame counts and the odometry state are unchanged (the normal cache may
+ * fill, with the bits it would get anyway); afterwards the last pose is the context's last search, as
+ * pls_register_scans leaves it, with its row's [0..29] as the last sums (pls_kdmap_last_correspondences,
+ * pls_last_icp_sums).  One launch packs every scan; each kernel is one launch for up to PLS_MAX_SEQUENCES poses, larger B
+ * runs in chunks of that many.  PLS_E_INVALID before any work, the context unchanged: a projective map, a communicator,
+ * a map that has had no update, S or B <= 0, an n[s] <= 0, a scan_of entry outside [0, S), a NULL scans, n, scan, T or
+ * out_stats, or a max_distance that is NaN or negative. */
+#define PLS_EVAL_STATS 32
+PLS_API int pls_kdmap_evaluate_poses(pls_context* ctx, const float* const* scans, const int64_t* n, int S,
+                                     const int* scan_of, const float* T, int B, double max_distance,
+                                     double* out_stats);
 /* ICPFrameToModel.do_process_next_frame (icp_odometry.py:157-246): `data` is [n,3] points
  * (PLS_INPUT_NDARRAY / PLS_INPUT_TENSOR: float; the _F64 variants: double) or a float [3,H,W] vertex map
  * (PLS_INPUT_VERTEX_MAP, n ignored).  init_pose [16] or NULL (identity).  On frame 0 the map is initialised and

@@ -19,6 +19,7 @@ MAP_KDTREE, MAP_PROJECTIVE = 0, 1
 INPUT_NDARRAY, INPUT_TENSOR, INPUT_VERTEX_MAP, INPUT_NDARRAY_F64, INPUT_TENSOR_F64 = 0, 1, 2, 3, 4
 PTR_DEVICE, PTR_HOST = 0x100, 0x200  # residency hints OR-ed into a layout
 MAX_SEQUENCES = 64  # PLS_MAX_SEQUENCES: contexts one pls_process_frames call advances
+EVAL_STATS = 32  # PLS_EVAL_STATS: doubles per pose of pls_kdmap_evaluate_poses
 
 
 class PlsConfig(C.Structure):
@@ -86,6 +87,7 @@ _SIGNATURES = {
     "pls_register_frame": [_P, _P, _L, _P, _P, _P, _P, C.POINTER(_I)],
     "pls_register_hypotheses": [_P, _P, _L, _P, _I, _P, _P, _P, _P, _P],
     "pls_register_scans": [_P, _P, _P, _I, _P, _P, _I, _P, _P, _P, _P, _P],
+    "pls_kdmap_evaluate_poses": [_P, _P, _P, _I, _P, _P, _I, _D, _P],
     "pls_process_frame": [_P, _P, _I, _L, _P, _P, _P, C.POINTER(_I), _P],
     "pls_process_frame_grid_sample": [_P, _P, _L, _D, _I, _P, _P, _P, C.POINTER(_I), _P],
     "pls_process_frames": [_P, _I, _P, _P, _P, _D, _P, _P, _P, _P, _P, _P],

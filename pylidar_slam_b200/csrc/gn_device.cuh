@@ -127,17 +127,18 @@ __device__ __forceinline__ void accumulate_normal_equations(double* acc, const T
     acc[29] += 1.0;
 }
 
-// Warp-shuffle + shared-memory block reduction of the 30 accumulators; thread a < 30 of the
-// block writes the block total of accumulator a to out[a].  Only the first WARPS warps hold accumulators (a block
-// whose extra warps only search skips them); every thread of the block must call.
-template <int THREADS, int WARPS = THREADS / 32>
+// Warp-shuffle + shared-memory block reduction of the N (30, or PLS_EVAL_STATS for the evaluation's rows) accumulators;
+// thread a < N of the block writes the block total of accumulator a to out[a].  Only the first WARPS warps hold
+// accumulators (a block whose extra warps only search skips them); every thread of the block must call.
+template <int THREADS, int WARPS = THREADS / 32, int N = NACC_DEV>
 __device__ __forceinline__ void block_reduce_store(double* acc, double* out) {
     static_assert(WARPS >= 1 && WARPS <= THREADS / 32, "block_reduce_store: warps");
-    __shared__ double red[WARPS][NACC_DEV];
+    static_assert(N >= 1 && N <= 32, "block_reduce_store: one warp of accumulators");
+    __shared__ double red[WARPS][N];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     if (WARPS == THREADS / 32 || warp < WARPS) {  // warp-uniform; always true (no branch) when every warp holds some
 #pragma unroll
-        for (int a = 0; a < NACC_DEV; ++a) {
+        for (int a = 0; a < N; ++a) {
             double v = acc[a];
 #pragma unroll
             for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -145,7 +146,7 @@ __device__ __forceinline__ void block_reduce_store(double* acc, double* out) {
         }
     }
     __syncthreads();
-    if (threadIdx.x < NACC_DEV) {
+    if (threadIdx.x < N) {
         double s = 0.0;
 #pragma unroll
         for (int w = 0; w < WARPS; ++w) s += red[w][threadIdx.x];

@@ -37,13 +37,15 @@ __device__ __forceinline__ void split_stamp(unsigned long long* rec, int i, doub
 // eight sums the rows w, w+8, ... of every accumulator (lane = accumulator, so a row is one coalesced 240-byte read and
 // the loads of a lane are independent), then the eight slices are added in fixed order -- the same additions in the
 // same order whatever the block size (a 128-thread block gives two slices to each warp, a 512-thread block none to
-// its last eight).
-template <int THREADS = 256>
+// its last eight).  N: the accumulators per row (NACC, or PLS_EVAL_STATS for pls_kdmap_evaluate_poses's rows), each
+// summed exactly as NACC-wide rows sum it.
+template <int THREADS = 256, int N = NACC>
 __device__ __forceinline__ void sum_partials_256(const double* __restrict__ partials, int num_blocks, double* sums) {
     static_assert(THREADS == 512 || THREADS == 256 || THREADS == 128, "sum_partials: 4, 8 or 16 warps");
-    __shared__ double slice_sum[8][NACC];
+    static_assert(N >= 1 && N <= 32, "sum_partials: a lane per accumulator");
+    __shared__ double slice_sum[8][N];
     const int a = threadIdx.x & 31;
-    if (a < NACC) {
+    if (a < N) {
         for (int slice = threadIdx.x >> 5; slice < 8; slice += THREADS / 32) {
             // sixteen rows in flight per lane (the additions keep their order; a missing row adds +0.0): the sum of a
             // few hundred rows is a chain of L2 round trips otherwise
@@ -53,7 +55,7 @@ __device__ __forceinline__ void sum_partials_256(const double* __restrict__ part
 #pragma unroll
                 for (int j = 0; j < 16; ++j) {
                     const int b = b0 + 8 * j;
-                    v[j] = b < num_blocks ? __ldcg(partials + (size_t)b * NACC + a) : 0.0;
+                    v[j] = b < num_blocks ? __ldcg(partials + (size_t)b * N + a) : 0.0;
                 }
 #pragma unroll
                 for (int j = 0; j < 16; ++j) s += v[j];
@@ -62,7 +64,7 @@ __device__ __forceinline__ void sum_partials_256(const double* __restrict__ part
         }
     }
     __syncthreads();
-    if (threadIdx.x < NACC) {
+    if (threadIdx.x < N) {
         double s = 0.0;
 #pragma unroll
         for (int k = 0; k < 8; ++k) s += slice_sum[k][threadIdx.x];

@@ -465,6 +465,10 @@ struct KdScan {
 void kdmap_hypotheses_begin(pls_context* ctx, const KdScan* scans, int num, cudaStream_t st, int* grid, FrameResult** frs,
                             uint32_t** words);
 void kdmap_hypothesis_adopt(pls_context* ctx, const KdScan& scan, int h, cudaStream_t st);
+// pls_kdmap_evaluate_poses: after kdmap_hypotheses_begin and the registrations' start at their poses, iteration 0's
+// 1-NN and normals, then the residual pass gated by max_d2 and no solve; registration h's row of PLS_EVAL_STATS
+// doubles into out[PLS_EVAL_STATS h] (device), its entries 0..29 also into its FrameResult's last_sums.  Enqueued on st.
+void kdmap_evaluate_batch(pls_context* ctx, int num, cudaStream_t st, const int* grid, double max_d2, double* out);
 // pls_register_scans: one scan to pack, its device rows [n,3] (n > 0) and where its valid rows and their count go.
 struct KdScanRows {
     const float* rows;

@@ -448,9 +448,9 @@ __device__ __forceinline__ void accumulate_match(double* acc, const KdIndex& ix,
 }
 
 // The end of a residual phase, called by every thread of a THREADS-thread block whose first KD_WARPS warps hold
-// accumulators: the block partial row `block`, then (fuse_threshold >= 0) the fixed-order sum of the `grid` rows and the
-// solve in the last block to arrive.
-template <int THREADS>
+// accumulators: the block partial row `block` of W accumulators, then (NACC-wide rows, fuse_threshold >= 0) the
+// fixed-order sum of the `grid` rows and the solve in the last block to arrive.
+template <int THREADS, int W = NACC>
 __device__ __forceinline__ void block_partial_and_finish(double* acc, FrameResult* fr, double* __restrict__ partials,
                                                          float fuse_threshold, unsigned block, unsigned grid KD_SPLIT_ARG) {
     KD_SPLIT_MAX(1, acc[0] + acc[29]);
@@ -458,9 +458,10 @@ __device__ __forceinline__ void block_partial_and_finish(double* acc, FrameResul
     // loop at different iterations; without this it took the divergent-warp path of the 30 x 5 shuffles, 35 us on H100
     // (profiles/h100_kd_residual_split_before.log) while every other block took 1.2 us -- and the solve waits for it.
     __syncwarp();
-    block_reduce_store<THREADS, KD_WARPS>(acc, partials + (size_t)block * NACC);
+    block_reduce_store<THREADS, KD_WARPS, W>(acc, partials + (size_t)block * W);
     KD_SPLIT_BLOCK_MAX()
-    if (fuse_threshold >= 0.f) icp_finish_in_last_block<THREADS>(fr, partials, (int)grid, fuse_threshold PLS_SPLIT_PASS);
+    if constexpr (W == NACC)
+        if (fuse_threshold >= 0.f) icp_finish_in_last_block<THREADS>(fr, partials, (int)grid, fuse_threshold PLS_SPLIT_PASS);
 }
 
 // Iterations after a frame's first on maps of KD_COLD_MAP_POINTS or more: a thread per query keeps its previous match
@@ -669,32 +670,61 @@ kd_normals_wide_kernel(KdIndex ix, int k_normals, const int* __restrict__ workli
     kd_normals_warp_body<R>(ix, k_normals, worklist, wl_count, done, counters, blockIdx.x, gridDim.x);
 }
 
+// The squared distance of a transformed query p to its match q in float64, every operation rounded on its own (no
+// contraction): ((dx dx + dy dy) + dz dz), dx = (double)p_x - (double)q_x -- numpy's element-wise float64 bits.
+__device__ __forceinline__ double match_d2_f64(const float* p, const float4& q) {
+    const double dx = __dsub_rn((double)p[0], (double)q.x);
+    const double dy = __dsub_rn((double)p[1], (double)q.y);
+    const double dz = __dsub_rn((double)p[2], (double)q.z);
+    return __dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz));
+}
+
 // A thread per query: accumulate_match -> block partials; the last block sums them in fixed order and runs the solve,
 // stop test and pose update.
+// EVAL (pls_kdmap_evaluate_poses, launched with fuse_threshold < 0: no solve): only the matches with
+// match_d2_f64 <= max_d2 are accumulated, their d^2 summed in acc[NACC], and every query is counted in acc[NACC + 1];
+// the block partial rows are PLS_EVAL_STATS wide.  The ICP instantiation (EVAL = false) is the same code as before.
+// kd_residual_body's pose.  Owned by this function rather than by the template, so that the module's shared variables
+// keep the order they had before kd_residual_body took EVAL: the ICP kernels keep their shared-memory layout and SASS
+// (profiles/sass_evaluate_poses_census.log).
+__device__ __forceinline__ float* kd_residual_pose() {
+    __shared__ float sT[12];
+    return sT;
+}
+
+template <bool EVAL = false>
 __device__ __forceinline__ void kd_residual_body(const KdIndex& ix, const float4* __restrict__ queries,
                                                  const uint32_t* __restrict__ nq_dev, int64_t q_begin, int64_t q_stride,
                                                  FrameResult* fr, int scheme, float sigma, const int* __restrict__ match,
                                                  double* __restrict__ partials, float fuse_threshold, unsigned block,
-                                                 unsigned grid KD_SPLIT_ARG) {
+                                                 unsigned grid, double max_d2 KD_SPLIT_ARG) {
+    static_assert(PLS_EVAL_STATS == NACC + 2, "evaluation rows: the 30 accumulators, sum d^2, |P|");
+    constexpr int W = EVAL ? PLS_EVAL_STATS : NACC;
     if (fr->done) return;
-    __shared__ float sT[12];
+    float* sT = kd_residual_pose();
     if (threadIdx.x < 12) sT[threadIdx.x] = fr->T[threadIdx.x];
     __syncthreads();
     if (threadIdx.x == 0) PLS_SPLIT(1);
     const int64_t nq = (int64_t)*nq_dev;
-    double acc[NACC];
+    double acc[W];
 #pragma unroll
-    for (int a = 0; a < NACC; ++a) acc[a] = 0.0;
+    for (int a = 0; a < W; ++a) acc[a] = 0.0;
     for (int64_t s = (int64_t)block * blockDim.x + threadIdx.x;; s += (int64_t)grid * blockDim.x) {
         const int64_t qi = q_begin + s * q_stride;
         if (qi >= nq) break;
         float p[3];
         transform_point(sT, queries[qi], p);
         const int pos = match[qi];
+        if constexpr (EVAL) acc[NACC + 1] += 1.0;
         if (pos < 0) continue;
+        if constexpr (EVAL) {
+            const double d2 = match_d2_f64(p, __ldg(ix.sorted + pos));
+            if (!(d2 <= max_d2)) continue;
+            acc[NACC] += d2;
+        }
         accumulate_match(acc, ix, p, pos, scheme, sigma KD_SPLIT_PASS);
     }
-    block_partial_and_finish<KD_THREADS>(acc, fr, partials, fuse_threshold, block, grid KD_SPLIT_PASS);
+    block_partial_and_finish<KD_THREADS, W>(acc, fr, partials, fuse_threshold, block, grid KD_SPLIT_PASS);
 }
 
 __global__ void __launch_bounds__(KD_THREADS)
@@ -707,7 +737,7 @@ kd_residual_kernel(KdIndex ix, const float4* __restrict__ queries, const uint32_
     if (blockIdx.x >= grid) return;
     KD_SPLIT_BEGIN()
     kd_residual_body(ix, queries, nq_dev, q_begin, q_stride, fr, scheme, sigma, match, partials, fuse_threshold, blockIdx.x,
-                     grid KD_SPLIT_PASS);
+                     grid, 0.0 KD_SPLIT_PASS);
 }
 
 // ICP iterations after a frame's first, in ONE launch.  Each block takes the queries kd_residual_kernel would give it
@@ -913,7 +943,29 @@ __global__ void __launch_bounds__(KD_THREADS) kd_residual_batch_kernel(const KdS
     if ((int)blockIdx.x >= s.blocks || !four_launch_step(s, it)) return;
     KD_SPLIT_NONE()
     kd_residual_body(s.ix, s.queries, s.nq_dev, 0, 1, s.fr, s.scheme, s.sigma, s.match, s.partials, s.fuse_threshold,
-                     blockIdx.x, s.blocks KD_SPLIT_PASS);
+                     blockIdx.x, s.blocks, 0.0 KD_SPLIT_PASS);
+}
+
+// pls_kdmap_evaluate_poses: iteration 0's residual pass of every registration at its FrameResult's pose, gated by
+// max_d2, with no solve (kd_residual_body<true>).
+__global__ void __launch_bounds__(KD_THREADS) kd_evaluate_batch_kernel(const KdSeq* __restrict__ seqs, double max_d2) {
+    __shared__ KdSeq s;
+    load_seq(seqs, s);
+    if ((int)blockIdx.x >= s.blocks) return;
+    KD_SPLIT_NONE()
+    kd_residual_body<true>(s.ix, s.queries, s.nq_dev, 0, 1, s.fr, s.scheme, s.sigma, s.match, s.partials, -1.f, blockIdx.x,
+                           s.blocks, max_d2 KD_SPLIT_PASS);
+}
+
+// Registration blockIdx.x's row: its block partials summed in the fixed order of icp_finish_in_last_block, into
+// out[PLS_EVAL_STATS * blockIdx.x], and entries 0..29 into its FrameResult's last_sums.
+__global__ void __launch_bounds__(256) kd_evaluate_finish_kernel(const KdSeq* __restrict__ seqs, double* __restrict__ out) {
+    __shared__ double sums[PLS_EVAL_STATS];
+    const KdSeq* s = seqs + blockIdx.x;
+    sum_partials_256<256, PLS_EVAL_STATS>(s->partials, s->blocks, sums);
+    __syncthreads();
+    if (threadIdx.x < PLS_EVAL_STATS) out[(size_t)PLS_EVAL_STATS * blockIdx.x + threadIdx.x] = sums[threadIdx.x];
+    if (threadIdx.x < NACC) s->fr->last_sums[threadIdx.x] = sums[threadIdx.x];
 }
 
 // Iteration `it` (>= 1) of every sequence that has not reached its max_iters and whose later iterations take one launch.
@@ -1532,6 +1584,21 @@ void kdmap_batch_begin(pls_context* lead, pls_context* const* ctxs, const int64_
 // launch per kernel for all of them.  A later iteration is kd_icp_refine_batch_kernel for the sequences whose later
 // iterations take one launch and the four launches verify / 1-NN / normals / residual for the others; the normals of a
 // wide k are one more launch, made only if some sequence has one.  No launch grows with num.
+// The 1-NN and normals launches of iteration `it` of the four-launch path for the sequences described in seqs.
+static void batch_search(const KdSeq* seqs, int num, cudaStream_t st, const int* grid, int it) {
+    kd_nn_warp_batch_kernel<<<dim3(grid[1], num), KD_THREADS, 0, st>>>(seqs, it);
+    PLS_CHECK_LAUNCH();
+    kd_normals_warp_batch_kernel<<<dim3(grid[2], num), KD_THREADS, 0, st>>>(seqs, it);
+    PLS_CHECK_LAUNCH();
+    if (grid[5]) {
+        const dim3 g(grid[2], num);
+        if (grid[5] == 2) kd_normals_wide_batch_kernel<2><<<g, KD_THREADS, 0, st>>>(seqs, it);
+        else if (grid[5] == 4) kd_normals_wide_batch_kernel<4><<<g, KD_THREADS, 0, st>>>(seqs, it);
+        else kd_normals_wide_batch_kernel<8><<<g, KD_THREADS, 0, st>>>(seqs, it);
+        PLS_CHECK_LAUNCH();
+    }
+}
+
 void kdmap_batch_iterations(pls_context* lead, int num, cudaStream_t st, const int* grid, int first, int last) {
     const KdSeq* seqs = lead->batch_buf.as<KdSeq>();
     for (int it = first; it < last; ++it) {
@@ -1544,20 +1611,21 @@ void kdmap_batch_iterations(pls_context* lead, int num, cudaStream_t st, const i
             kd_nn_verify_batch_kernel<<<dim3(grid[3], num), KD_THREADS, 0, st>>>(seqs, it);
             PLS_CHECK_LAUNCH();
         }
-        kd_nn_warp_batch_kernel<<<dim3(grid[1], num), KD_THREADS, 0, st>>>(seqs, it);
-        PLS_CHECK_LAUNCH();
-        kd_normals_warp_batch_kernel<<<dim3(grid[2], num), KD_THREADS, 0, st>>>(seqs, it);
-        PLS_CHECK_LAUNCH();
-        if (grid[5]) {
-            const dim3 g(grid[2], num);
-            if (grid[5] == 2) kd_normals_wide_batch_kernel<2><<<g, KD_THREADS, 0, st>>>(seqs, it);
-            else if (grid[5] == 4) kd_normals_wide_batch_kernel<4><<<g, KD_THREADS, 0, st>>>(seqs, it);
-            else kd_normals_wide_batch_kernel<8><<<g, KD_THREADS, 0, st>>>(seqs, it);
-            PLS_CHECK_LAUNCH();
-        }
+        batch_search(seqs, num, st, grid, it);
         kd_residual_batch_kernel<<<dim3(grid[0], num), KD_THREADS, 0, st>>>(seqs, it);
         PLS_CHECK_LAUNCH();
     }
+}
+
+// pls_kdmap_evaluate_poses: iteration 0's search of the registrations kdmap_hypotheses_begin described (started at
+// their poses), then their gated residual pass and their rows into out [num, PLS_EVAL_STATS] (device), on st.
+void kdmap_evaluate_batch(pls_context* ctx, int num, cudaStream_t st, const int* grid, double max_d2, double* out) {
+    const KdSeq* seqs = ctx->batch_buf.as<KdSeq>();
+    batch_search(seqs, num, st, grid, 0);
+    kd_evaluate_batch_kernel<<<dim3(grid[0], num), KD_THREADS, 0, st>>>(seqs, max_d2);
+    PLS_CHECK_LAUNCH();
+    kd_evaluate_finish_kernel<<<num, 256, 0, st>>>(seqs, out);
+    PLS_CHECK_LAUNCH();
 }
 
 // pls_register_hypotheses / pls_register_scans: the ICP state of `num` registrations on ctx's map, registration h of
@@ -1581,8 +1649,9 @@ void kdmap_hypotheses_begin(pls_context* ctx, const KdScan* scans, int num, cuda
         plans.push_back(plan_kd_iteration(ctx, scans[h].bound, 1));
         const KdPlan& p = plans.back();
         offs.push_back(total);
+        // partial rows wide enough for pls_kdmap_evaluate_poses's (PLS_EVAL_STATS >= NACC)
         total += up((size_t)scans[h].bound * sizeof(int)) + up(p.slots * sizeof(float4)) + up(2 * p.slots * sizeof(int)) +
-                 up((size_t)p.blocks * NACC * sizeof(double));
+                 up((size_t)p.blocks * PLS_EVAL_STATS * sizeof(double));
     }
     ctx->hyp_buf.reserve(total, st);
     char* base = ctx->hyp_buf.as<char>();

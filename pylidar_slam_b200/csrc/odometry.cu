@@ -1055,6 +1055,43 @@ static void register_batch(pls_context* ctx, const KdScan* scans, int64_t n, con
     if (!out_status) raise_status(ctx, first_error);
 }
 
+// pls_register_scans / pls_kdmap_evaluate_poses: the S scans staged (host scans back to back, as to_device stages one)
+// and packed into ctx->queries by one launch; returns the scan each of the B registrations reads.
+static std::vector<KdScan> stage_scans(pls_context* ctx, const float* const* scans, const int64_t* n, int S,
+                                       const int* scan_of, int B) {
+    cudaStream_t st = ctx->stream;
+    size_t host_rows = 0;
+    for (int s = 0; s < S; ++s)
+        if (!is_device_ptr(scans[s])) host_rows += (size_t)n[s];
+    if (host_rows) ctx->stage_in[0].reserve(host_rows * 3 * sizeof(float), st);
+    // scan s's packed rows go to ctx->queries at the sum of the earlier scans' row counts, the S counts behind them
+    size_t rows = 0;
+    for (int s = 0; s < S; ++s) rows += (size_t)n[s];
+    ctx->queries.reserve(rows * sizeof(float4) + (size_t)S * sizeof(uint32_t), st);
+    float4* q = ctx->queries.as<float4>();
+    uint32_t* counts = reinterpret_cast<uint32_t*>(q + rows);
+    std::vector<KdScanRows> pack((size_t)S);
+    std::vector<KdScan> packed((size_t)S);
+    float* staged = ctx->stage_in[0].as<float>();
+    for (int s = 0; s < S; ++s) {
+        const float* d = scans[s];
+        if (!is_device_ptr(d)) {
+            PLS_CUDA(cudaMemcpyAsync(staged, d, (size_t)n[s] * 3 * sizeof(float), cudaMemcpyHostToDevice, st));
+            d = staged;
+            staged += (size_t)n[s] * 3;
+        }
+        pack[(size_t)s] = KdScanRows{d, n[s], q, counts + s};
+        packed[(size_t)s] = KdScan{q, counts + s, n[s]};
+        q += n[s];
+    }
+    FrameResult* fr = frame_result_dev(ctx);
+    PLS_CUDA(cudaMemsetAsync(fr->counts, 0, sizeof(fr->counts), st));
+    pack_valid_scans(ctx, pack);
+    std::vector<KdScan> regs((size_t)B);
+    for (int b = 0; b < B; ++b) regs[(size_t)b] = packed[(size_t)(scan_of ? scan_of[b] : b)];
+    return regs;
+}
+
 }  // namespace pls
 
 using namespace pls;
@@ -1163,42 +1200,56 @@ int pls_register_scans(pls_context* ctx, const float* const* scans, const int64_
     for (int s = 0; s < S; ++s) PLS_REQUIRE(scans[s] && n[s] > 0, "pls_register_scans: every scan must be [n,3] with n > 0");
     for (int b = 0; scan_of && b < B; ++b)
         PLS_REQUIRE(scan_of[b] >= 0 && scan_of[b] < S, "pls_register_scans: scan_of entries must lie in [0, S)");
-    cudaStream_t st = ctx->stream;
     map_stream_wait(ctx);
-    // host scans are staged back to back, as to_device stages one
-    size_t host_rows = 0;
-    for (int s = 0; s < S; ++s)
-        if (!is_device_ptr(scans[s])) host_rows += (size_t)n[s];
-    if (host_rows) ctx->stage_in[0].reserve(host_rows * 3 * sizeof(float), st);
-    // scan s's packed rows go to ctx->queries at the sum of the earlier scans' row counts, the S counts behind them
-    size_t rows = 0;
-    for (int s = 0; s < S; ++s) rows += (size_t)n[s];
-    ctx->queries.reserve(rows * sizeof(float4) + (size_t)S * sizeof(uint32_t), st);
-    float4* q = ctx->queries.as<float4>();
-    uint32_t* counts = reinterpret_cast<uint32_t*>(q + rows);
-    std::vector<KdScanRows> pack((size_t)S);
-    std::vector<KdScan> packed((size_t)S);
-    float* staged = ctx->stage_in[0].as<float>();
-    for (int s = 0; s < S; ++s) {
-        const float* d = scans[s];
-        if (!is_device_ptr(d)) {
-            PLS_CUDA(cudaMemcpyAsync(staged, d, (size_t)n[s] * 3 * sizeof(float), cudaMemcpyHostToDevice, st));
-            d = staged;
-            staged += (size_t)n[s] * 3;
-        }
-        pack[(size_t)s] = KdScanRows{d, n[s], q, counts + s};
-        packed[(size_t)s] = KdScan{q, counts + s, n[s]};
-        q += n[s];
-    }
+    const std::vector<KdScan> regs = stage_scans(ctx, scans, n, S, scan_of, B);
     const float* T0_dev = (const float*)to_device(ctx, T0s, (size_t)B * 16 * sizeof(float), ctx->stage_in[1]);
-    FrameResult* fr = frame_result_dev(ctx);
-    PLS_CUDA(cudaMemsetAsync(fr->counts, 0, sizeof(fr->counts), st));
-    pack_valid_scans(ctx, pack);
-    std::vector<KdScan> regs((size_t)B);
-    for (int b = 0; b < B; ++b) regs[(size_t)b] = packed[(size_t)(scan_of ? scan_of[b] : b)];
     register_batch(ctx, regs.data(), 0, T0_dev, B, out_T, out_params, out_losses, out_iters, out_status);
     PLS_API_END(ctx)
 }
+
+int pls_kdmap_evaluate_poses(pls_context* ctx, const float* const* scans, const int64_t* n, int S, const int* scan_of,
+                             const float* T, int B, double max_distance, double* out_stats) {
+    PLS_API_BEGIN(ctx)
+    // every argument is checked before anything is enqueued: a refused call changes nothing
+    PLS_REQUIRE(ctx->cfg.local_map_type == PLS_MAP_KDTREE, "pls_kdmap_evaluate_poses: needs a kd-tree local map");
+    PLS_REQUIRE(!ctx->comm, "pls_kdmap_evaluate_poses: a context with a multi-GPU communicator is not supported");
+    PLS_REQUIRE(ctx->kd.valid, "kd map: search before any update");
+    PLS_REQUIRE(scans && n && S > 0, "pls_kdmap_evaluate_poses: scans and n must hold S > 0 scans");
+    PLS_REQUIRE(T && B > 0, "pls_kdmap_evaluate_poses: T must be [B,16] with B > 0");
+    PLS_REQUIRE(out_stats, "pls_kdmap_evaluate_poses: null out_stats");
+    PLS_REQUIRE(scan_of || B == S, "pls_kdmap_evaluate_poses: without scan_of, B must equal S");
+    PLS_REQUIRE(max_distance >= 0.0, "pls_kdmap_evaluate_poses: max_distance must be >= 0 (not NaN)");
+    for (int s = 0; s < S; ++s)
+        PLS_REQUIRE(scans[s] && n[s] > 0, "pls_kdmap_evaluate_poses: every scan must be [n,3] with n > 0");
+    for (int b = 0; scan_of && b < B; ++b)
+        PLS_REQUIRE(scan_of[b] >= 0 && scan_of[b] < S, "pls_kdmap_evaluate_poses: scan_of entries must lie in [0, S)");
+    cudaStream_t st = ctx->stream;
+    map_stream_wait(ctx);
+    const std::vector<KdScan> regs = stage_scans(ctx, scans, n, S, scan_of, B);
+    const float* T_dev = (const float*)to_device(ctx, T, (size_t)B * 16 * sizeof(float), ctx->stage_in[1]);
+    OutArg o = out_arg(ctx, out_stats, (size_t)B * PLS_EVAL_STATS * sizeof(double), ctx->stage_out[0]);
+    const double max_d2 = max_distance * max_distance;
+    int last = 0;
+    // no host synchronisation between the chunks: a buffer that grows waits for the stream itself (DBuf::reserve)
+    for (int c0 = 0; c0 < B; c0 += PLS_MAX_SEQUENCES) {
+        const int num = B - c0 < PLS_MAX_SEQUENCES ? B - c0 : PLS_MAX_SEQUENCES;
+        int grid[KD_BATCH_GRID];
+        FrameResult* frs = nullptr;
+        uint32_t* words = nullptr;
+        kdmap_hypotheses_begin(ctx, regs.data() + c0, num, st, grid, &frs, &words);
+        hypotheses_begin_kernel<<<num, kMaxAlign, 0, st>>>(frs, T_dev + 16 * (size_t)c0, words);
+        PLS_CHECK_LAUNCH();
+        kdmap_evaluate_batch(ctx, num, st, grid, max_d2, (double*)o.dev + (size_t)PLS_EVAL_STATS * c0);
+        last = num - 1;
+    }
+    kdmap_hypothesis_adopt(ctx, regs[(size_t)B - 1], last, st);
+    fetch_result(ctx);
+    ctx->icp_result = true;
+    finish_out(ctx, o);
+    PLS_CUDA(cudaStreamSynchronize(st));
+    PLS_API_END(ctx)
+}
+
 
 int pls_process_frame(pls_context* ctx, const void* data, int layout, int64_t n, const float* init_pose,
                       float* out_pose, float* out_params, int* out_has_pose, double* out_info) {

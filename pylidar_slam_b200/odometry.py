@@ -327,6 +327,64 @@ def _pose_candidates(T0, coarse, T, iters, status, scores) -> list:
                           coarse_rank=int(r), iterations=int(iters[r]), status=int(status[r])) for r in order]
 
 
+_UPPER6 = [(a, b) for a in range(6) for b in range(a, 6)]
+
+
+@dataclass
+class RegistrationQuality:
+    """How well one pose registers its scan on the kd map (ICPFrameToModel.evaluate_registrations): what a filter, a
+    pose graph or an acceptance test needs of a registration.
+
+    valid: the scan's valid rows (no NaN coordinate); inliers: those whose exact nearest map point lies within
+    max_distance of the transformed row; fitness = inliers / valid; rmse = sqrt(sum d^2 / inliers), d the distance to
+    that nearest point; plane_rmse = sqrt(sum r^2 / inliers), r the point-to-plane residual.  NaN where a denominator
+    is zero.
+
+    information [6,6]: J^T W J over the inliers, J = [n, p' x n] the point-to-plane Jacobian of the first ICP iteration
+    and W its robust weights (the context's scheme).  The parameters are (tx, ty, tz, rx, ry, rz) of a small increment
+    left-multiplied onto the pose, in the map frame.  eigenvalues [6] (ascending) and eigenvectors [6,6] (columns) are
+    np.linalg.eigh(information): a small eigenvalue marks a direction the map does not constrain (a tunnel, a
+    corridor, a flat field).  covariance [6,6] = (sum (w r)^2 / (inliers - 6)) information^-1, the least-squares
+    formula: exact for the unweighted scheme, an approximation under robust weights.  None when inliers <= 6 or when the
+    float64 Cholesky factorisation of information fails."""
+    valid: int
+    inliers: int
+    fitness: float
+    rmse: float
+    plane_rmse: float
+    information: np.ndarray
+    covariance: Optional[np.ndarray]
+    eigenvalues: np.ndarray
+    eigenvectors: np.ndarray
+
+    @staticmethod
+    def from_stats(row) -> "RegistrationQuality":
+        """From one row of pls_kdmap_evaluate_poses (PLS_EVAL_STATS doubles: 21 J^T W J upper, 6 J^T W r,
+        sum (w r)^2, sum r^2, inliers, sum d^2, valid rows)."""
+        row = np.asarray(row, np.float64)
+        H = np.zeros((6, 6))
+        for k, (a, b) in enumerate(_UPPER6):
+            H[a, b] = H[b, a] = row[k]
+        inliers, valid = int(row[29]), int(row[31])
+
+        def ratio(num, den):
+            return float(num / den) if den > 0 else float("nan")
+
+        covariance = None
+        if inliers > 6:
+            try:
+                L = np.linalg.cholesky(H)
+                L_inv = np.linalg.inv(L)
+                covariance = (row[27] / (inliers - 6)) * (L_inv.T @ L_inv)
+            except np.linalg.LinAlgError:
+                covariance = None
+        w, v = np.linalg.eigh(H)
+        return RegistrationQuality(valid=valid, inliers=inliers, fitness=ratio(inliers, valid),
+                                   rmse=float(np.sqrt(ratio(row[30], inliers))),
+                                   plane_rmse=float(np.sqrt(ratio(row[28], inliers))), information=H,
+                                   covariance=covariance, eigenvalues=w, eigenvectors=v)
+
+
 class KdTreeLocalMap(LocalMap):
     """KdTreeLocalMap (local_map.py:254-427) on the GPU: exact 1-NN over the hashed cell pyramid + lazily cached 10-NN normals.
 
@@ -1127,24 +1185,8 @@ class ICPFrameToModel(OdometryAlgorithm):
         register_new_frame(scans[scan_indices[b]], initial_estimates[b]) returns, bit for bit.  A singular registration
         does not stop the others: it is logged, and last_registrations_status[b] holds each one's status (PLS_OK,
         PLS_W_TINY_RESIDUAL or PLS_E_SINGULAR)."""
-        _check_given_normals(self.ctx)
-        pts = []
-        for scan in scans:
-            check_tensor(scan, [-1, 3])
-            pts.append(_f32c(scan))
-        if isinstance(initial_estimates, torch.Tensor):
-            initial_estimates = initial_estimates.detach().cpu().numpy()
-        check_tensor(initial_estimates, [-1, 4, 4])
-        T0 = np.ascontiguousarray(initial_estimates, dtype=np.float32)
+        pts, addresses, rows, T0, index = self._scans_args(scans, initial_estimates, scan_indices)
         B, S, M = T0.shape[0], len(pts), int(self.config.max_num_alignments)
-        index = None
-        if scan_indices is not None:
-            if isinstance(scan_indices, torch.Tensor):
-                scan_indices = scan_indices.detach().cpu().numpy()
-            index = np.ascontiguousarray(scan_indices, dtype=np.int32).reshape(-1)
-            assert_debug(index.shape[0] == B, f"scan_indices must hold one scan index per initial estimate ({B})")
-        addresses = np.array([_lib.ptr(p) for p in pts], dtype=np.uint64)
-        rows = np.array([p.shape[0] for p in pts], dtype=np.int64)
         T, params = np.zeros((B, 4, 4), np.float32), np.zeros((B, 6), np.float32)
         losses = np.zeros((B, M), np.float32)
         iters, status = np.zeros(B, np.int32), np.zeros(B, np.int32)
@@ -1157,6 +1199,47 @@ class ICPFrameToModel(OdometryAlgorithm):
             logging.error(f"Invalid Jacobian in Gauss Newton minimization, the hessian is not invertible "
                           f"(registrations {singular.tolist()})")
         return params, T, [list(losses[b, :iters[b]]) for b in range(B)], iters
+
+    def _scans_args(self, scans, poses, scan_indices):
+        """register_new_frames' and evaluate_registrations' inputs as pls_register_scans / pls_kdmap_evaluate_poses
+        take them: (float32 scans kept alive, their addresses [S], rows [S], poses [B,4,4] float32, scan_of [B] int32 or
+        None).  IndexError while the map carries given normals."""
+        _check_given_normals(self.ctx)
+        pts = []
+        for scan in scans:
+            check_tensor(scan, [-1, 3])
+            pts.append(_f32c(scan))
+        if isinstance(poses, torch.Tensor):
+            poses = poses.detach().cpu().numpy()
+        check_tensor(poses, [-1, 4, 4])
+        T0 = np.ascontiguousarray(poses, dtype=np.float32)
+        B = T0.shape[0]
+        index = None
+        if scan_indices is not None:
+            if isinstance(scan_indices, torch.Tensor):
+                scan_indices = scan_indices.detach().cpu().numpy()
+            index = np.ascontiguousarray(scan_indices, dtype=np.int32).reshape(-1)
+            assert_debug(index.shape[0] == B, f"scan_indices must hold one scan index per initial estimate ({B})")
+        addresses = np.array([_lib.ptr(p) for p in pts], dtype=np.uint64)
+        rows = np.array([p.shape[0] for p in pts], dtype=np.int64)
+        return pts, addresses, rows, T0, index
+
+    def evaluate_registrations(self, scans, poses, max_distance: float = np.inf, scan_indices=None) -> list:
+        """The quality of B poses of S scans on the kd map this odometry's context holds, in one call
+        (pls_kdmap_evaluate_poses; no reference counterpart): an inlier fraction, an inlier RMSE and an information
+        matrix per pose, for a filter or a pose graph fed by a localiser, for accepting or rejecting a registration,
+        and for re-ranking localize's candidates (one call on their T).  Inputs as register_new_frames: `scans` S
+        [n_i,3] arrays or tensors, `poses` [B,4,4], pose b applied to scans[scan_indices[b]] (None: scan b, B == S).
+        A valid row is an inlier when its exact nearest map point lies within max_distance (>= 0; inf admits every
+        match).  Nothing is solved and the map is left unchanged.  Returns B RegistrationQuality; with max_distance
+        inf, pose b's information matrix is built from the sums the first ICP iteration of
+        register_new_frame(scans[scan_indices[b]], poses[b]) forms.  IndexError while the map carries given normals."""
+        pts, addresses, rows, T, index = self._scans_args(scans, poses, scan_indices)
+        B = T.shape[0]
+        stats = np.zeros((B, _lib.EVAL_STATS), np.float64)
+        self.ctx.call("pls_kdmap_evaluate_poses", _lib.ptr(addresses), _lib.ptr(rows), len(pts), _lib.ptr(index),
+                      _lib.ptr(T), B, float(max_distance), _lib.ptr(stats))
+        return [RegistrationQuality.from_stats(stats[b]) for b in range(B)]
 
 
 class ICPFrameToModelBatch:
