@@ -362,6 +362,29 @@ PLS_API int pls_register_hypotheses(pls_context* ctx, const float* points, int64
 PLS_API int pls_register_scans(pls_context* ctx, const float* const* scans, const int64_t* n, int S,
                                const int* scan_of, const float* T0s, int B, float* out_T, float* out_params,
                                float* out_losses, int* out_iters, int* out_status);
+/* pls_register_scans with a correspondence gate (no reference counterpart: the reference registers against its own
+ * fresh local map; a prior map is stale -- moved cars, construction, partial overlap -- and a match beyond a distance
+ * biases the pose).  Arguments, outputs and rules as pls_register_scans, plus max_distance and out_inliers.
+ * For registration b, ICP iteration i, and a valid row p of its scan:
+ *   p'      transform_point(T_b,i, p); q p's exact 1-NN in the map -- the point, with the tie rule, the ungated search
+ *           returns;
+ *   d^2     match_d2_f64 as pls_kdmap_evaluate_poses computes it: float64, every operation rounded on its own;
+ *   inlier  d^2 <= max_distance * max_distance in float64.  Only inliers enter the 30 accumulators, the loss and the
+ *           count; the search may report no match for an outlier (pls_kdmap_last_correspondences), never another
+ *           point than q for an inlier.
+ * out_inliers [B] (nullable, host or device): registration b's inlier count in its last executed iteration (its count
+ * accumulator, pls_last_icp_sums[29] for the last registration).  A registration with too few inliers to solve stops
+ * with PLS_E_SINGULAR in out_status, and so does one whose last iteration had no inlier at all (its pose is the last
+ * one solved); the others go on.  max_distance = +inf gives pls_register_scans's bits for every
+ * output.  Iteration 0 of a registration accumulates, bit for bit, entries 0..29 of pls_kdmap_evaluate_poses's row for
+ * its initial pose and the same max_distance.  The map, its index and the odometry state are unchanged (the normal
+ * cache may fill, with the bits it would get anyway); afterwards the last registration is the context's last search.
+ * PLS_E_INVALID before any work, the context unchanged: everything pls_register_scans refuses, and a max_distance that
+ * is NaN or negative. */
+PLS_API int pls_register_scans_gated(pls_context* ctx, const float* const* scans, const int64_t* n, int S,
+                                     const int* scan_of, const float* T0s, int B, double max_distance, float* out_T,
+                                     float* out_params, float* out_losses, int* out_iters, int* out_status,
+                                     int* out_inliers);
 /* The quality of B registrations on the kd map ctx holds, in one call (no reference counterpart: a localiser that feeds
  * a filter or a pose graph needs each registration's inlier fraction, inlier RMSE and information matrix, and a
  * re-ranking of pose candidates needs more than an occupancy score).  Arguments, staging and pointer rules are those

@@ -1,6 +1,7 @@
 // Internal declarations shared by the translation units of libplslam_b200.so.
 #pragma once
 #include <cuda_runtime.h>
+#include <math.h>
 #include <stddef.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -449,7 +450,10 @@ void kdmap_update_packed(pls_context* ctx, const float* rel_pose_host, const flo
 constexpr int KD_BATCH_GRID = 6;
 void kdmap_batch_begin(pls_context* lead, pls_context* const* ctxs, const int64_t* query_bounds, int num, cudaStream_t st,
                        int* grid);
-void kdmap_batch_iterations(pls_context* lead, int num, cudaStream_t st, const int* grid, int first, int last);
+// max_distance (pls_register_scans_gated, registrations only): finite, the iterations run the gated kernels with that
+// gate (KdGate); +inf, the ungated ones.
+void kdmap_batch_iterations(pls_context* lead, int num, cudaStream_t st, const int* grid, int first, int last,
+                            double max_distance = HUGE_VAL);
 void kdmap_batch_done(pls_context* lead, int num, cudaStream_t st, int* out);
 // The scan one registration of pls_register_hypotheses / pls_register_scans reads: its packed float4 queries, their
 // count on the device (u32) and the query bound of its single pls_register_frame call (the scan's row count).

@@ -401,7 +401,15 @@ __device__ __forceinline__ bool claim_normal(const KdIndex& ix, int pos) {
 // other than its match.  If the query, now at p, has moved by eps since then and its match `pos` is now at distance d,
 // every other point is still at least (bound - eps) away, so d + eps < bound proves the match unchanged -- one point
 // load and a dozen flops per query.  False when there is no match (pos < 0).
-__device__ __forceinline__ bool match_proven(const KdIndex& ix, const float* p, int pos, const float4& state) {
+// GATE: no match is a gated search's outlier, whose state holds a lower bound of the squared distance to EVERY map
+// point (warp_nearest<true>).  It stays an outlier, with no search, while (bound - eps) > max_distance is proven in
+// float32 with match_proven's own slack; otherwise it is searched again.  A proven match is kept whatever its distance:
+// the residual pass tests it against the gate in every iteration.
+template <bool GATE = false>
+__device__ __forceinline__ bool match_proven(const KdIndex& ix, const float* p, int pos, const float4& state,
+                                             float dmax = 0.f) {
+    if constexpr (GATE)
+        if (pos < 0) return (sqrtf(dist2_point(p[0], p[1], p[2], state)) + dmax) * 1.00001f + 1e-6f < sqrtf(state.w);
     if (pos < 0) return false;
     const float4 s = state;
     const float d = sqrtf(dist2_point(p[0], p[1], p[2], __ldg(ix.sorted + pos)));
@@ -465,12 +473,14 @@ __device__ __forceinline__ void block_partial_and_finish(double* acc, FrameResul
 }
 
 // Iterations after a frame's first on maps of KD_COLD_MAP_POINTS or more: a thread per query keeps its previous match
-// if match_proven; the few others are queued for kd_nn_warp_kernel.
+// if match_proven; the few others are queued for kd_nn_warp_kernel.  GATE: match_proven<true> with gate.dmax.
+template <bool GATE = false>
 __device__ __forceinline__ void kd_nn_verify_body(const KdIndex& ix, const float4* __restrict__ queries,
                                                   const uint32_t* __restrict__ nq_dev, int64_t q_begin, int64_t q_stride,
                                                   const float* __restrict__ T, const int* __restrict__ done,
                                                   const int* __restrict__ match, const float4* __restrict__ nn_state,
-                                                  int* __restrict__ hard, uint32_t* lists, int parity, unsigned block) {
+                                                  int* __restrict__ hard, uint32_t* lists, int parity, unsigned block,
+                                                  float dmax = 0.f) {
     if (done && *done) return;
     __shared__ float sT[12];
     __shared__ int s_hard[KD_THREADS];
@@ -487,7 +497,7 @@ __device__ __forceinline__ void kd_nn_verify_body(const KdIndex& ix, const float
     if (qi < nq) {
         float p[3];
         transform_point(sT, queries[qi], p);
-        if (!match_proven(ix, p, match[qi], nn_state[qi])) s_hard[atomicAdd(&s_nh, 1)] = (int)qi;
+        if (!match_proven<GATE>(ix, p, match[qi], nn_state[qi], dmax)) s_hard[atomicAdd(&s_nh, 1)] = (int)qi;
     }
     __syncthreads();
     block_flush_list(s_hard, s_nh, hard, lists + KDL_HARD_NN + parity, &s_base);
@@ -510,13 +520,15 @@ kd_nn_verify_kernel(KdIndex ix, const float4* __restrict__ queries, const uint32
 // match a map point whose normal is not cached claims it (CAS on the state word) and queues it; claims are made by all
 // lanes at once after 32 queries.  Each query's position and runner-up bound are kept for the later iterations' checks.
 // Which warp searches which query does not change its result, so any block count gives the same bits.
+// GATE: warp_nearest<true>; an outlier's match is -1, so it claims no normal.
+template <bool GATE = false>
 __device__ __forceinline__ void kd_nn_warp_body(const KdIndex& ix, const float4* __restrict__ queries,
                                                 const uint32_t* __restrict__ nq_dev, int64_t q_begin, int64_t q_stride,
                                                 const int* __restrict__ hard, uint32_t* lists, int parity,
                                                 const float* __restrict__ T, const int* __restrict__ done,
                                                 int* __restrict__ match, float4* __restrict__ nn_state, int want_normals,
                                                 int* __restrict__ pending, unsigned long long* __restrict__ counters,
-                                                unsigned block, unsigned grid) {
+                                                unsigned block, unsigned grid, KdGate gate = KdGate{}) {
     if (done && *done) return;
     int n;
     if (hard) {
@@ -567,7 +579,7 @@ __device__ __forceinline__ void kd_nn_warp_body(const KdIndex& ix, const float4*
         float p[3];
         transform_point(t, p0, p);
         float second;
-        const int pos = warp_nearest(ix, g, p[0], p[1], p[2], hint, lane, &cand, &second);
+        const int pos = warp_nearest<GATE>(ix, g, p[0], p[1], p[2], hint, lane, &cand, &second, gate);
         if (lane == 0) {
             match[qi] = pos;
             if (nn_state) nn_state[qi] = make_float4(p[0], p[1], p[2], second);
@@ -670,20 +682,13 @@ kd_normals_wide_kernel(KdIndex ix, int k_normals, const int* __restrict__ workli
     kd_normals_warp_body<R>(ix, k_normals, worklist, wl_count, done, counters, blockIdx.x, gridDim.x);
 }
 
-// The squared distance of a transformed query p to its match q in float64, every operation rounded on its own (no
-// contraction): ((dx dx + dy dy) + dz dz), dx = (double)p_x - (double)q_x -- numpy's element-wise float64 bits.
-__device__ __forceinline__ double match_d2_f64(const float* p, const float4& q) {
-    const double dx = __dsub_rn((double)p[0], (double)q.x);
-    const double dy = __dsub_rn((double)p[1], (double)q.y);
-    const double dz = __dsub_rn((double)p[2], (double)q.z);
-    return __dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz));
-}
-
 // A thread per query: accumulate_match -> block partials; the last block sums them in fixed order and runs the solve,
 // stop test and pose update.
 // EVAL (pls_kdmap_evaluate_poses, launched with fuse_threshold < 0: no solve): only the matches with
 // match_d2_f64 <= max_d2 are accumulated, their d^2 summed in acc[NACC], and every query is counted in acc[NACC + 1];
 // the block partial rows are PLS_EVAL_STATS wide.  The ICP instantiation (EVAL = false) is the same code as before.
+// GATE without EVAL (a gated registration): the same distance test on NACC-wide rows with the fused solve, so the
+// count accumulator (29) counts the inliers.
 // kd_residual_body's pose.  Owned by this function rather than by the template, so that the module's shared variables
 // keep the order they had before kd_residual_body took EVAL: the ICP kernels keep their shared-memory layout and SASS
 // (profiles/sass_evaluate_poses_census.log).
@@ -692,7 +697,7 @@ __device__ __forceinline__ float* kd_residual_pose() {
     return sT;
 }
 
-template <bool EVAL = false>
+template <bool EVAL = false, bool GATE = EVAL>
 __device__ __forceinline__ void kd_residual_body(const KdIndex& ix, const float4* __restrict__ queries,
                                                  const uint32_t* __restrict__ nq_dev, int64_t q_begin, int64_t q_stride,
                                                  FrameResult* fr, int scheme, float sigma, const int* __restrict__ match,
@@ -717,10 +722,10 @@ __device__ __forceinline__ void kd_residual_body(const KdIndex& ix, const float4
         const int pos = match[qi];
         if constexpr (EVAL) acc[NACC + 1] += 1.0;
         if (pos < 0) continue;
-        if constexpr (EVAL) {
+        if constexpr (GATE) {
             const double d2 = match_d2_f64(p, __ldg(ix.sorted + pos));
             if (!(d2 <= max_d2)) continue;
-            acc[NACC] += d2;
+            if constexpr (EVAL) acc[NACC] += d2;
         }
         accumulate_match(acc, ix, p, pos, scheme, sigma KD_SPLIT_PASS);
     }
@@ -752,20 +757,39 @@ kd_residual_kernel(KdIndex ix, const float4* __restrict__ queries, const uint32_
 // kd_residual_kernel's geometry), all of its warps share the searches of step 2.  A cfg2 block re-searches 13 queries
 // and computes 4 normals in the median, 30 and 13 at most (profiles/h100_kd_residual_split_after.log): with 8 warps
 // the slowest block's searches took 35 us, a chain of up to four searches per warp.
+// GATE: match_proven<true>, warp_nearest<true> (an outlier computes no normal) and the residual's distance test.
 constexpr int KD_REFINE_THREADS = 512;
 constexpr int KD_REFINE_WARPS = KD_REFINE_THREADS / 32;
+// kd_icp_refine_body's shared state, owned by this function rather than by the template for the reason kd_residual_pose
+// gives: the ungated kernels keep their shared-memory layout and SASS.
+struct KdRefineShared {
+    float* sT;
+    int* s_hard;
+    int* s_nh;
+    unsigned long long (*s_stage)[KNN_STAGE];
+};
+__device__ __forceinline__ KdRefineShared kd_refine_shared() {
+    __shared__ float sT[12];
+    __shared__ int s_hard[KD_THREADS];
+    __shared__ int s_nh;
+    __shared__ unsigned long long s_stage[KD_REFINE_WARPS][KNN_STAGE];
+    return KdRefineShared{sT, s_hard, &s_nh, s_stage};
+}
+
+template <bool GATE = false>
 __device__ __forceinline__ void kd_icp_refine_body(const KdIndex& ix, const float4* __restrict__ queries,
                                                    const uint32_t* __restrict__ nq_dev, int64_t q_begin, int64_t q_stride,
                                                    FrameResult* fr, int scheme, float sigma, int k_normals,
                                                    int* __restrict__ match, float4* __restrict__ nn_state,
                                                    double* __restrict__ partials, float fuse_threshold,
                                                    unsigned long long* __restrict__ counters, unsigned block,
-                                                   unsigned grid KD_SPLIT_ARG) {
+                                                   unsigned grid KD_SPLIT_ARG, KdGate gate = KdGate{}) {
     if (fr->done) return;
-    __shared__ float sT[12];
-    __shared__ int s_hard[KD_THREADS];
-    __shared__ int s_nh;
-    __shared__ unsigned long long s_stage[KD_REFINE_WARPS][KNN_STAGE];
+    const KdRefineShared sh = kd_refine_shared();
+    float* sT = sh.sT;
+    int* s_hard = sh.s_hard;
+    int& s_nh = *sh.s_nh;
+    unsigned long long(*s_stage)[KNN_STAGE] = sh.s_stage;
     if (threadIdx.x < 12) sT[threadIdx.x] = fr->T[threadIdx.x];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const bool owner = threadIdx.x < KD_THREADS;  // warp-uniform: this thread has a query slot
@@ -780,7 +804,7 @@ __device__ __forceinline__ void kd_icp_refine_body(const KdIndex& ix, const floa
         if (owner && qi < nq) {
             float p[3];
             transform_point(sT, queries[qi], p);
-            if (!match_proven(ix, p, match[qi], nn_state[qi])) s_hard[atomicAdd(&s_nh, 1)] = threadIdx.x;
+            if (!match_proven<GATE>(ix, p, match[qi], nn_state[qi], gate.dmax)) s_hard[atomicAdd(&s_nh, 1)] = threadIdx.x;
         }
         __syncthreads();
         const int nh = s_nh;
@@ -794,7 +818,7 @@ __device__ __forceinline__ void kd_icp_refine_body(const KdIndex& ix, const floa
                 float p[3];
                 transform_point(sT, queries[q], p);
                 float second;
-                const int pos = warp_nearest(ix, g, p[0], p[1], p[2], match[q], lane, &cand_nn, &second);
+                const int pos = warp_nearest<GATE>(ix, g, p[0], p[1], p[2], match[q], lane, &cand_nn, &second, gate);
                 if (lane == 0) {
                     match[q] = pos;
                     nn_state[q] = make_float4(p[0], p[1], p[2], second);
@@ -830,6 +854,8 @@ __device__ __forceinline__ void kd_icp_refine_body(const KdIndex& ix, const floa
         if (pos < 0) continue;
         float p[3];
         transform_point(sT, queries[qi], p);
+        if constexpr (GATE)
+            if (!(match_d2_f64(p, __ldg(ix.sorted + pos)) <= gate.max_d2)) continue;
         accumulate_match(acc, ix, p, pos, scheme, sigma KD_SPLIT_PASS);
     }
     block_partial_and_finish<KD_REFINE_THREADS>(acc, fr, partials, fuse_threshold, block, grid KD_SPLIT_PASS);
@@ -976,6 +1002,47 @@ __global__ void __launch_bounds__(KD_REFINE_THREADS) kd_icp_refine_batch_kernel(
     KD_SPLIT_NONE()
     kd_icp_refine_body(s.ix, s.queries, s.nq_dev, 0, 1, s.fr, s.scheme, s.sigma, s.k_normals, s.match, s.nn_state,
                        s.partials, s.fuse_threshold, s.counters, blockIdx.x, s.refine_blocks KD_SPLIT_PASS);
+}
+
+// The gated twins of the four-launch and refine batch kernels (pls_register_scans_gated): the same bodies with GATE,
+// the registrations' gate a launch argument.  It is not a KdSeq field: a wider descriptor would change the copy and the
+// stride of every batch kernel above.
+__global__ void __launch_bounds__(KD_THREADS) kd_nn_verify_gated_batch_kernel(const KdSeq* __restrict__ seqs, int it,
+                                                                              KdGate gate) {
+    __shared__ KdSeq s;
+    load_seq(seqs, s);
+    if ((int)blockIdx.x >= s.verify_blocks || !four_launch_step(s, it)) return;
+    kd_nn_verify_body<true>(s.ix, s.queries, s.nq_dev, 0, 1, s.fr->T, &s.fr->done, s.match, s.nn_state, s.hard, s.lists,
+                            it & 1, blockIdx.x, gate.dmax);
+}
+
+__global__ void __launch_bounds__(KD_THREADS) kd_nn_warp_gated_batch_kernel(const KdSeq* __restrict__ seqs, int it,
+                                                                            KdGate gate) {
+    __shared__ KdSeq s;
+    load_seq(seqs, s);
+    if ((int)blockIdx.x >= s.nn_blocks || !four_launch_step(s, it)) return;
+    kd_nn_warp_body<true>(s.ix, s.queries, s.nq_dev, 0, 1, it == 0 ? nullptr : s.hard, s.lists, it & 1, s.fr->T,
+                          &s.fr->done, s.match, s.nn_state, 1, s.pending, s.counters, blockIdx.x, s.nn_blocks, gate);
+}
+
+__global__ void __launch_bounds__(KD_THREADS) kd_residual_gated_batch_kernel(const KdSeq* __restrict__ seqs, int it,
+                                                                             double max_d2) {
+    __shared__ KdSeq s;
+    load_seq(seqs, s);
+    if ((int)blockIdx.x >= s.blocks || !four_launch_step(s, it)) return;
+    KD_SPLIT_NONE()
+    kd_residual_body<false, true>(s.ix, s.queries, s.nq_dev, 0, 1, s.fr, s.scheme, s.sigma, s.match, s.partials,
+                                  s.fuse_threshold, blockIdx.x, s.blocks, max_d2 KD_SPLIT_PASS);
+}
+
+__global__ void __launch_bounds__(KD_REFINE_THREADS) kd_icp_refine_gated_batch_kernel(const KdSeq* __restrict__ seqs,
+                                                                                      int it, KdGate gate) {
+    __shared__ KdSeq s;
+    load_seq(seqs, s);
+    if ((int)blockIdx.x >= s.refine_blocks || it >= s.max_iters) return;
+    KD_SPLIT_NONE()
+    kd_icp_refine_body<true>(s.ix, s.queries, s.nq_dev, 0, 1, s.fr, s.scheme, s.sigma, s.k_normals, s.match, s.nn_state,
+                             s.partials, s.fuse_threshold, s.counters, blockIdx.x, s.refine_blocks KD_SPLIT_PASS, gate);
 }
 
 // The done flags of every sequence, for the host's extra-round check.
@@ -1584,9 +1651,12 @@ void kdmap_batch_begin(pls_context* lead, pls_context* const* ctxs, const int64_
 // launch per kernel for all of them.  A later iteration is kd_icp_refine_batch_kernel for the sequences whose later
 // iterations take one launch and the four launches verify / 1-NN / normals / residual for the others; the normals of a
 // wide k are one more launch, made only if some sequence has one.  No launch grows with num.
-// The 1-NN and normals launches of iteration `it` of the four-launch path for the sequences described in seqs.
-static void batch_search(const KdSeq* seqs, int num, cudaStream_t st, const int* grid, int it) {
-    kd_nn_warp_batch_kernel<<<dim3(grid[1], num), KD_THREADS, 0, st>>>(seqs, it);
+// The 1-NN and normals launches of iteration `it` of the four-launch path for the sequences described in seqs; gate
+// (nullable): the gated registrations' gate.
+static void batch_search(const KdSeq* seqs, int num, cudaStream_t st, const int* grid, int it,
+                         const KdGate* gate = nullptr) {
+    if (gate) kd_nn_warp_gated_batch_kernel<<<dim3(grid[1], num), KD_THREADS, 0, st>>>(seqs, it, *gate);
+    else kd_nn_warp_batch_kernel<<<dim3(grid[1], num), KD_THREADS, 0, st>>>(seqs, it);
     PLS_CHECK_LAUNCH();
     kd_normals_warp_batch_kernel<<<dim3(grid[2], num), KD_THREADS, 0, st>>>(seqs, it);
     PLS_CHECK_LAUNCH();
@@ -1599,20 +1669,41 @@ static void batch_search(const KdSeq* seqs, int num, cudaStream_t st, const int*
     }
 }
 
-void kdmap_batch_iterations(pls_context* lead, int num, cudaStream_t st, const int* grid, int first, int last) {
+// The gate of a finite max_distance >= 0 (KdGate, kdmap_device.cuh): max_d2 = max_distance^2 in float64, and the
+// float32 bounds rounded up.
+static KdGate kd_gate_of(double max_distance) {
+    auto up = [](double v) {  // the least float32 >= v (+inf above FLT_MAX)
+        if (!(v <= (double)FLT_MAX)) return INFINITY;
+        float f = (float)v;
+        return (double)f < v ? nextafterf(f, INFINITY) : f;
+    };
+    KdGate g;
+    g.max_d2 = max_distance * max_distance;
+    g.g2 = up(g.max_d2 * (1.0 + 0x1p-20) + 0x1p-126);
+    g.dmax = up(max_distance);
+    return g;
+}
+
+void kdmap_batch_iterations(pls_context* lead, int num, cudaStream_t st, const int* grid, int first, int last,
+                            double max_distance) {
     const KdSeq* seqs = lead->batch_buf.as<KdSeq>();
+    const KdGate g = kd_gate_of(isinf(max_distance) ? 0.0 : max_distance);
+    const KdGate* gate = isinf(max_distance) ? nullptr : &g;
     for (int it = first; it < last; ++it) {
         if (it > 0 && grid[4]) {
-            kd_icp_refine_batch_kernel<<<dim3(grid[0], num), KD_REFINE_THREADS, 0, st>>>(seqs, it);
+            if (gate) kd_icp_refine_gated_batch_kernel<<<dim3(grid[0], num), KD_REFINE_THREADS, 0, st>>>(seqs, it, *gate);
+            else kd_icp_refine_batch_kernel<<<dim3(grid[0], num), KD_REFINE_THREADS, 0, st>>>(seqs, it);
             PLS_CHECK_LAUNCH();
         }
         if (it > 0 && !grid[3]) continue;
         if (it > 0) {
-            kd_nn_verify_batch_kernel<<<dim3(grid[3], num), KD_THREADS, 0, st>>>(seqs, it);
+            if (gate) kd_nn_verify_gated_batch_kernel<<<dim3(grid[3], num), KD_THREADS, 0, st>>>(seqs, it, *gate);
+            else kd_nn_verify_batch_kernel<<<dim3(grid[3], num), KD_THREADS, 0, st>>>(seqs, it);
             PLS_CHECK_LAUNCH();
         }
-        batch_search(seqs, num, st, grid, it);
-        kd_residual_batch_kernel<<<dim3(grid[0], num), KD_THREADS, 0, st>>>(seqs, it);
+        batch_search(seqs, num, st, grid, it, gate);
+        if (gate) kd_residual_gated_batch_kernel<<<dim3(grid[0], num), KD_THREADS, 0, st>>>(seqs, it, gate->max_d2);
+        else kd_residual_batch_kernel<<<dim3(grid[0], num), KD_THREADS, 0, st>>>(seqs, it);
         PLS_CHECK_LAUNCH();
     }
 }

@@ -195,6 +195,33 @@ __device__ __forceinline__ int warp_candidate(int incl, int adj /* = start - exc
     return __shfl_sync(FULL, adj, c) + t;
 }
 
+// The squared distance of a transformed query p to its match q in float64, every operation rounded on its own (no
+// contraction): ((dx dx + dy dy) + dz dz), dx = (double)p_x - (double)q_x -- numpy's element-wise float64 bits.
+__device__ __forceinline__ double match_d2_f64(const float* p, const float4& q) {
+    const double dx = __dsub_rn((double)p[0], (double)q.x);
+    const double dy = __dsub_rn((double)p[1], (double)q.y);
+    const double dz = __dsub_rn((double)p[2], (double)q.z);
+    return __dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz));
+}
+
+// The correspondence gate of a gated registration (pls_register_scans_gated): a query p whose exact 1-NN q has
+// match_d2_f64(p, q) <= max_d2 is an inlier; every other query is an outlier and has no match.
+//   g2    G, the float32 bound of the search: every inlier's float32 d^2 (dist2_point) is strictly below it.
+//         Derivation (u = 2^-24, s = the exact squared distance of the two float32 points):
+//           float64: dx = (p_x - q_x)(1 + e), |e| <= 2^-53, then three products and two sums, each rounded once, so
+//                    match_d2_f64 >= s (1 - 2^-53)^5 and an inlier has s <= max_d2 (1 + 6 2^-53);
+//           float32: the difference of two floats is rounded once (exact when subnormal); dist2_point squares and sums
+//                    with at most three more roundings whatever the FMA contraction, so
+//                    dist2_point <= s (1 + u)^5 + 3 2^-150 (underflow) <= s (1 + 5.01 u) + 2^-147;
+//           together dist2_point < max_d2 (1 + 2^-20) + 2^-126, with room: 5.01 u + 6 2^-53 < 2^-20 / 3.
+//         kd_gate_of rounds that bound up to float32 (+inf once it passes FLT_MAX: the search is never cut short).
+//   dmax  max_distance rounded up to float32 (+inf above FLT_MAX): the outlier proof of match_proven<true>.
+struct KdGate {
+    double max_d2;
+    float g2;
+    float dmax;
+};
+
 // Exact 1-NN of (x, y, z) by the whole warp; every lane returns the same sorted position (-1 if the map is empty).
 // `hint` (a sorted position or -1, warp-uniform) only seeds the pruning bound; its load overlaps the level-0 probes.
 // *cand_out (optional) accumulates the number of candidates tested.
@@ -202,8 +229,15 @@ __device__ __forceinline__ int warp_candidate(int incl, int adj /* = start - exc
 // (the runner-up inside the scanned block, the boxes of the cells that were pruned, the block's exactness radius):
 // as long as the query moves by less than the gap between the two, the winner stays the nearest neighbour -- the next
 // ICP iterations verify that instead of searching again (kd_icp_refine_kernel).
+// GATE (a gated registration, KdGate): the climb also stops at the first level whose exactness radius r2 is at least
+// G = gate.g2.  Every inlier's float32 d^2 is below G, so an inlier lies inside that block and the search ends at the
+// very level -- with the very match and runner-up bound -- of the ungated search; a winner beyond r2 is then an outlier,
+// and so is every point outside the block.  An outlier (no candidate, or match_d2_f64 > max_d2) returns -1, and
+// *second_out becomes a lower bound of the squared distance to EVERY map point: min(best, runner-up bound).  A level
+// whose table overflowed (r2 < 0) proves nothing and never stops the climb.
+template <bool GATE = false>
 __device__ __forceinline__ int warp_nearest(const KdIndex& ix, const KdGridLocal& g, float x, float y, float z, int hint,
-                                            int lane, int* cand_out, float* second_out) {
+                                            int lane, int* cand_out, float* second_out, KdGate gate = KdGate{}) {
     float best = FLT_MAX, second = FLT_MAX;
     int best_i = -1;
     float4 hp = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -257,6 +291,15 @@ __device__ __forceinline__ int warp_nearest(const KdIndex& ix, const KdGridLocal
             if (level == 0) kd_stat(ix, (best_i >= 0 && best <= r2) ? 1 : 2);
         }
         if (best_i >= 0 && best <= r2) break;
+        if constexpr (GATE)
+            if (r2 >= gate.g2) break;
+    }
+    if constexpr (GATE) {
+        const float p[3] = {x, y, z};
+        if (best_i < 0 || !(match_d2_f64(p, __ldg(ix.sorted + best_i)) <= gate.max_d2)) {
+            second = fminf(best, second);
+            best_i = -1;
+        }
     }
     if (second_out) *second_out = second;
     return best_i;

@@ -1003,14 +1003,19 @@ void odometry_reset(pls_context* ctx) {
 // packed, in chunks of PLS_MAX_SEQUENCES.  kd map: registration b reads scans[b].  Projective map: every registration
 // reads the scan in ctx->query_ptr, bound n.  Outputs and status as pls_register_hypotheses; afterwards the last
 // registration is ctx's last search and last ICP result, as if pls_register_frame had run it last.
+// max_distance (kd map): the gate of pls_register_scans_gated, +inf for none; out_inliers [B] (nullable): each
+// registration's count accumulator of its last executed iteration, its inliers there.  A gated registration whose last
+// iteration had no inlier reports PLS_E_SINGULAR: its sums are all zero, which the solve's zero-residual test would
+// otherwise report as PLS_W_TINY_RESIDUAL, the flag of a near-perfect fit.
 static void register_batch(pls_context* ctx, const KdScan* scans, int64_t n, const float* T0_dev, int B, float* out_T,
-                           float* out_params, float* out_losses, int* out_iters, int* out_status) {
+                           float* out_params, float* out_losses, int* out_iters, int* out_status,
+                           double max_distance = HUGE_VAL, int* out_inliers = nullptr) {
     const bool kd = ctx->cfg.local_map_type == PLS_MAP_KDTREE;
     cudaStream_t st = ctx->stream;
     const int M = ctx->cfg.max_num_alignments;
     std::vector<FrameResult> h((size_t)PLS_MAX_SEQUENCES);
     std::vector<float> T((size_t)B * 16), params((size_t)B * 6), losses((size_t)B * M);
-    std::vector<int> iters((size_t)B), status((size_t)B);
+    std::vector<int> iters((size_t)B), status((size_t)B), inliers((size_t)B);
     int first_error = PLS_OK, last = 0;
     for (int c0 = 0; c0 < B; c0 += PLS_MAX_SEQUENCES) {  // chunks of at most PLS_MAX_SEQUENCES registrations
         const int num = B - c0 < PLS_MAX_SEQUENCES ? B - c0 : PLS_MAX_SEQUENCES;
@@ -1024,7 +1029,8 @@ static void register_batch(pls_context* ctx, const KdScan* scans, int64_t n, con
         // every registration has ctx's settings: icp_rounds sees num copies of ctx
         std::vector<pls_context*> same((size_t)num, ctx);
         if (kd)
-            icp_rounds(same.data(), num, [&](int a, int b) { kdmap_batch_iterations(ctx, num, st, grid, a, b); },
+            icp_rounds(same.data(), num,
+                       [&](int a, int b) { kdmap_batch_iterations(ctx, num, st, grid, a, b, max_distance); },
                        [&](int* done) { kdmap_batch_done(ctx, num, st, done); });
         else
             icp_rounds(same.data(), num, [&](int a, int b) { projmap_hypotheses_iterations(ctx, n, num, st, a, b); },
@@ -1039,7 +1045,9 @@ static void register_batch(pls_context* ctx, const KdScan* scans, int64_t n, con
             memcpy(&losses[(size_t)M * b], r.losses, (size_t)M * sizeof(float));
             iters[b] = r.iters;
             status[b] = r.status;
-            if (first_error == PLS_OK && (r.status == PLS_E_SINGULAR || r.status == PLS_E_COMM)) first_error = r.status;
+            inliers[b] = (int)r.last_sums[29];
+            if (!isinf(max_distance) && inliers[b] == 0) status[b] = PLS_E_SINGULAR;
+            if (first_error == PLS_OK && (status[b] == PLS_E_SINGULAR || r.status == PLS_E_COMM)) first_error = status[b];
         }
         last = num - 1;
     }
@@ -1052,6 +1060,7 @@ static void register_batch(pls_context* ctx, const KdScan* scans, int64_t n, con
     put_out(out_losses, losses.data(), losses.size() * sizeof(float));
     put_out(out_iters, iters.data(), iters.size() * sizeof(int));
     put_out(out_status, status.data(), status.size() * sizeof(int));
+    put_out(out_inliers, inliers.data(), inliers.size() * sizeof(int));
     if (!out_status) raise_status(ctx, first_error);
 }
 
@@ -1185,25 +1194,45 @@ int pls_register_hypotheses(pls_context* ctx, const float* points, int64_t n, co
     PLS_API_END(ctx)
 }
 
+// pls_register_scans and pls_register_scans_gated (fn names the entry point in refusals).
+static void register_scans(pls_context* ctx, const char* fn, const float* const* scans, const int64_t* n, int S,
+                           const int* scan_of, const float* T0s, int B, double max_distance, float* out_T,
+                           float* out_params, float* out_losses, int* out_iters, int* out_status, int* out_inliers) {
+    const std::string f(fn);
+    // every argument is checked before anything is enqueued: a refused call changes nothing
+    PLS_REQUIRE(ctx->cfg.local_map_type == PLS_MAP_KDTREE, f + ": needs a kd-tree local map");
+    PLS_REQUIRE(ctx->cfg.gn_max_iters == 1, "fused ICP path supports gauss_newton_config.max_iters == 1");
+    PLS_REQUIRE(!ctx->comm, f + ": a context with a multi-GPU communicator is not supported");
+    PLS_REQUIRE(ctx->kd.valid, "kd map: search before any update");
+    PLS_REQUIRE(scans && n && S > 0, f + ": scans and n must hold S > 0 scans");
+    PLS_REQUIRE(T0s && B > 0, f + ": T0s must be [B,16] with B > 0");
+    PLS_REQUIRE(scan_of || B == S, f + ": without scan_of, B must equal S");
+    PLS_REQUIRE(max_distance >= 0.0, f + ": max_distance must be >= 0 (not NaN)");
+    for (int s = 0; s < S; ++s) PLS_REQUIRE(scans[s] && n[s] > 0, f + ": every scan must be [n,3] with n > 0");
+    for (int b = 0; scan_of && b < B; ++b)
+        PLS_REQUIRE(scan_of[b] >= 0 && scan_of[b] < S, f + ": scan_of entries must lie in [0, S)");
+    map_stream_wait(ctx);
+    const std::vector<KdScan> regs = stage_scans(ctx, scans, n, S, scan_of, B);
+    const float* T0_dev = (const float*)to_device(ctx, T0s, (size_t)B * 16 * sizeof(float), ctx->stage_in[1]);
+    register_batch(ctx, regs.data(), 0, T0_dev, B, out_T, out_params, out_losses, out_iters, out_status, max_distance,
+                   out_inliers);
+}
+
 int pls_register_scans(pls_context* ctx, const float* const* scans, const int64_t* n, int S, const int* scan_of,
                        const float* T0s, int B, float* out_T, float* out_params, float* out_losses, int* out_iters,
                        int* out_status) {
     PLS_API_BEGIN(ctx)
-    // every argument is checked before anything is enqueued: a refused call changes nothing
-    PLS_REQUIRE(ctx->cfg.local_map_type == PLS_MAP_KDTREE, "pls_register_scans: needs a kd-tree local map");
-    PLS_REQUIRE(ctx->cfg.gn_max_iters == 1, "fused ICP path supports gauss_newton_config.max_iters == 1");
-    PLS_REQUIRE(!ctx->comm, "pls_register_scans: a context with a multi-GPU communicator is not supported");
-    PLS_REQUIRE(ctx->kd.valid, "kd map: search before any update");
-    PLS_REQUIRE(scans && n && S > 0, "pls_register_scans: scans and n must hold S > 0 scans");
-    PLS_REQUIRE(T0s && B > 0, "pls_register_scans: T0s must be [B,16] with B > 0");
-    PLS_REQUIRE(scan_of || B == S, "pls_register_scans: without scan_of, B must equal S");
-    for (int s = 0; s < S; ++s) PLS_REQUIRE(scans[s] && n[s] > 0, "pls_register_scans: every scan must be [n,3] with n > 0");
-    for (int b = 0; scan_of && b < B; ++b)
-        PLS_REQUIRE(scan_of[b] >= 0 && scan_of[b] < S, "pls_register_scans: scan_of entries must lie in [0, S)");
-    map_stream_wait(ctx);
-    const std::vector<KdScan> regs = stage_scans(ctx, scans, n, S, scan_of, B);
-    const float* T0_dev = (const float*)to_device(ctx, T0s, (size_t)B * 16 * sizeof(float), ctx->stage_in[1]);
-    register_batch(ctx, regs.data(), 0, T0_dev, B, out_T, out_params, out_losses, out_iters, out_status);
+    register_scans(ctx, "pls_register_scans", scans, n, S, scan_of, T0s, B, HUGE_VAL, out_T, out_params, out_losses,
+                   out_iters, out_status, nullptr);
+    PLS_API_END(ctx)
+}
+
+int pls_register_scans_gated(pls_context* ctx, const float* const* scans, const int64_t* n, int S, const int* scan_of,
+                             const float* T0s, int B, double max_distance, float* out_T, float* out_params,
+                             float* out_losses, int* out_iters, int* out_status, int* out_inliers) {
+    PLS_API_BEGIN(ctx)
+    register_scans(ctx, "pls_register_scans_gated", scans, n, S, scan_of, T0s, B, max_distance, out_T, out_params,
+                   out_losses, out_iters, out_status, out_inliers);
     PLS_API_END(ctx)
 }
 

@@ -138,6 +138,17 @@ def _check_given_normals(ctx):
         raise IndexError(_NORMALS_INDEX_ERROR)
 
 
+def _gated(ctx, max_distance) -> bool:
+    """Whether max_distance asks for a gated registration; refuses a NaN or negative gate, and a finite one on a
+    projective map, before any call."""
+    d = float(max_distance)
+    assert_debug(d >= 0.0, "max_distance must be >= 0 (not NaN)")
+    if np.isinf(d):
+        return False
+    assert_debug(ctx.cfg.local_map_type == _lib.MAP_KDTREE, "a finite max_distance needs a kd-tree local map")
+    return True
+
+
 # Pose count A*(2*half_x+1)*(2*half_y+1) from which _pose_search takes pls_kdmap_pose_search_pyramid (branch and
 # bound) instead of scoring every pose with pls_kdmap_pose_search.  Measured on an H100 SXM at 700 W, K = 8, 72 yaws
 # (profiles/h100_pose_search_pyramid.json, DESIGN section 18): up to 30 M poses the exhaustive call is faster in all
@@ -1074,7 +1085,7 @@ class ICPFrameToModel(OdometryAlgorithm):
                       _lib.ptr(losses), C.byref(iters))
         return params, T, list(losses[:iters.value])
 
-    def register_new_frame_hypotheses(self, target_points, initial_estimates):
+    def register_new_frame_hypotheses(self, target_points, initial_estimates, max_distance: float = np.inf):
         """register_new_frame for B initial estimates [B,4,4] of one scan [n,3], in one call (pls_register_hypotheses;
         no reference counterpart): relocalisation in a prior map registers a scan from many guesses -- a yaw sweep, a
         grid of positions, place-recognition candidates -- and keeps the best converged result.  Registers against the
@@ -1084,7 +1095,17 @@ class ICPFrameToModel(OdometryAlgorithm):
         Returns (params [B,6], T [B,4,4], losses: B lists, iterations [B]); hypothesis b's are what
         register_new_frame(target_points, initial_estimates[b]) returns, bit for bit.  A singular hypothesis does not
         stop the others: it is logged, and last_hypotheses_status[b] holds each one's status (PLS_OK,
-        PLS_W_TINY_RESIDUAL or PLS_E_SINGULAR)."""
+        PLS_W_TINY_RESIDUAL or PLS_E_SINGULAR).
+        max_distance gates the correspondences as in register_new_frames (kd map only: a finite gate on a projective
+        map raises before any call).  Gated, the hypotheses are what register_new_frames([target_points],
+        initial_estimates, zeros, max_distance) returns, and last_hypotheses_inliers[b] holds each one's inlier count in
+        its last iteration (None when ungated).  The last_registrations_* attributes are left as they are."""
+        if _gated(self.ctx, max_distance):
+            params, T, losses, iters, self.last_hypotheses_status, self.last_hypotheses_inliers = \
+                self._register_scans([target_points], initial_estimates, np.zeros(len(initial_estimates), np.int32),
+                                     max_distance, "hypotheses")
+            return params, T, losses, iters
+        self.last_hypotheses_inliers = None
         _check_given_normals(self.ctx)
         check_tensor(target_points, [-1, 3])
         pts = _f32c(target_points)
@@ -1107,14 +1128,15 @@ class ICPFrameToModel(OdometryAlgorithm):
         return params, T, [list(losses[b, :iters[b]]) for b in range(B)], iters
 
     def localize(self, scan, prior_pose, radius: float, cell_size: float, yaw_range: float = np.pi,
-                 yaw_step: float = np.deg2rad(5), num_candidates: int = 8):
+                 yaw_step: float = np.deg2rad(5), num_candidates: int = 8, max_distance: float = np.inf):
         """Finds the pose of `scan` [n,3] on the kd map this odometry's context holds (e.g. loaded with
         KdTreeLocalMap(ctx=self.ctx).set_map_pointcloud) from a coarse prior: start-up on a stored map, recovery after
         odometry is lost.  No reference counterpart.
         1. bases = yaw_sweep(prior_pose, yaw_range, yaw_step);
         2. a correlative search of those bases moved by up to ceil(radius / cell_size) cells along x and y
            (KdTreeLocalMap.search_poses) keeps num_candidates local maxima;
-        3. one register_new_frame_hypotheses call refines them from their float32-rounded poses;
+        3. one register_new_frame_hypotheses call refines them from their float32-rounded poses, with the
+           correspondence gate max_distance (inf: none; the search and the rescoring are not gated);
         4. score_poses rescores the refined poses.
         The search in step 2 is exact at any radius, and a large one is searched by branch and bound, so `radius` may
         span the whole map when the position is unknown.
@@ -1124,26 +1146,28 @@ class ICPFrameToModel(OdometryAlgorithm):
         _check_given_normals(self.ctx)
         assert_debug(np.isfinite(radius) and radius >= 0, "radius must be finite and >= 0")
         assert_debug(np.isfinite(cell_size) and cell_size > 0, "cell_size must be finite and > 0")
+        _gated(self.ctx, max_distance)   # refused before the search
         bases = yaw_sweep(prior_pose, yaw_range, yaw_step)
         half = int(np.ceil(radius / cell_size))
         T0, coarse, _ = _pose_search(self.ctx, scan, bases, cell_size, half, half, num_candidates)
         if T0.shape[0] == 0:
             return []
-        _, T, _, iters = self.register_new_frame_hypotheses(scan, T0.astype(np.float32))
+        _, T, _, iters = self.register_new_frame_hypotheses(scan, T0.astype(np.float32), max_distance)
         status = self.last_hypotheses_status
         scores = _score_poses(self.ctx, scan, T.astype(np.float64), cell_size)
         return _pose_candidates(T0, coarse, T, iters, status, scores)
 
     def localize_scans(self, scans, prior_poses, radius, cell_size: float, yaw_range: float = np.pi,
-                       yaw_step: float = np.deg2rad(5), num_candidates: int = 8):
+                       yaw_step: float = np.deg2rad(5), num_candidates: int = 8, max_distance: float = np.inf):
         """localize for S scans on the one kd map this odometry's context holds (no reference counterpart): a
         localisation server re-localising many vehicles' scans, offline map matching a recorded drive's scans from
         GNSS fixes.  scans: S [n_s,3] arrays or tensors; prior_poses [S,4,4]; radius a scalar or [S].
         One batched search over every scan's yaw_sweep bases (KdTreeLocalMap.search_poses_scans), one
         register_new_frames call over every candidate, one batched rescoring of the refined poses.  Returns S lists of
         PoseCandidate; list s equals localize(scans[s], prior_poses[s], radius[s], cell_size, yaw_range, yaw_step,
-        num_candidates), field for field."""
+        num_candidates, max_distance), field for field; max_distance gates the refinement only."""
         _check_given_normals(self.ctx)
+        _gated(self.ctx, max_distance)   # refused before the search
         S = len(scans)
         if isinstance(prior_poses, torch.Tensor):
             prior_poses = prior_poses.detach().cpu().numpy()
@@ -1159,7 +1183,7 @@ class ICPFrameToModel(OdometryAlgorithm):
             return [[] for _ in range(S)]
         T0_all = np.concatenate([T0 for T0, _, _ in found])
         _, T, _, iters = self.register_new_frames(scans, T0_all.astype(np.float32),
-                                                  np.repeat(np.arange(S, dtype=np.int32), counts))
+                                                  np.repeat(np.arange(S, dtype=np.int32), counts), max_distance)
         status = self.last_registrations_status
         hit = [s for s in range(S) if counts[s]]
         first = np.concatenate([[0], np.cumsum(counts)])
@@ -1174,7 +1198,7 @@ class ICPFrameToModel(OdometryAlgorithm):
                        else [])
         return out
 
-    def register_new_frames(self, scans, initial_estimates, scan_indices=None):
+    def register_new_frames(self, scans, initial_estimates, scan_indices=None, max_distance: float = np.inf):
         """register_new_frame for many scans against the one map this odometry's context holds, in one call
         (pls_register_scans; no reference counterpart): a localisation server registers many vehicles' scans on one
         city map, offline map matching registers a recorded drive's scans on a prior map.  `scans` is a list of S
@@ -1184,21 +1208,42 @@ class ICPFrameToModel(OdometryAlgorithm):
         Returns (params [B,6], T [B,4,4], losses: B lists, iterations [B]); registration b's are what
         register_new_frame(scans[scan_indices[b]], initial_estimates[b]) returns, bit for bit.  A singular registration
         does not stop the others: it is logged, and last_registrations_status[b] holds each one's status (PLS_OK,
-        PLS_W_TINY_RESIDUAL or PLS_E_SINGULAR)."""
+        PLS_W_TINY_RESIDUAL or PLS_E_SINGULAR).
+        A finite max_distance gates the correspondences (pls_register_scans_gated): in every ICP iteration a valid row
+        is an inlier when the float64 squared distance to its exact nearest map point is at most max_distance**2, and
+        only inliers enter the normal equations, the loss and the count, so a stale prior map -- moved cars,
+        construction, partial overlap -- cannot pull the pose towards far matches.  A registration left with too few
+        inliers, or none, ends singular (PLS_E_SINGULAR) without stopping the others.  last_registrations_inliers[b]
+        then holds registration b's inlier count in its last iteration (None when ungated).  max_distance = inf, the
+        default, makes the ungated call, bit for bit as before; NaN or a negative gate raises before any call."""
+        params, T, losses, iters, self.last_registrations_status, self.last_registrations_inliers = \
+            self._register_scans(scans, initial_estimates, scan_indices, max_distance, "registrations")
+        return params, T, losses, iters
+
+    def _register_scans(self, scans, initial_estimates, scan_indices, max_distance, what):
+        """register_new_frames' call: (params, T, losses, iterations, status, inliers or None), singular ones logged
+        as `what`."""
+        gated = _gated(self.ctx, max_distance)
         pts, addresses, rows, T0, index = self._scans_args(scans, initial_estimates, scan_indices)
         B, S, M = T0.shape[0], len(pts), int(self.config.max_num_alignments)
         T, params = np.zeros((B, 4, 4), np.float32), np.zeros((B, 6), np.float32)
         losses = np.zeros((B, M), np.float32)
         iters, status = np.zeros(B, np.int32), np.zeros(B, np.int32)
-        self.ctx.call("pls_register_scans", _lib.ptr(addresses), _lib.ptr(rows), S, _lib.ptr(index), _lib.ptr(T0), B,
-                      _lib.ptr(T), _lib.ptr(params), _lib.ptr(losses), _lib.ptr(iters), _lib.ptr(status))
-        self.last_registrations_status = status
+        inliers = None
+        if gated:
+            inliers = np.zeros(B, np.int32)
+            self.ctx.call("pls_register_scans_gated", _lib.ptr(addresses), _lib.ptr(rows), S, _lib.ptr(index),
+                          _lib.ptr(T0), B, float(max_distance), _lib.ptr(T), _lib.ptr(params), _lib.ptr(losses),
+                          _lib.ptr(iters), _lib.ptr(status), _lib.ptr(inliers))
+        else:
+            self.ctx.call("pls_register_scans", _lib.ptr(addresses), _lib.ptr(rows), S, _lib.ptr(index), _lib.ptr(T0),
+                          B, _lib.ptr(T), _lib.ptr(params), _lib.ptr(losses), _lib.ptr(iters), _lib.ptr(status))
         singular = np.flatnonzero(status == _lib.PLS_E_SINGULAR)
         if singular.size:
             import logging
             logging.error(f"Invalid Jacobian in Gauss Newton minimization, the hessian is not invertible "
-                          f"(registrations {singular.tolist()})")
-        return params, T, [list(losses[b, :iters[b]]) for b in range(B)], iters
+                          f"({what} {singular.tolist()})")
+        return params, T, [list(losses[b, :iters[b]]) for b in range(B)], iters, status, inliers
 
     def _scans_args(self, scans, poses, scan_indices):
         """register_new_frames' and evaluate_registrations' inputs as pls_register_scans / pls_kdmap_evaluate_poses
