@@ -385,6 +385,40 @@ PLS_API int pls_register_scans_gated(pls_context* ctx, const float* const* scans
                                      const int* scan_of, const float* T0s, int B, double max_distance, float* out_T,
                                      float* out_params, float* out_losses, int* out_iters, int* out_status,
                                      int* out_inliers);
+/* pls_register_scans_gated with a solve that acts only in the directions the map constrains (no reference counterpart:
+ * a tunnel, a corridor, an underpass or an open field leaves some directions of the pose unconstrained, and an ICP
+ * step along them is driven by noise, or makes the registration singular).  This is the solution remapping of Zhang,
+ * Kaess and Singh ("On degeneracy of optimization-based state estimation problems", ICRA 2016), which for a
+ * Gauss-Newton step taken from the current pose is a truncated eigen-solve.  Arguments, staging, pointer rules,
+ * chunking, outputs and the context's state afterwards are those of pls_register_scans_gated (max_distance = +inf: no
+ * gate), plus min_eigenvalue, out_degenerate and out_eigenvalues.
+ * Unchanged: the matches, normals and the 30 accumulators of every iteration are exactly those the gated call (at
+ * +inf, pls_register_scans) forms at that iteration's pose; iteration 0's entries 0..29 are, bit for bit,
+ * pls_kdmap_evaluate_poses's row at the initial pose and the same max_distance.  Only the solve differs.  For the sums
+ * s of iteration i:
+ *   H        the symmetric 6x6 matrix of the 21 upper-triangle entries s[0..20]; g = s[21..26]; N = s[29], the inlier
+ *            (or match) count;
+ *   (l_k, v_k)  the eigen-decomposition of H, in float64 on the device (cyclic Jacobi);
+ *   kept     direction k when N > 0 and l_k >= min_eigenvalue * N in float64; otherwise it is degenerate;
+ *   step     dx = -sum over the kept k of v_k (v_k^T g) / l_k, then the float32 cast, the threshold_delta_pose stop test
+ *            and the pose update of pls_register_scans.  Along a degenerate direction the pose keeps its estimate.
+ * Status: N = 0 is PLS_E_SINGULAR; then the tiny-residual rule (sqrt(s[28]) < 1e-7: PLS_W_TINY_RESIDUAL) as before;
+ * then PLS_E_SINGULAR when no direction is kept -- this replaces the |det| >= 1e-7 test.  A finite gate with no inlier
+ * in the last iteration is PLS_E_SINGULAR, as in pls_register_scans_gated.
+ * out_degenerate [B] (nullable, host or device): the number of degenerate directions in registration b's last executed
+ * iteration.  out_eigenvalues [B,6] (nullable, host or device): the ascending eigenvalues of H / N in that iteration
+ * (zeros when N = 0).
+ * Units: the threshold mixes them, as Zhang's does.  Per point, H's translation block is dimensionless -- at most 1
+ * under the unweighted scheme, as it sums n n^T over unit normals -- and its rotation block is in m^2 (it grows with the
+ * square of the points' range).  Calibrate min_eigenvalue on your own map from pls_kdmap_evaluate_poses's
+ * (evaluate_registrations') eigenvalues / inliers, which is the same quantity as out_eigenvalues.
+ * PLS_E_INVALID before any work, the context unchanged: everything pls_register_scans_gated refuses, and a
+ * min_eigenvalue that is NaN, <= 0 or infinite. */
+PLS_API int pls_register_scans_degeneracy(pls_context* ctx, const float* const* scans, const int64_t* n, int S,
+                                          const int* scan_of, const float* T0s, int B, double max_distance,
+                                          double min_eigenvalue, float* out_T, float* out_params, float* out_losses,
+                                          int* out_iters, int* out_status, int* out_inliers, int* out_degenerate,
+                                          double* out_eigenvalues);
 /* The quality of B registrations on the kd map ctx holds, in one call (no reference counterpart: a localiser that feeds
  * a filter or a pose graph needs each registration's inlier fraction, inlier RMSE and information matrix, and a
  * re-ranking of pose candidates needs more than an occupancy score).  Arguments, staging and pointer rules are those

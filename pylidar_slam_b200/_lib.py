@@ -88,6 +88,7 @@ _SIGNATURES = {
     "pls_register_hypotheses": [_P, _P, _L, _P, _I, _P, _P, _P, _P, _P],
     "pls_register_scans": [_P, _P, _P, _I, _P, _P, _I, _P, _P, _P, _P, _P],
     "pls_register_scans_gated": [_P, _P, _P, _I, _P, _P, _I, _D, _P, _P, _P, _P, _P, _P],
+    "pls_register_scans_degeneracy": [_P, _P, _P, _I, _P, _P, _I, _D, _D, _P, _P, _P, _P, _P, _P, _P, _P],
     "pls_kdmap_evaluate_poses": [_P, _P, _P, _I, _P, _P, _I, _D, _P],
     "pls_process_frame": [_P, _P, _I, _L, _P, _P, _P, C.POINTER(_I), _P],
     "pls_process_frame_grid_sample": [_P, _P, _L, _D, _I, _P, _P, _P, C.POINTER(_I), _P],

@@ -104,4 +104,117 @@ __host__ __device__ inline void smallest_eigenvector(const float* c, float* n) {
     if (!smallest_eigenvector_closed_form(c, n)) smallest_eigenvector_jacobi(c, n);
 }
 
+// Eigen-decomposition of a symmetric 6x6 matrix by cyclic Jacobi in float64: A [36] (row-major, both triangles) is
+// overwritten, V [36] receives the eigenvectors as columns and w [6] the eigenvalues, ascending (V's columns in the
+// same order).  The normal-equation matrix J^T W J of a registration is what it is for: its translation and rotation
+// entries differ by the square of the scene's radius, and its degenerate directions have eigenvalues at or near 0.
+//   * rotation order: the pairs (p, q), p < q, row by row, in every sweep;
+//   * a pair is skipped, its entry set to 0, when |a_pq| <= 2^-53 sqrt(|a_pp|) sqrt(|a_qq|) (0 when a diagonal entry is
+//     0).  This relative rule keeps the small eigenvalues of a positive semi-definite matrix accurate to their own size
+//     (Demmel and Veselic, "Jacobi's method is more accurate than QR", 1992), so a tiny eigenvalue of a strongly scaled
+//     matrix is not drowned by the rounding of its large ones;
+//   * it stops after the first sweep that rotates nothing, or after EIGEN6_SWEEPS sweeps;
+//   * ties in the ordering keep the lower index first.
+// A and V are pointers so that a device caller can keep them in shared memory: in registers, one thread's 72 doubles
+// would spill under a 128-register cap.  The same code on the same inputs gives the same bits on every call.
+constexpr int EIGEN6_SWEEPS = 30;
+__host__ __device__ inline void eigen6_jacobi(double* A, double* V, double* w) {
+    for (int i = 0; i < 36; ++i) V[i] = (i % 7 == 0) ? 1.0 : 0.0;
+#pragma unroll 1
+    for (int sweep = 0; sweep < EIGEN6_SWEEPS; ++sweep) {
+        bool rotated = false;
+#pragma unroll 1
+        for (int p = 0; p < 5; ++p) {
+#pragma unroll 1
+            for (int q = p + 1; q < 6; ++q) {
+                const double apq = A[p * 6 + q];
+                if (apq == 0.0) continue;
+                const double app = A[p * 6 + p], aqq = A[q * 6 + q];
+                if (fabs(apq) <= 0x1p-53 * (sqrt(fabs(app)) * sqrt(fabs(aqq)))) {
+                    A[p * 6 + q] = 0.0;
+                    A[q * 6 + p] = 0.0;
+                    continue;
+                }
+                rotated = true;
+                // the rotation that zeroes a_pq (t = tan of its angle, the smaller root)
+                const double theta = (aqq - app) / (2.0 * apq);
+                const double t = fabs(theta) > 1e150 ? 0.5 / theta
+                                                     : (theta >= 0.0 ? 1.0 : -1.0) / (fabs(theta) + sqrt(theta * theta + 1.0));
+                const double c = 1.0 / sqrt(t * t + 1.0), s = t * c;
+                A[p * 6 + p] = app - t * apq;
+                A[q * 6 + q] = aqq + t * apq;
+                A[p * 6 + q] = 0.0;
+                A[q * 6 + p] = 0.0;
+#pragma unroll 1
+                for (int r = 0; r < 6; ++r) {
+                    if (r != p && r != q) {
+                        const double arp = A[r * 6 + p], arq = A[r * 6 + q];
+                        const double np = c * arp - s * arq, nq = s * arp + c * arq;
+                        A[r * 6 + p] = np;
+                        A[p * 6 + r] = np;
+                        A[r * 6 + q] = nq;
+                        A[q * 6 + r] = nq;
+                    }
+                    const double vrp = V[r * 6 + p], vrq = V[r * 6 + q];
+                    V[r * 6 + p] = c * vrp - s * vrq;
+                    V[r * 6 + q] = s * vrp + c * vrq;
+                }
+            }
+        }
+        if (!rotated) break;
+    }
+    // insertion sort of the diagonal, V's columns with it: stable, so equal eigenvalues keep their order
+#pragma unroll 1
+    for (int i = 1; i < 6; ++i)
+#pragma unroll 1
+        for (int j = i; j > 0 && A[j * 7] < A[(j - 1) * 7]; --j) {
+            const double d = A[j * 7];
+            A[j * 7] = A[(j - 1) * 7];
+            A[(j - 1) * 7] = d;
+            for (int r = 0; r < 6; ++r) {
+                const double v = V[r * 6 + j];
+                V[r * 6 + j] = V[r * 6 + j - 1];
+                V[r * 6 + j - 1] = v;
+            }
+        }
+    for (int k = 0; k < 6; ++k) w[k] = A[k * 7];
+}
+
+// The Gauss-Newton step of an ICP iteration restricted to the directions the map constrains (Zhang, Kaess and Singh,
+// "On degeneracy of optimization-based state estimation problems", ICRA 2016, whose solution remapping is this
+// truncated eigen-solve for a step taken from the current pose).  sums: the 30 accumulators of the iteration (21 upper
+// entries of H = J^T W J, g = J^T W r, ..., the count N in sums[29]).  With (lambda_k, v_k) the eigen-pairs of H
+// (eigen6_jacobi), direction k is kept when N > 0 and lambda_k >= min_eigenvalue * N, and
+//   dx = -sum over the kept k, ascending, of v_k (v_k^T g) / lambda_k.
+// Returns the number of kept directions (0: dx is all zeros); lambda_n [6] receives the ascending eigenvalues of H / N
+// (zeros when N = 0).  A, V: [36] scratch, as eigen6_jacobi's.
+__host__ __device__ inline int solve6_projected(const double* sums, double min_eigenvalue, double* A, double* V,
+                                                double* dx, double* lambda_n) {
+    {
+        int k = 0;
+        for (int i = 0; i < 6; ++i)
+            for (int j = i; j < 6; ++j) {
+                A[i * 6 + j] = sums[k];
+                A[j * 6 + i] = sums[k];
+                ++k;
+            }
+    }
+    eigen6_jacobi(A, V, lambda_n);  // H's eigenvalues, divided by N below
+    const double N = sums[29];
+    const double thr = min_eigenvalue * N;
+    for (int i = 0; i < 6; ++i) dx[i] = 0.0;
+    int kept = 0;
+    for (int k = 0; k < 6; ++k) {
+        const double w = lambda_n[k];
+        lambda_n[k] = N > 0.0 ? w / N : 0.0;
+        if (!(N > 0.0 && w >= thr)) continue;
+        ++kept;
+        double vg = 0.0;
+        for (int i = 0; i < 6; ++i) vg += V[i * 6 + k] * sums[21 + i];
+        const double a = vg / w;
+        for (int i = 0; i < 6; ++i) dx[i] -= V[i * 6 + k] * a;
+    }
+    return kept;
+}
+
 }  // namespace pls

@@ -1,6 +1,7 @@
 // Device-side tail of an ICP iteration, shared by the stand-alone step kernels (odometry.cu) and the
 // correspondence kernels that finish the iteration in their last block (kdmap.cu).
 #pragma once
+#include "eigen_device.cuh"
 #include "internal.cuh"
 #include "pose_device.cuh"
 
@@ -72,10 +73,37 @@ __device__ __forceinline__ void sum_partials_256(const double* __restrict__ part
     }
 }
 
+// The eigenvalue-thresholded solve of a registration (pls_register_scans_degeneracy), a launch argument of the kernels
+// that finish an iteration: the threshold, and where the iteration writes the registration's ICP_DEGEN_STRIDE doubles --
+// the ascending eigenvalues of H / N, then the number of degenerate directions.  Not a FrameResult field: its stride is
+// read by the kernels of every other path.
+constexpr int ICP_DEGEN_STRIDE = 8;
+struct IcpDegen {
+    double min_eigenvalue;
+    double* out;      // [ICP_DEGEN_STRIDE]
+    double* scratch;  // [72] shared memory: the matrix and the eigenvectors of eigen6_jacobi
+};
+
 // The serial tail of an ICP iteration (thread 0): Gauss-Newton guards, 6x6 solve, stop test, pose update.
-__device__ __forceinline__ void icp_solve_and_update(FrameResult* fr, const double* sums, float threshold_delta PLS_SPLIT_ARG) {
+// DEGEN (pls_register_scans_degeneracy): the step is solve6_projected's with dg.min_eigenvalue, in place of solve6's;
+// the iteration is singular when its count N is 0 or no direction is kept, instead of when |det| < 1e-7.  Its
+// eigenvalues of H / N and degenerate count go to dg.out whatever the iteration's outcome.
+template <bool DEGEN = false>
+__device__ __forceinline__ void icp_solve_and_update(FrameResult* fr, const double* sums, float threshold_delta PLS_SPLIT_ARG,
+                                                     IcpDegen dg = IcpDegen{}) {
     const int it = fr->iters;
     fr->iters = it + 1;
+    double dx[6];
+    int kept = 0;
+    if constexpr (DEGEN) {
+        kept = solve6_projected(sums, dg.min_eigenvalue, dg.scratch, dg.scratch + 36, dx, dg.out);
+        dg.out[6] = (double)(6 - kept);
+        if (!(sums[29] > 0.0)) {  // no match, or no inlier: nothing to solve, and all-zero sums are no fit
+            fr->status = PLS_E_SINGULAR;
+            fr->done = 1;
+            return;
+        }
+    }
     // optimization.py:323-327: |r| < 1e-7 -> warning, x stays 0, the residuals are r^2.  The ICP loop then sees delta = 0:
     // it breaks if 0 < threshold_delta_pose (icp_odometry.py:292) and otherwise goes on, the pose unchanged
     // (delta_pose_matrix = I, so `new_pose_matrix` only passes through the Euler round trip again)
@@ -92,13 +120,20 @@ __device__ __forceinline__ void icp_solve_and_update(FrameResult* fr, const doub
         }
         return;
     }
-    double dx[6];
-    const double det = solve6(sums, dx);
-    PLS_SPLIT(7, det + dx[0] + dx[5]);
-    if (!(fabs(det) >= 1e-7)) {  // optimization.py:334-336
-        fr->status = PLS_E_SINGULAR;
-        fr->done = 1;
-        return;
+    if constexpr (DEGEN) {
+        if (kept == 0) {
+            fr->status = PLS_E_SINGULAR;
+            fr->done = 1;
+            return;
+        }
+    } else {
+        const double det = solve6(sums, dx);
+        PLS_SPLIT(7, det + dx[0] + dx[5]);
+        if (!(fabs(det) >= 1e-7)) {  // optimization.py:334-336
+            fr->status = PLS_E_SINGULAR;
+            fr->done = 1;
+            return;
+        }
     }
     fr->losses[it] = (float)sums[27];
     float delta[6];
@@ -138,12 +173,20 @@ __device__ __forceinline__ void icp_step_body(FrameResult* fr, const double* __r
     icp_solve_and_update(fr, sums, threshold_delta);
 }
 
+// The shared memory of icp_solve_and_update<true>'s eigen-solve.  Owned by this function rather than by the template,
+// so that the kernels without DEGEN keep their shared-memory layout and SASS.
+__device__ __forceinline__ double* icp_degen_scratch() {
+    __shared__ double s_eig[72];
+    return s_eig;
+}
+
 // Called by every block of a correspondence kernel (512, 256 or 128 threads) after it stored its partial row: the block
 // that arrives last of the num_blocks (ticket in fr->pad) sums all rows in the fixed order and runs the solve -- one
 // launch and one dependent-launch gap less per ICP iteration than a separate step kernel.
-template <int THREADS = 256>
+// DEGEN: icp_solve_and_update<true> with dg, its scratch in this block's shared memory (icp_degen_scratch).
+template <int THREADS = 256, bool DEGEN = false>
 __device__ __forceinline__ void icp_finish_in_last_block(FrameResult* fr, const double* __restrict__ partials, int num_blocks,
-                                                         float threshold_delta PLS_SPLIT_ARG) {
+                                                         float threshold_delta PLS_SPLIT_ARG, IcpDegen dg = IcpDegen{}) {
     __shared__ int s_last;
     __shared__ double s_sums[NACC];
     if (threadIdx.x == 0) PLS_SPLIT(4);
@@ -163,7 +206,8 @@ __device__ __forceinline__ void icp_finish_in_last_block(FrameResult* fr, const 
     if (threadIdx.x != 0) return;
     PLS_SPLIT(6, s_sums[0] + s_sums[29]);
     fr->pad = 0;
-    icp_solve_and_update(fr, s_sums, threshold_delta PLS_SPLIT_PASS);
+    if constexpr (DEGEN) dg.scratch = icp_degen_scratch();
+    icp_solve_and_update<DEGEN>(fr, s_sums, threshold_delta PLS_SPLIT_PASS, dg);
 }
 
 }  // namespace pls

@@ -260,6 +260,7 @@ struct pls_context {
     pls::DBuf partials;                 // [blocks][NACC] doubles
     pls::DBuf batch_buf;                // pls_process_frames led by this context: sequence descriptors, then done flags
     pls::DBuf hyp_buf;                  // pls_register_hypotheses: FrameResults and per-query state of the hypotheses
+    pls::DBuf degen_buf;                // pls_register_scans_degeneracy: a chunk's eigenvalues and degenerate counts
     cudaEvent_t ev_batch = nullptr;     // pls_process_frames: this context's input stage, before the batched ICP
     cudaEvent_t ev_icp_done = nullptr;  // a frame's ICP launches and its map-update decision, before the map stream's update
     pls::DBuf gs_keys, gs_vals, gs_out_xyz, gs_out_idx;
@@ -451,9 +452,11 @@ constexpr int KD_BATCH_GRID = 6;
 void kdmap_batch_begin(pls_context* lead, pls_context* const* ctxs, const int64_t* query_bounds, int num, cudaStream_t st,
                        int* grid);
 // max_distance (pls_register_scans_gated, registrations only): finite, the iterations run the gated kernels with that
-// gate (KdGate); +inf, the ungated ones.
+// gate (KdGate); +inf, the ungated ones.  min_eigenvalue > 0 (pls_register_scans_degeneracy, registrations only): the
+// gated kernels' twins with the eigenvalue-thresholded solve, at any max_distance; registration j of the batch writes
+// its eigenvalues and degenerate count to degen + ICP_DEGEN_STRIDE j (icp_device.cuh).
 void kdmap_batch_iterations(pls_context* lead, int num, cudaStream_t st, const int* grid, int first, int last,
-                            double max_distance = HUGE_VAL);
+                            double max_distance = HUGE_VAL, double min_eigenvalue = 0.0, double* degen = nullptr);
 void kdmap_batch_done(pls_context* lead, int num, cudaStream_t st, int* out);
 // The scan one registration of pls_register_hypotheses / pls_register_scans reads: its packed float4 queries, their
 // count on the device (u32) and the query bound of its single pls_register_frame call (the scan's row count).

@@ -457,10 +457,12 @@ __device__ __forceinline__ void accumulate_match(double* acc, const KdIndex& ix,
 
 // The end of a residual phase, called by every thread of a THREADS-thread block whose first KD_WARPS warps hold
 // accumulators: the block partial row `block` of W accumulators, then (NACC-wide rows, fuse_threshold >= 0) the
-// fixed-order sum of the `grid` rows and the solve in the last block to arrive.
-template <int THREADS, int W = NACC>
+// fixed-order sum of the `grid` rows and the solve in the last block to arrive.  DEGEN: that solve is
+// icp_solve_and_update<true> with dg.
+template <int THREADS, int W = NACC, bool DEGEN = false>
 __device__ __forceinline__ void block_partial_and_finish(double* acc, FrameResult* fr, double* __restrict__ partials,
-                                                         float fuse_threshold, unsigned block, unsigned grid KD_SPLIT_ARG) {
+                                                         float fuse_threshold, unsigned block, unsigned grid KD_SPLIT_ARG,
+                                                         IcpDegen dg = IcpDegen{}) {
     KD_SPLIT_MAX(1, acc[0] + acc[29]);
     // The shuffle tree must start on a converged warp.  The grid's last block holds a warp whose lanes left the query
     // loop at different iterations; without this it took the divergent-warp path of the 30 x 5 shuffles, 35 us on H100
@@ -469,7 +471,8 @@ __device__ __forceinline__ void block_partial_and_finish(double* acc, FrameResul
     block_reduce_store<THREADS, KD_WARPS, W>(acc, partials + (size_t)block * W);
     KD_SPLIT_BLOCK_MAX()
     if constexpr (W == NACC)
-        if (fuse_threshold >= 0.f) icp_finish_in_last_block<THREADS>(fr, partials, (int)grid, fuse_threshold PLS_SPLIT_PASS);
+        if (fuse_threshold >= 0.f)
+            icp_finish_in_last_block<THREADS, DEGEN>(fr, partials, (int)grid, fuse_threshold PLS_SPLIT_PASS, dg);
 }
 
 // Iterations after a frame's first on maps of KD_COLD_MAP_POINTS or more: a thread per query keeps its previous match
@@ -689,6 +692,7 @@ kd_normals_wide_kernel(KdIndex ix, int k_normals, const int* __restrict__ workli
 // the block partial rows are PLS_EVAL_STATS wide.  The ICP instantiation (EVAL = false) is the same code as before.
 // GATE without EVAL (a gated registration): the same distance test on NACC-wide rows with the fused solve, so the
 // count accumulator (29) counts the inliers.
+// DEGEN (pls_register_scans_degeneracy): the fused solve is the eigenvalue-thresholded one of block_partial_and_finish.
 // kd_residual_body's pose.  Owned by this function rather than by the template, so that the module's shared variables
 // keep the order they had before kd_residual_body took EVAL: the ICP kernels keep their shared-memory layout and SASS
 // (profiles/sass_evaluate_poses_census.log).
@@ -697,12 +701,12 @@ __device__ __forceinline__ float* kd_residual_pose() {
     return sT;
 }
 
-template <bool EVAL = false, bool GATE = EVAL>
+template <bool EVAL = false, bool GATE = EVAL, bool DEGEN = false>
 __device__ __forceinline__ void kd_residual_body(const KdIndex& ix, const float4* __restrict__ queries,
                                                  const uint32_t* __restrict__ nq_dev, int64_t q_begin, int64_t q_stride,
                                                  FrameResult* fr, int scheme, float sigma, const int* __restrict__ match,
                                                  double* __restrict__ partials, float fuse_threshold, unsigned block,
-                                                 unsigned grid, double max_d2 KD_SPLIT_ARG) {
+                                                 unsigned grid, double max_d2 KD_SPLIT_ARG, IcpDegen dg = IcpDegen{}) {
     static_assert(PLS_EVAL_STATS == NACC + 2, "evaluation rows: the 30 accumulators, sum d^2, |P|");
     constexpr int W = EVAL ? PLS_EVAL_STATS : NACC;
     if (fr->done) return;
@@ -729,7 +733,7 @@ __device__ __forceinline__ void kd_residual_body(const KdIndex& ix, const float4
         }
         accumulate_match(acc, ix, p, pos, scheme, sigma KD_SPLIT_PASS);
     }
-    block_partial_and_finish<KD_THREADS, W>(acc, fr, partials, fuse_threshold, block, grid KD_SPLIT_PASS);
+    block_partial_and_finish<KD_THREADS, W, DEGEN>(acc, fr, partials, fuse_threshold, block, grid KD_SPLIT_PASS, dg);
 }
 
 __global__ void __launch_bounds__(KD_THREADS)
@@ -758,6 +762,7 @@ kd_residual_kernel(KdIndex ix, const float4* __restrict__ queries, const uint32_
 // and computes 4 normals in the median, 30 and 13 at most (profiles/h100_kd_residual_split_after.log): with 8 warps
 // the slowest block's searches took 35 us, a chain of up to four searches per warp.
 // GATE: match_proven<true>, warp_nearest<true> (an outlier computes no normal) and the residual's distance test.
+// DEGEN: the eigenvalue-thresholded solve (block_partial_and_finish).
 constexpr int KD_REFINE_THREADS = 512;
 constexpr int KD_REFINE_WARPS = KD_REFINE_THREADS / 32;
 // kd_icp_refine_body's shared state, owned by this function rather than by the template for the reason kd_residual_pose
@@ -776,14 +781,15 @@ __device__ __forceinline__ KdRefineShared kd_refine_shared() {
     return KdRefineShared{sT, s_hard, &s_nh, s_stage};
 }
 
-template <bool GATE = false>
+template <bool GATE = false, bool DEGEN = false>
 __device__ __forceinline__ void kd_icp_refine_body(const KdIndex& ix, const float4* __restrict__ queries,
                                                    const uint32_t* __restrict__ nq_dev, int64_t q_begin, int64_t q_stride,
                                                    FrameResult* fr, int scheme, float sigma, int k_normals,
                                                    int* __restrict__ match, float4* __restrict__ nn_state,
                                                    double* __restrict__ partials, float fuse_threshold,
                                                    unsigned long long* __restrict__ counters, unsigned block,
-                                                   unsigned grid KD_SPLIT_ARG, KdGate gate = KdGate{}) {
+                                                   unsigned grid KD_SPLIT_ARG, KdGate gate = KdGate{},
+                                                   IcpDegen dg = IcpDegen{}) {
     if (fr->done) return;
     const KdRefineShared sh = kd_refine_shared();
     float* sT = sh.sT;
@@ -858,7 +864,8 @@ __device__ __forceinline__ void kd_icp_refine_body(const KdIndex& ix, const floa
             if (!(match_d2_f64(p, __ldg(ix.sorted + pos)) <= gate.max_d2)) continue;
         accumulate_match(acc, ix, p, pos, scheme, sigma KD_SPLIT_PASS);
     }
-    block_partial_and_finish<KD_REFINE_THREADS>(acc, fr, partials, fuse_threshold, block, grid KD_SPLIT_PASS);
+    block_partial_and_finish<KD_REFINE_THREADS, NACC, DEGEN>(acc, fr, partials, fuse_threshold, block,
+                                                            grid KD_SPLIT_PASS, dg);
 }
 
 __global__ void __launch_bounds__(KD_REFINE_THREADS)
@@ -1043,6 +1050,35 @@ __global__ void __launch_bounds__(KD_REFINE_THREADS) kd_icp_refine_gated_batch_k
     KD_SPLIT_NONE()
     kd_icp_refine_body<true>(s.ix, s.queries, s.nq_dev, 0, 1, s.fr, s.scheme, s.sigma, s.k_normals, s.match, s.nn_state,
                              s.partials, s.fuse_threshold, s.counters, blockIdx.x, s.refine_blocks KD_SPLIT_PASS, gate);
+}
+
+// The twins of the gated residual and refine batch kernels with the eigenvalue-thresholded solve
+// (pls_register_scans_degeneracy; an ungated one runs them with an infinite gate, which matches as the ungated search
+// does).  min_eigenvalue and the output rows, registration blockIdx.y's at degen + ICP_DEGEN_STRIDE * blockIdx.y, are
+// launch arguments for the reason the gate is one.
+__global__ void __launch_bounds__(KD_THREADS) kd_residual_gated_degen_batch_kernel(const KdSeq* __restrict__ seqs, int it,
+                                                                                   double max_d2, double min_eigenvalue,
+                                                                                   double* __restrict__ degen) {
+    __shared__ KdSeq s;
+    load_seq(seqs, s);
+    if ((int)blockIdx.x >= s.blocks || !four_launch_step(s, it)) return;
+    KD_SPLIT_NONE()
+    const IcpDegen dg{min_eigenvalue, degen + (size_t)ICP_DEGEN_STRIDE * blockIdx.y, nullptr};
+    kd_residual_body<false, true, true>(s.ix, s.queries, s.nq_dev, 0, 1, s.fr, s.scheme, s.sigma, s.match, s.partials,
+                                        s.fuse_threshold, blockIdx.x, s.blocks, max_d2 KD_SPLIT_PASS, dg);
+}
+
+__global__ void __launch_bounds__(KD_REFINE_THREADS)
+kd_icp_refine_gated_degen_batch_kernel(const KdSeq* __restrict__ seqs, int it, KdGate gate, double min_eigenvalue,
+                                       double* __restrict__ degen) {
+    __shared__ KdSeq s;
+    load_seq(seqs, s);
+    if ((int)blockIdx.x >= s.refine_blocks || it >= s.max_iters) return;
+    KD_SPLIT_NONE()
+    const IcpDegen dg{min_eigenvalue, degen + (size_t)ICP_DEGEN_STRIDE * blockIdx.y, nullptr};
+    kd_icp_refine_body<true, true>(s.ix, s.queries, s.nq_dev, 0, 1, s.fr, s.scheme, s.sigma, s.k_normals, s.match,
+                                   s.nn_state, s.partials, s.fuse_threshold, s.counters, blockIdx.x,
+                                   s.refine_blocks KD_SPLIT_PASS, gate, dg);
 }
 
 // The done flags of every sequence, for the host's extra-round check.
@@ -1685,13 +1721,19 @@ static KdGate kd_gate_of(double max_distance) {
 }
 
 void kdmap_batch_iterations(pls_context* lead, int num, cudaStream_t st, const int* grid, int first, int last,
-                            double max_distance) {
+                            double max_distance, double min_eigenvalue, double* degen) {
     const KdSeq* seqs = lead->batch_buf.as<KdSeq>();
-    const KdGate g = kd_gate_of(isinf(max_distance) ? 0.0 : max_distance);
-    const KdGate* gate = isinf(max_distance) ? nullptr : &g;
+    // the thresholded solve runs in the gated kernels; at max_distance = +inf their gate (kd_gate_of: every bound +inf)
+    // keeps every match, and matches exactly as the ungated search
+    const bool thresholded = min_eigenvalue > 0.0;
+    const KdGate g = kd_gate_of(isinf(max_distance) && !thresholded ? 0.0 : max_distance);
+    const KdGate* gate = isinf(max_distance) && !thresholded ? nullptr : &g;
     for (int it = first; it < last; ++it) {
         if (it > 0 && grid[4]) {
-            if (gate) kd_icp_refine_gated_batch_kernel<<<dim3(grid[0], num), KD_REFINE_THREADS, 0, st>>>(seqs, it, *gate);
+            if (thresholded)
+                kd_icp_refine_gated_degen_batch_kernel<<<dim3(grid[0], num), KD_REFINE_THREADS, 0, st>>>(
+                    seqs, it, *gate, min_eigenvalue, degen);
+            else if (gate) kd_icp_refine_gated_batch_kernel<<<dim3(grid[0], num), KD_REFINE_THREADS, 0, st>>>(seqs, it, *gate);
             else kd_icp_refine_batch_kernel<<<dim3(grid[0], num), KD_REFINE_THREADS, 0, st>>>(seqs, it);
             PLS_CHECK_LAUNCH();
         }
@@ -1702,7 +1744,10 @@ void kdmap_batch_iterations(pls_context* lead, int num, cudaStream_t st, const i
             PLS_CHECK_LAUNCH();
         }
         batch_search(seqs, num, st, grid, it, gate);
-        if (gate) kd_residual_gated_batch_kernel<<<dim3(grid[0], num), KD_THREADS, 0, st>>>(seqs, it, gate->max_d2);
+        if (thresholded)
+            kd_residual_gated_degen_batch_kernel<<<dim3(grid[0], num), KD_THREADS, 0, st>>>(seqs, it, gate->max_d2,
+                                                                                          min_eigenvalue, degen);
+        else if (gate) kd_residual_gated_batch_kernel<<<dim3(grid[0], num), KD_THREADS, 0, st>>>(seqs, it, gate->max_d2);
         else kd_residual_batch_kernel<<<dim3(grid[0], num), KD_THREADS, 0, st>>>(seqs, it);
         PLS_CHECK_LAUNCH();
     }

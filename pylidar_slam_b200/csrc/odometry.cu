@@ -1007,15 +1007,27 @@ void odometry_reset(pls_context* ctx) {
 // registration's count accumulator of its last executed iteration, its inliers there.  A gated registration whose last
 // iteration had no inlier reports PLS_E_SINGULAR: its sums are all zero, which the solve's zero-residual test would
 // otherwise report as PLS_W_TINY_RESIDUAL, the flag of a near-perfect fit.
+// min_eigenvalue > 0 (kd map): the eigenvalue-thresholded solve of pls_register_scans_degeneracy; out_degenerate [B] and
+// out_eigenvalues [B,6] (nullable): each registration's degenerate count and eigenvalues of H / N in its last executed
+// iteration.
 static void register_batch(pls_context* ctx, const KdScan* scans, int64_t n, const float* T0_dev, int B, float* out_T,
                            float* out_params, float* out_losses, int* out_iters, int* out_status,
-                           double max_distance = HUGE_VAL, int* out_inliers = nullptr) {
+                           double max_distance = HUGE_VAL, int* out_inliers = nullptr, double min_eigenvalue = 0.0,
+                           int* out_degenerate = nullptr, double* out_eigenvalues = nullptr) {
     const bool kd = ctx->cfg.local_map_type == PLS_MAP_KDTREE;
     cudaStream_t st = ctx->stream;
     const int M = ctx->cfg.max_num_alignments;
     std::vector<FrameResult> h((size_t)PLS_MAX_SEQUENCES);
     std::vector<float> T((size_t)B * 16), params((size_t)B * 6), losses((size_t)B * M);
-    std::vector<int> iters((size_t)B), status((size_t)B), inliers((size_t)B);
+    std::vector<int> iters((size_t)B), status((size_t)B), inliers((size_t)B), degenerate((size_t)B);
+    std::vector<double> eigenvalues((size_t)B * 6), degen_rows;
+    const bool thresholded = min_eigenvalue > 0.0;
+    double* degen = nullptr;
+    if (thresholded) {
+        ctx->degen_buf.reserve((size_t)PLS_MAX_SEQUENCES * ICP_DEGEN_STRIDE * sizeof(double), st);
+        degen = ctx->degen_buf.as<double>();
+        degen_rows.resize((size_t)PLS_MAX_SEQUENCES * ICP_DEGEN_STRIDE);
+    }
     int first_error = PLS_OK, last = 0;
     for (int c0 = 0; c0 < B; c0 += PLS_MAX_SEQUENCES) {  // chunks of at most PLS_MAX_SEQUENCES registrations
         const int num = B - c0 < PLS_MAX_SEQUENCES ? B - c0 : PLS_MAX_SEQUENCES;
@@ -1030,12 +1042,17 @@ static void register_batch(pls_context* ctx, const KdScan* scans, int64_t n, con
         std::vector<pls_context*> same((size_t)num, ctx);
         if (kd)
             icp_rounds(same.data(), num,
-                       [&](int a, int b) { kdmap_batch_iterations(ctx, num, st, grid, a, b, max_distance); },
+                       [&](int a, int b) {
+                           kdmap_batch_iterations(ctx, num, st, grid, a, b, max_distance, min_eigenvalue, degen);
+                       },
                        [&](int* done) { kdmap_batch_done(ctx, num, st, done); });
         else
             icp_rounds(same.data(), num, [&](int a, int b) { projmap_hypotheses_iterations(ctx, n, num, st, a, b); },
                        [&](int* done) { projmap_batch_done(ctx, num, st, done); });
         PLS_CUDA(cudaMemcpyAsync(h.data(), frs, (size_t)num * sizeof(FrameResult), cudaMemcpyDeviceToHost, st));
+        if (thresholded)
+            PLS_CUDA(cudaMemcpyAsync(degen_rows.data(), degen, (size_t)num * ICP_DEGEN_STRIDE * sizeof(double),
+                                     cudaMemcpyDeviceToHost, st));
         PLS_CUDA(cudaStreamSynchronize(st));
         for (int j = 0; j < num; ++j) {
             const FrameResult& r = h[(size_t)j];
@@ -1047,6 +1064,11 @@ static void register_batch(pls_context* ctx, const KdScan* scans, int64_t n, con
             status[b] = r.status;
             inliers[b] = (int)r.last_sums[29];
             if (!isinf(max_distance) && inliers[b] == 0) status[b] = PLS_E_SINGULAR;
+            if (thresholded) {
+                const double* row = &degen_rows[(size_t)ICP_DEGEN_STRIDE * j];
+                memcpy(&eigenvalues[6 * b], row, 6 * sizeof(double));
+                degenerate[b] = (int)row[6];
+            }
             if (first_error == PLS_OK && (status[b] == PLS_E_SINGULAR || r.status == PLS_E_COMM)) first_error = status[b];
         }
         last = num - 1;
@@ -1061,6 +1083,8 @@ static void register_batch(pls_context* ctx, const KdScan* scans, int64_t n, con
     put_out(out_iters, iters.data(), iters.size() * sizeof(int));
     put_out(out_status, status.data(), status.size() * sizeof(int));
     put_out(out_inliers, inliers.data(), inliers.size() * sizeof(int));
+    put_out(out_degenerate, degenerate.data(), degenerate.size() * sizeof(int));
+    put_out(out_eigenvalues, eigenvalues.data(), eigenvalues.size() * sizeof(double));
     if (!out_status) raise_status(ctx, first_error);
 }
 
@@ -1194,10 +1218,13 @@ int pls_register_hypotheses(pls_context* ctx, const float* points, int64_t n, co
     PLS_API_END(ctx)
 }
 
-// pls_register_scans and pls_register_scans_gated (fn names the entry point in refusals).
+// pls_register_scans, pls_register_scans_gated and pls_register_scans_degeneracy (fn names the entry point in
+// refusals; min_eigenvalue 0: the solve of the first two).
 static void register_scans(pls_context* ctx, const char* fn, const float* const* scans, const int64_t* n, int S,
                            const int* scan_of, const float* T0s, int B, double max_distance, float* out_T,
-                           float* out_params, float* out_losses, int* out_iters, int* out_status, int* out_inliers) {
+                           float* out_params, float* out_losses, int* out_iters, int* out_status, int* out_inliers,
+                           double min_eigenvalue = 0.0, int* out_degenerate = nullptr,
+                           double* out_eigenvalues = nullptr) {
     const std::string f(fn);
     // every argument is checked before anything is enqueued: a refused call changes nothing
     PLS_REQUIRE(ctx->cfg.local_map_type == PLS_MAP_KDTREE, f + ": needs a kd-tree local map");
@@ -1215,7 +1242,7 @@ static void register_scans(pls_context* ctx, const char* fn, const float* const*
     const std::vector<KdScan> regs = stage_scans(ctx, scans, n, S, scan_of, B);
     const float* T0_dev = (const float*)to_device(ctx, T0s, (size_t)B * 16 * sizeof(float), ctx->stage_in[1]);
     register_batch(ctx, regs.data(), 0, T0_dev, B, out_T, out_params, out_losses, out_iters, out_status, max_distance,
-                   out_inliers);
+                   out_inliers, min_eigenvalue, out_degenerate, out_eigenvalues);
 }
 
 int pls_register_scans(pls_context* ctx, const float* const* scans, const int64_t* n, int S, const int* scan_of,
@@ -1233,6 +1260,19 @@ int pls_register_scans_gated(pls_context* ctx, const float* const* scans, const 
     PLS_API_BEGIN(ctx)
     register_scans(ctx, "pls_register_scans_gated", scans, n, S, scan_of, T0s, B, max_distance, out_T, out_params,
                    out_losses, out_iters, out_status, out_inliers);
+    PLS_API_END(ctx)
+}
+
+int pls_register_scans_degeneracy(pls_context* ctx, const float* const* scans, const int64_t* n, int S,
+                                  const int* scan_of, const float* T0s, int B, double max_distance,
+                                  double min_eigenvalue, float* out_T, float* out_params, float* out_losses,
+                                  int* out_iters, int* out_status, int* out_inliers, int* out_degenerate,
+                                  double* out_eigenvalues) {
+    PLS_API_BEGIN(ctx)
+    PLS_REQUIRE(min_eigenvalue > 0.0 && !isinf(min_eigenvalue),
+                "pls_register_scans_degeneracy: min_eigenvalue must be finite and > 0 (not NaN)");
+    register_scans(ctx, "pls_register_scans_degeneracy", scans, n, S, scan_of, T0s, B, max_distance, out_T, out_params,
+                   out_losses, out_iters, out_status, out_inliers, min_eigenvalue, out_degenerate, out_eigenvalues);
     PLS_API_END(ctx)
 }
 

@@ -149,6 +149,17 @@ def _gated(ctx, max_distance) -> bool:
     return True
 
 
+def _thresholded(ctx, min_eigenvalue) -> bool:
+    """Whether min_eigenvalue asks for the eigenvalue-thresholded solve; refuses a NaN, negative or infinite threshold,
+    and a positive one on a projective map, before any call."""
+    e = float(min_eigenvalue)
+    assert_debug(e >= 0.0 and np.isfinite(e), "min_eigenvalue must be finite and >= 0 (not NaN)")
+    if e == 0.0:
+        return False
+    assert_debug(ctx.cfg.local_map_type == _lib.MAP_KDTREE, "a min_eigenvalue > 0 needs a kd-tree local map")
+    return True
+
+
 # Pose count A*(2*half_x+1)*(2*half_y+1) from which _pose_search takes pls_kdmap_pose_search_pyramid (branch and
 # bound) instead of scoring every pose with pls_kdmap_pose_search.  Measured on an H100 SXM at 700 W, K = 8, 72 yaws
 # (profiles/h100_pose_search_pyramid.json, DESIGN section 18): up to 30 M poses the exhaustive call is faster in all
@@ -1085,7 +1096,8 @@ class ICPFrameToModel(OdometryAlgorithm):
                       _lib.ptr(losses), C.byref(iters))
         return params, T, list(losses[:iters.value])
 
-    def register_new_frame_hypotheses(self, target_points, initial_estimates, max_distance: float = np.inf):
+    def register_new_frame_hypotheses(self, target_points, initial_estimates, max_distance: float = np.inf,
+                                      min_eigenvalue: float = 0.0):
         """register_new_frame for B initial estimates [B,4,4] of one scan [n,3], in one call (pls_register_hypotheses;
         no reference counterpart): relocalisation in a prior map registers a scan from many guesses -- a yaw sweep, a
         grid of positions, place-recognition candidates -- and keeps the best converged result.  Registers against the
@@ -1099,13 +1111,18 @@ class ICPFrameToModel(OdometryAlgorithm):
         max_distance gates the correspondences as in register_new_frames (kd map only: a finite gate on a projective
         map raises before any call).  Gated, the hypotheses are what register_new_frames([target_points],
         initial_estimates, zeros, max_distance) returns, and last_hypotheses_inliers[b] holds each one's inlier count in
-        its last iteration (None when ungated).  The last_registrations_* attributes are left as they are."""
-        if _gated(self.ctx, max_distance):
-            params, T, losses, iters, self.last_hypotheses_status, self.last_hypotheses_inliers = \
+        its last iteration (None when ungated).  min_eigenvalue > 0 solves each iteration only in the directions the map
+        constrains, as in register_new_frames (kd map only), with last_hypotheses_degenerate and
+        last_hypotheses_eigenvalues (None when 0).  The last_registrations_* attributes are left as they are."""
+        gated, thresholded = _gated(self.ctx, max_distance), _thresholded(self.ctx, min_eigenvalue)
+        if gated or thresholded:
+            (params, T, losses, iters, self.last_hypotheses_status, self.last_hypotheses_inliers,
+             self.last_hypotheses_degenerate, self.last_hypotheses_eigenvalues) = \
                 self._register_scans([target_points], initial_estimates, np.zeros(len(initial_estimates), np.int32),
-                                     max_distance, "hypotheses")
+                                     max_distance, "hypotheses", min_eigenvalue)
             return params, T, losses, iters
         self.last_hypotheses_inliers = None
+        self.last_hypotheses_degenerate = self.last_hypotheses_eigenvalues = None
         _check_given_normals(self.ctx)
         check_tensor(target_points, [-1, 3])
         pts = _f32c(target_points)
@@ -1128,7 +1145,8 @@ class ICPFrameToModel(OdometryAlgorithm):
         return params, T, [list(losses[b, :iters[b]]) for b in range(B)], iters
 
     def localize(self, scan, prior_pose, radius: float, cell_size: float, yaw_range: float = np.pi,
-                 yaw_step: float = np.deg2rad(5), num_candidates: int = 8, max_distance: float = np.inf):
+                 yaw_step: float = np.deg2rad(5), num_candidates: int = 8, max_distance: float = np.inf,
+                 min_eigenvalue: float = 0.0):
         """Finds the pose of `scan` [n,3] on the kd map this odometry's context holds (e.g. loaded with
         KdTreeLocalMap(ctx=self.ctx).set_map_pointcloud) from a coarse prior: start-up on a stored map, recovery after
         odometry is lost.  No reference counterpart.
@@ -1136,7 +1154,8 @@ class ICPFrameToModel(OdometryAlgorithm):
         2. a correlative search of those bases moved by up to ceil(radius / cell_size) cells along x and y
            (KdTreeLocalMap.search_poses) keeps num_candidates local maxima;
         3. one register_new_frame_hypotheses call refines them from their float32-rounded poses, with the
-           correspondence gate max_distance (inf: none; the search and the rescoring are not gated);
+           correspondence gate max_distance (inf: none; the search and the rescoring are not gated) and the
+           eigenvalue threshold min_eigenvalue of its solve (0: none);
         4. score_poses rescores the refined poses.
         The search in step 2 is exact at any radius, and a large one is searched by branch and bound, so `radius` may
         span the whole map when the position is unknown.
@@ -1147,27 +1166,31 @@ class ICPFrameToModel(OdometryAlgorithm):
         assert_debug(np.isfinite(radius) and radius >= 0, "radius must be finite and >= 0")
         assert_debug(np.isfinite(cell_size) and cell_size > 0, "cell_size must be finite and > 0")
         _gated(self.ctx, max_distance)   # refused before the search
+        _thresholded(self.ctx, min_eigenvalue)
         bases = yaw_sweep(prior_pose, yaw_range, yaw_step)
         half = int(np.ceil(radius / cell_size))
         T0, coarse, _ = _pose_search(self.ctx, scan, bases, cell_size, half, half, num_candidates)
         if T0.shape[0] == 0:
             return []
-        _, T, _, iters = self.register_new_frame_hypotheses(scan, T0.astype(np.float32), max_distance)
+        _, T, _, iters = self.register_new_frame_hypotheses(scan, T0.astype(np.float32), max_distance, min_eigenvalue)
         status = self.last_hypotheses_status
         scores = _score_poses(self.ctx, scan, T.astype(np.float64), cell_size)
         return _pose_candidates(T0, coarse, T, iters, status, scores)
 
     def localize_scans(self, scans, prior_poses, radius, cell_size: float, yaw_range: float = np.pi,
-                       yaw_step: float = np.deg2rad(5), num_candidates: int = 8, max_distance: float = np.inf):
+                       yaw_step: float = np.deg2rad(5), num_candidates: int = 8, max_distance: float = np.inf,
+                       min_eigenvalue: float = 0.0):
         """localize for S scans on the one kd map this odometry's context holds (no reference counterpart): a
         localisation server re-localising many vehicles' scans, offline map matching a recorded drive's scans from
         GNSS fixes.  scans: S [n_s,3] arrays or tensors; prior_poses [S,4,4]; radius a scalar or [S].
         One batched search over every scan's yaw_sweep bases (KdTreeLocalMap.search_poses_scans), one
         register_new_frames call over every candidate, one batched rescoring of the refined poses.  Returns S lists of
         PoseCandidate; list s equals localize(scans[s], prior_poses[s], radius[s], cell_size, yaw_range, yaw_step,
-        num_candidates, max_distance), field for field; max_distance gates the refinement only."""
+        num_candidates, max_distance, min_eigenvalue), field for field; max_distance and min_eigenvalue apply to the
+        refinement only."""
         _check_given_normals(self.ctx)
         _gated(self.ctx, max_distance)   # refused before the search
+        _thresholded(self.ctx, min_eigenvalue)
         S = len(scans)
         if isinstance(prior_poses, torch.Tensor):
             prior_poses = prior_poses.detach().cpu().numpy()
@@ -1183,7 +1206,8 @@ class ICPFrameToModel(OdometryAlgorithm):
             return [[] for _ in range(S)]
         T0_all = np.concatenate([T0 for T0, _, _ in found])
         _, T, _, iters = self.register_new_frames(scans, T0_all.astype(np.float32),
-                                                  np.repeat(np.arange(S, dtype=np.int32), counts), max_distance)
+                                                  np.repeat(np.arange(S, dtype=np.int32), counts), max_distance,
+                                                  min_eigenvalue)
         status = self.last_registrations_status
         hit = [s for s in range(S) if counts[s]]
         first = np.concatenate([[0], np.cumsum(counts)])
@@ -1198,7 +1222,8 @@ class ICPFrameToModel(OdometryAlgorithm):
                        else [])
         return out
 
-    def register_new_frames(self, scans, initial_estimates, scan_indices=None, max_distance: float = np.inf):
+    def register_new_frames(self, scans, initial_estimates, scan_indices=None, max_distance: float = np.inf,
+                            min_eigenvalue: float = 0.0):
         """register_new_frame for many scans against the one map this odometry's context holds, in one call
         (pls_register_scans; no reference counterpart): a localisation server registers many vehicles' scans on one
         city map, offline map matching registers a recorded drive's scans on a prior map.  `scans` is a list of S
@@ -1215,23 +1240,40 @@ class ICPFrameToModel(OdometryAlgorithm):
         construction, partial overlap -- cannot pull the pose towards far matches.  A registration left with too few
         inliers, or none, ends singular (PLS_E_SINGULAR) without stopping the others.  last_registrations_inliers[b]
         then holds registration b's inlier count in its last iteration (None when ungated).  max_distance = inf, the
-        default, makes the ungated call, bit for bit as before; NaN or a negative gate raises before any call."""
-        params, T, losses, iters, self.last_registrations_status, self.last_registrations_inliers = \
-            self._register_scans(scans, initial_estimates, scan_indices, max_distance, "registrations")
+        default, makes the ungated call, bit for bit as before; NaN or a negative gate raises before any call.
+        min_eigenvalue > 0 solves every ICP iteration only in the directions the map constrains
+        (pls_register_scans_degeneracy): a tunnel, a corridor or a flat field leaves some directions unconstrained, and
+        there the pose keeps its initial estimate instead of sliding on noise or ending singular.  With H the
+        iteration's 6x6 normal-equation matrix and N its inlier (or match) count, an eigen-direction of H is kept when
+        its eigenvalue is at least min_eigenvalue * N.  The threshold mixes units: per point, translation eigenvalues
+        are dimensionless (at most 1 unweighted) and rotation eigenvalues are in m^2; calibrate it from
+        evaluate_registrations' eigenvalues / inliers on your own map.  last_registrations_degenerate [B] then holds
+        each registration's number of degenerate directions and last_registrations_eigenvalues [B,6] the ascending
+        eigenvalues of H / N, both of its last iteration (None when min_eigenvalue is 0).  0, the default, makes the
+        call made without it; NaN, a negative or an infinite threshold raises before any call."""
+        (params, T, losses, iters, self.last_registrations_status, self.last_registrations_inliers,
+         self.last_registrations_degenerate, self.last_registrations_eigenvalues) = \
+            self._register_scans(scans, initial_estimates, scan_indices, max_distance, "registrations", min_eigenvalue)
         return params, T, losses, iters
 
-    def _register_scans(self, scans, initial_estimates, scan_indices, max_distance, what):
-        """register_new_frames' call: (params, T, losses, iterations, status, inliers or None), singular ones logged
-        as `what`."""
-        gated = _gated(self.ctx, max_distance)
+    def _register_scans(self, scans, initial_estimates, scan_indices, max_distance, what, min_eigenvalue=0.0):
+        """register_new_frames' call: (params, T, losses, iterations, status, inliers or None, degenerate counts or
+        None, eigenvalues or None), singular ones logged as `what`."""
+        gated, thresholded = _gated(self.ctx, max_distance), _thresholded(self.ctx, min_eigenvalue)
         pts, addresses, rows, T0, index = self._scans_args(scans, initial_estimates, scan_indices)
         B, S, M = T0.shape[0], len(pts), int(self.config.max_num_alignments)
         T, params = np.zeros((B, 4, 4), np.float32), np.zeros((B, 6), np.float32)
         losses = np.zeros((B, M), np.float32)
         iters, status = np.zeros(B, np.int32), np.zeros(B, np.int32)
-        inliers = None
-        if gated:
-            inliers = np.zeros(B, np.int32)
+        inliers = np.zeros(B, np.int32) if gated else None
+        degenerate = eigenvalues = None
+        if thresholded:
+            degenerate, eigenvalues = np.zeros(B, np.int32), np.zeros((B, 6), np.float64)
+            self.ctx.call("pls_register_scans_degeneracy", _lib.ptr(addresses), _lib.ptr(rows), S, _lib.ptr(index),
+                          _lib.ptr(T0), B, float(max_distance), float(min_eigenvalue), _lib.ptr(T), _lib.ptr(params),
+                          _lib.ptr(losses), _lib.ptr(iters), _lib.ptr(status), _lib.ptr(inliers),
+                          _lib.ptr(degenerate), _lib.ptr(eigenvalues))
+        elif gated:
             self.ctx.call("pls_register_scans_gated", _lib.ptr(addresses), _lib.ptr(rows), S, _lib.ptr(index),
                           _lib.ptr(T0), B, float(max_distance), _lib.ptr(T), _lib.ptr(params), _lib.ptr(losses),
                           _lib.ptr(iters), _lib.ptr(status), _lib.ptr(inliers))
@@ -1243,7 +1285,7 @@ class ICPFrameToModel(OdometryAlgorithm):
             import logging
             logging.error(f"Invalid Jacobian in Gauss Newton minimization, the hessian is not invertible "
                           f"({what} {singular.tolist()})")
-        return params, T, [list(losses[b, :iters[b]]) for b in range(B)], iters, status, inliers
+        return params, T, [list(losses[b, :iters[b]]) for b in range(B)], iters, status, inliers, degenerate, eigenvalues
 
     def _scans_args(self, scans, poses, scan_indices):
         """register_new_frames' and evaluate_registrations' inputs as pls_register_scans / pls_kdmap_evaluate_poses
