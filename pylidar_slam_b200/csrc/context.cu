@@ -335,7 +335,7 @@ int pls_destroy(pls_context* ctx) {
     for (auto& b : ctx->frame_pts_buf) b.release();
     ctx->queries.release(); ctx->nn_prev.release();
     ctx->partials.release(); ctx->batch_buf.release(); ctx->hyp_buf.release(); ctx->degen_buf.release(); ctx->gs_keys.release(); ctx->gs_vals.release(); ctx->gs_out_xyz.release();
-    ctx->gs_out_idx.release();
+    ctx->gs_out_idx.release(); ctx->gs_bins.release(); ctx->gs_buckets.release();
     for (auto& s : ctx->prof)
         for (auto e : s.pool) cudaEventDestroy(e);
     if (ctx->ev_map_done) cudaEventDestroy(ctx->ev_map_done);

@@ -1,5 +1,13 @@
 // K1 -- voxel-grid subsample.
 //
+// Compact keys, n <= SEL_MAX_N (every frame of the kd path): three launches, no memset.
+//   gs_hash_bins_kernel      : the hash below, composite key key40 << 24 | index, counts of 2^16 bins (top 16 key
+//                              bits); the last block turns the occupied bins into offsets and cuts buckets of whole bins
+//   gs_bucket_scatter_kernel : every key to its bin's cursor -- each bucket lands in its own slice
+//   gs_bucket_select_kernel  : a block per bucket sorts it by composite key (the smallest index of a run sorts first),
+//                              keeps the run heads and chains the buckets' counts to place them
+// Larger clouds and the 64-bit replay after an overflow take the path below:
+//
 //   voxel_hash_kernel : voxel coordinate = int64(round_half_even(double(p) / voxel)) per axis
 //                       and hash = 73856093 x + 19349669 y + 83492791 z in signed 64-bit
 //                       (slam/common/pointcloud.py:13-23,40-79).  Also emits the sort key
@@ -120,6 +128,343 @@ struct GridSampleSelect {
     }
 };
 
+// ---- bucket grid sample (compact keys, n <= SEL_MAX_N) -------------------------------------------------------
+// Composite key = key40 << 24 | point index: sorted, the head of every run of equal key40 is its smallest index, so no
+// stable sort is needed.  Bins are the top 16 bits of key40 (2^24 hash units each): LiDAR hashes crowd around 0, and
+// fine bins keep the buckets cut from them balanced.
+constexpr int GS_BIN_BITS = 16;
+constexpr int GS_BINS = 1 << GS_BIN_BITS;
+constexpr int GS_IDX_BITS = 24;
+constexpr uint64_t GS_IDX_MASK = (1ull << GS_IDX_BITS) - 1ull;
+constexpr uint32_t GS_BUCKET_TARGET = 1024;  // bucket b: the bins whose first key ranks in [b, b + 1) * GS_BUCKET_TARGET
+constexpr uint32_t GS_BUCKET_CAP = 4096;     // the largest bucket sorted in shared memory (32 KB of keys)
+constexpr int GS_SELECT_THREADS = 512;
+constexpr int GS_SCAN_ITEMS = 8;             // bins per thread and tile in the hash kernel's offset scan
+constexpr uint32_t GS_FLAG_AGG = 1u << 30, GS_FLAG_PREFIX = 2u << 30, GS_VALUE_MASK = (1u << 30) - 1u;
+// control words behind the bins: the hash kernel's last-block ticket, the occupied bin range while it is being taken
+// (65535 - lowest bin, highest bin: both start at 0), that range for the select kernel, the select kernel's bucket ticket
+enum { GSW_TICKET = 0, GSW_LO_INV, GSW_HI, GSW_RANGE_LO, GSW_RANGE_HI, GSW_BUCKET_TICKET, GSW_WORDS = 8 };
+
+__device__ __forceinline__ uint32_t gs_ld_volatile(const uint32_t* p) {
+    uint32_t v;
+    asm volatile("ld.volatile.global.u32 %0, [%1];" : "=r"(v) : "l"(p));
+    return v;
+}
+__device__ __forceinline__ void gs_st_volatile(uint32_t* p, uint32_t v) {
+    asm volatile("st.volatile.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
+
+// Exclusive scan of one value per thread over the block; `total` gets the sum.  Every thread of the block calls it.
+__device__ __forceinline__ uint32_t gs_block_scan(uint32_t v, uint32_t* s_warp, uint32_t& total) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, warps = blockDim.x >> 5;
+    uint32_t inc = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const uint32_t t = __shfl_up_sync(0xffffffffu, inc, o);
+        if (lane >= o) inc += t;
+    }
+    if (lane == 31) s_warp[warp] = inc;
+    __syncthreads();
+    uint32_t before = 0, tot = 0;
+    for (int w = 0; w < warps; ++w) {
+        const uint32_t c = s_warp[w];
+        before += w < warp ? c : 0u;
+        tot += c;
+    }
+    __syncthreads();  // s_warp is free for the next scan
+    total = tot;
+    return before + inc - v;
+}
+
+// K1: the voxel hash of voxel_hash_kernel, the composite key with the overflow stamp, and the bin counts.  The block
+// that finishes last turns the counts of the occupied bin range into exclusive offsets in place (the scatter's
+// cursors) and cuts the buckets; it also resets the control words for the next call.
+template <typename T>
+__global__ void __launch_bounds__(256)
+gs_hash_bins_kernel(const T* __restrict__ xyz, int64_t n, double voxel, uint64_t* __restrict__ keys, uint32_t* bins,
+                    uint32_t* words, uint32_t* __restrict__ bucket_start, uint32_t* __restrict__ status, int num_buckets,
+                    uint32_t* __restrict__ overflow, uint32_t stamp) {
+    __shared__ uint32_t s_lo_inv, s_hi, s_warp[8];
+    __shared__ int s_last;
+    const int tid = threadIdx.x, lane = tid & 31;
+    if (tid == 0) s_lo_inv = s_hi = 0u;
+    __syncthreads();
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    // the select kernel's look-back words (the last call's select kernel has completed)
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + tid; i <= num_buckets; i += stride) status[i] = 0u;
+    // warp-uniform trip count: the match below needs every lane
+    for (int64_t base = (int64_t)blockIdx.x * blockDim.x + (tid & ~31); base < n; base += stride) {
+        const int64_t i = base + lane;
+        const bool valid = i < n;
+        uint32_t bin = 0xffffffffu;
+        if (valid) {
+            const long long cx = voxel_coord((double)xyz[3 * i], voxel);
+            const long long cy = voxel_coord((double)xyz[3 * i + 1], voxel);
+            const long long cz = voxel_coord((double)xyz[3 * i + 2], voxel);
+            const uint64_t h = (uint64_t)HX * (uint64_t)cx + (uint64_t)HY * (uint64_t)cy + (uint64_t)HZ * (uint64_t)cz;
+            const uint64_t hb = h + (1ull << (GS_COMPACT_BITS - 1));
+            if (hb >> GS_COMPACT_BITS) *overflow = stamp;
+            const uint64_t k40 = hb & ((1ull << GS_COMPACT_BITS) - 1ull);
+            keys[i] = (k40 << GS_IDX_BITS) | (uint64_t)i;
+            bin = (uint32_t)(k40 >> (GS_COMPACT_BITS - GS_BIN_BITS));
+        }
+        // consecutive points of a scan often share a voxel: one atomic per bin and warp
+        const uint32_t peers = __match_any_sync(0xffffffffu, bin);
+        if (valid && lane == __ffs(peers) - 1) atomicAdd(&bins[bin], (uint32_t)__popc(peers));
+        const uint32_t lo_inv = __reduce_max_sync(0xffffffffu, valid ? (uint32_t)(GS_BINS - 1) - bin : 0u);
+        const uint32_t hi = __reduce_max_sync(0xffffffffu, valid ? bin : 0u);
+        if (lane == 0) {
+            atomicMax(&s_lo_inv, lo_inv);
+            atomicMax(&s_hi, hi);
+        }
+    }
+    __syncthreads();
+    if (tid == 0) {
+        atomicMax(&words[GSW_LO_INV], s_lo_inv);
+        atomicMax(&words[GSW_HI], s_hi);
+    }
+    __threadfence();
+    __syncthreads();
+    if (tid == 0) s_last = atomicAdd(&words[GSW_TICKET], 1u) == gridDim.x - 1;
+    __syncthreads();
+    if (!s_last) return;
+    __threadfence();
+    const uint32_t lo = (uint32_t)(GS_BINS - 1) - __ldcg(&words[GSW_LO_INV]), hi = __ldcg(&words[GSW_HI]);
+    // tiles of GS_SCAN_ITEMS bins per thread, loaded together: one L2 round trip per tile, not one per bin
+    uint32_t carry = 0;
+    for (uint32_t t0 = lo; t0 <= hi; t0 += blockDim.x * GS_SCAN_ITEMS) {
+        const uint32_t b0 = t0 + tid * GS_SCAN_ITEMS;
+        uint32_t c[GS_SCAN_ITEMS], sum = 0;
+#pragma unroll
+        for (int j = 0; j < GS_SCAN_ITEMS; ++j) {
+            c[j] = b0 + j <= hi ? __ldcg(&bins[b0 + j]) : 0u;
+            sum += c[j];
+        }
+        uint32_t total;
+        uint32_t p = carry + gs_block_scan(sum, s_warp, total);
+        carry += total;
+#pragma unroll
+        for (int j = 0; j < GS_SCAN_ITEMS; ++j) {
+            if (b0 + j > hi) break;
+            bins[b0 + j] = p;
+            // bucket k starts at the first bin offset >= k * target: the buckets whose k * target lies in (p, p + c]
+            for (uint32_t k = p / GS_BUCKET_TARGET + 1; k * GS_BUCKET_TARGET <= p + c[j] && k < (uint32_t)num_buckets; ++k)
+                bucket_start[k] = p + c[j];
+            p += c[j];
+        }
+    }
+    if (tid == 0) {
+        bucket_start[0] = 0u;
+        bucket_start[num_buckets] = (uint32_t)n;
+        words[GSW_TICKET] = 0u;
+        words[GSW_LO_INV] = 0u;
+        words[GSW_HI] = 0u;
+        words[GSW_RANGE_LO] = lo;
+        words[GSW_RANGE_HI] = hi;
+        words[GSW_BUCKET_TICKET] = 0u;
+    }
+}
+
+// K2: every composite key to its bin's cursor.  The bins are contiguous key ranges in key order, so every bucket ends
+// up in its own slice of `sorted`; the order inside a bin does not matter.
+__global__ void __launch_bounds__(256)
+gs_bucket_scatter_kernel(const uint64_t* __restrict__ keys, int64_t n, uint32_t* bins, uint64_t* __restrict__ sorted) {
+    pls_grid_dependency_wait();
+    const int lane = threadIdx.x & 31;
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t base = (int64_t)blockIdx.x * blockDim.x + (threadIdx.x & ~31); base < n; base += stride) {
+        const int64_t i = base + lane;
+        const bool valid = i < n;
+        const uint64_t k = valid ? keys[i] : 0ull;
+        const uint32_t bin = valid ? (uint32_t)(k >> (GS_IDX_BITS + GS_COMPACT_BITS - GS_BIN_BITS)) : 0xffffffffu;
+        const uint32_t peers = __match_any_sync(0xffffffffu, bin);
+        const int leader = __ffs(peers) - 1;
+        uint32_t pos = 0;
+        if (valid && lane == leader) pos = atomicAdd(&bins[bin], (uint32_t)__popc(peers));
+        pos = __shfl_sync(0xffffffffu, pos, leader) + __popc(peers & ((1u << lane) - 1u));
+        if (valid) sorted[pos] = k;
+    }
+}
+
+// The output offset of bucket b (run by one warp): decoupled look-back over the buckets before it, 32 per round trip.
+__device__ uint32_t gs_bucket_prefix(uint32_t* status, uint32_t b, uint32_t agg) {
+    const int lane = threadIdx.x & 31;
+    if (b == 0) {
+        if (lane == 0) gs_st_volatile(status, GS_FLAG_PREFIX | agg);
+        return 0u;
+    }
+    if (lane == 0) gs_st_volatile(status + b, GS_FLAG_AGG | agg);
+    uint32_t excl = 0;
+    for (int64_t t = (int64_t)b - 1;; t -= 32) {
+        const int64_t j = t - lane;
+        uint32_t v = j >= 0 ? gs_ld_volatile(status + j) : GS_FLAG_PREFIX;  // before bucket 0: a prefix of 0
+        while (__any_sync(0xffffffffu, (v >> 30) == 0u))
+            if ((v >> 30) == 0u) v = gs_ld_volatile(status + j);
+        const int first = __ffs(__ballot_sync(0xffffffffu, (v & GS_FLAG_PREFIX) != 0u)) - 1;
+        excl += __reduce_add_sync(0xffffffffu, (first < 0 || lane <= first) ? (v & GS_VALUE_MASK) : 0u);
+        if (first >= 0) break;
+    }
+    if (lane == 0) gs_st_volatile(status + b, GS_FLAG_PREFIX | (excl + agg));
+    return excl;
+}
+
+template <typename T>
+__device__ __forceinline__ void gs_emit(const T* __restrict__ xyz, T* __restrict__ out_xyz, long long* __restrict__ out_idx,
+                                        uint64_t key, uint32_t dst) {
+    const uint32_t src = (uint32_t)(key & GS_IDX_MASK);
+    const T x = xyz[3 * (size_t)src], y = xyz[3 * (size_t)src + 1], z = xyz[3 * (size_t)src + 2];
+    if (out_idx) out_idx[dst] = (long long)src;
+    out_xyz[3 * (size_t)dst] = x;
+    out_xyz[3 * (size_t)dst + 1] = y;
+    out_xyz[3 * (size_t)dst + 2] = z;
+}
+
+__device__ __forceinline__ bool gs_is_head(const uint64_t* k, uint32_t i) {
+    // buckets hold whole bins, so the first key of a bucket always starts a run
+    return i == 0 || (k[i] >> GS_IDX_BITS) != (k[i - 1] >> GS_IDX_BITS);
+}
+
+// K3: one block per bucket (in ticket order, for the look-back): sort the bucket by composite key, keep the run heads,
+// write them at the bucket's output offset.  The last bucket writes the sample count.  The block also clears the bins
+// the scatter used, for the next call.
+template <typename T>
+__global__ void __launch_bounds__(GS_SELECT_THREADS)
+gs_bucket_select_kernel(uint64_t* sorted, uint64_t* scratch, const uint32_t* __restrict__ bucket_start, uint32_t* status,
+                        uint32_t* words, uint32_t* bins, int num_buckets, const T* __restrict__ xyz, T* __restrict__ out_xyz,
+                        long long* __restrict__ out_idx, uint32_t* __restrict__ count_out) {
+    __shared__ uint64_t s_keys[GS_BUCKET_CAP];
+    __shared__ uint32_t s_warp[GS_SELECT_THREADS / 32];
+    __shared__ uint32_t s_bucket, s_excl;
+    const int tid = threadIdx.x;
+    pls_grid_dependency_wait();
+    if (tid == 0) s_bucket = atomicAdd(&words[GSW_BUCKET_TICKET], 1u);
+    {
+        const uint32_t lo = words[GSW_RANGE_LO], hi = words[GSW_RANGE_HI];
+        for (uint32_t b = lo + blockIdx.x * blockDim.x + tid; b <= hi; b += gridDim.x * blockDim.x) bins[b] = 0u;
+    }
+    __syncthreads();
+    const uint32_t b = s_bucket;
+    const uint32_t s = bucket_start[b], m = bucket_start[b + 1] - s;
+    uint32_t total;
+    if (m <= GS_BUCKET_CAP) {
+        // bitonic sort in shared memory, padded to a power of two with keys above every composite key
+        uint32_t P = 1;
+        while (P < m) P <<= 1;
+        for (uint32_t i = tid; i < P; i += blockDim.x) s_keys[i] = i < m ? sorted[s + i] : ~0ull;
+        __syncthreads();
+        for (uint32_t k = 2; k <= P; k <<= 1)
+            for (uint32_t j = k >> 1; j > 0; j >>= 1) {
+                for (uint32_t i = tid; i < P / 2; i += blockDim.x) {
+                    const uint32_t lo = ((i & ~(j - 1)) << 1) | (i & (j - 1)), hi = lo | j;
+                    const uint64_t a = s_keys[lo], c = s_keys[hi];
+                    if ((a > c) == ((lo & k) == 0)) {
+                        s_keys[lo] = c;
+                        s_keys[hi] = a;
+                    }
+                }
+                __syncthreads();
+            }
+        // contiguous items per thread: heads, their block offsets, the bucket's offset, the samples
+        const uint32_t per = (m + blockDim.x - 1) / blockDim.x;
+        const uint32_t i0 = min(tid * per, m), i1 = min(i0 + per, m);
+        uint32_t heads = 0;
+        for (uint32_t i = i0; i < i1; ++i) heads += gs_is_head(s_keys, i);
+        uint32_t dst = gs_block_scan(heads, s_warp, total);
+        if (tid < 32) {
+            const uint32_t e = gs_bucket_prefix(status, b, total);
+            if (tid == 0) s_excl = e;
+        }
+        __syncthreads();
+        dst += s_excl;
+        for (uint32_t i = i0; i < i1; ++i)
+            if (gs_is_head(s_keys, i)) gs_emit(xyz, out_xyz, out_idx, s_keys[i], dst++);
+    } else {
+        // A bucket beyond shared memory (more than GS_BUCKET_CAP - GS_BUCKET_TARGET points in one bin, e.g. many points
+        // in one voxel): a stable LSD radix sort through global memory by this block alone, on the bits in which the
+        // bucket's keys differ, one chunk of blockDim.x keys after the other.
+        uint64_t* a = sorted + s;
+        uint64_t* alt = scratch + s;
+        uint32_t* hist = reinterpret_cast<uint32_t*>(s_keys);  // [256] digit offsets
+        uint32_t* warp_cnt = hist + 256;                       // [warps][256] digit counts of a chunk
+        uint64_t kmin = ~0ull, kmax = 0ull;
+        for (uint32_t i = tid; i < m; i += blockDim.x) {
+            const uint64_t k = a[i];
+            kmin = min(kmin, k);
+            kmax = max(kmax, k);
+        }
+        __shared__ unsigned long long s_min, s_max;
+        if (tid == 0) {
+            s_min = ~0ull;
+            s_max = 0ull;
+        }
+        __syncthreads();
+        atomicMin(&s_min, (unsigned long long)kmin);
+        atomicMax(&s_max, (unsigned long long)kmax);
+        __syncthreads();
+        kmin = s_min;
+        const int bits = 64 - __clzll((long long)(s_max - kmin));
+        const int lane = tid & 31, warp = tid >> 5, warps = blockDim.x >> 5;
+        for (int shift = 0; shift < bits; shift += 8) {
+            for (int d = tid; d < 256; d += blockDim.x) hist[d] = 0u;
+            __syncthreads();
+            for (uint32_t i = tid; i < m; i += blockDim.x) atomicAdd(&hist[(uint32_t)((a[i] - kmin) >> shift) & 255u], 1u);
+            __syncthreads();
+            {
+                const uint32_t c = tid < 256 ? hist[tid] : 0u;
+                const uint32_t e = gs_block_scan(c, s_warp, total);
+                if (tid < 256) hist[tid] = e;
+                __syncthreads();
+            }
+            for (uint32_t c0 = 0; c0 < m; c0 += blockDim.x) {
+                for (int w = tid; w < warps * 256; w += blockDim.x) warp_cnt[w] = 0u;
+                __syncthreads();
+                const uint32_t i = c0 + tid;
+                const bool valid = i < m;
+                const uint64_t k = valid ? a[i] : 0ull;
+                const uint32_t d = valid ? ((uint32_t)((k - kmin) >> shift) & 255u) : 256u;
+                const uint32_t peers = __match_any_sync(0xffffffffu, d);
+                const uint32_t rank = __popc(peers & ((1u << lane) - 1u));
+                if (valid && lane == __ffs(peers) - 1) warp_cnt[warp * 256 + d] = __popc(peers);
+                __syncthreads();
+                if (tid < 256) {
+                    uint32_t run = hist[tid];
+                    for (int w = 0; w < warps; ++w) {
+                        const uint32_t c = warp_cnt[w * 256 + tid];
+                        warp_cnt[w * 256 + tid] = run;
+                        run += c;
+                    }
+                    hist[tid] = run;
+                }
+                __syncthreads();
+                if (valid) alt[warp_cnt[warp * 256 + d] + rank] = k;
+                __syncthreads();
+            }
+            uint64_t* t = a;
+            a = alt;
+            alt = t;
+        }
+        uint32_t heads = 0;
+        for (uint32_t i = tid; i < m; i += blockDim.x) heads += gs_is_head(a, i);
+        gs_block_scan(heads, s_warp, total);
+        if (tid < 32) {
+            const uint32_t e = gs_bucket_prefix(status, b, total);
+            if (tid == 0) s_excl = e;
+        }
+        __syncthreads();
+        uint32_t carry = s_excl;
+        for (uint32_t c0 = 0; c0 < m; c0 += blockDim.x) {
+            const uint32_t i = c0 + tid;
+            const bool head = i < m && gs_is_head(a, i);
+            uint32_t chunk;
+            const uint32_t dst = carry + gs_block_scan(head ? 1u : 0u, s_warp, chunk);
+            if (head) gs_emit(xyz, out_xyz, out_idx, a[i], dst);
+            carry += chunk;
+        }
+        total = carry - s_excl;
+    }
+    if (b == (uint32_t)num_buckets - 1 && tid == 0) *count_out = s_excl + total;
+}
+
 // ---- voxel statistics (Voxelization filter) ---------------------------------------------------------------
 // After the same hash + stable sort as the subsample: rank of every run of equal hashes = voxel id
 // (pointcloud.py:99-150 walks the sorted hashes the same way), scattered back to the points' original order.
@@ -183,6 +528,32 @@ inline int grid_for(int64_t n, int threads = 256) {
     return (int)(b < 1 ? 1 : (b > cap ? cap : b));
 }
 
+// The three launches of the bucket path; the count lands in SC_GS_COUNT, an overflow stamp in SC_GS_OVERFLOW.
+template <typename T>
+void grid_sample_buckets(pls_context* ctx, const T* xyz_dev, int64_t n, double voxel, T* out_xyz_dev, long long* out_idx_dev) {
+    cudaStream_t st = ctx->stream;
+    const int num_buckets = (int)((n + GS_BUCKET_TARGET - 1) / GS_BUCKET_TARGET);
+    if (!ctx->gs_bins.p) {  // the bins and control words start at zero; every call leaves them so
+        ctx->gs_bins.reserve_exact((GS_BINS + GSW_WORDS) * sizeof(uint32_t), st);
+        PLS_CUDA(cudaMemsetAsync(ctx->gs_bins.p, 0, (GS_BINS + GSW_WORDS) * sizeof(uint32_t), st));
+    }
+    ctx->gs_buckets.reserve(2 * ((size_t)num_buckets + 1) * sizeof(uint32_t), st);
+    ctx->sort.keys_alt.reserve((size_t)n * sizeof(uint64_t), st);
+    uint32_t* bins = ctx->gs_bins.as<uint32_t>();
+    uint32_t* words = bins + GS_BINS;
+    uint32_t* bucket_start = ctx->gs_buckets.as<uint32_t>();
+    uint32_t* status = bucket_start + num_buckets + 1;
+    uint64_t* keys = ctx->gs_keys.as<uint64_t>();
+    uint64_t* sorted = ctx->sort.keys_alt.as<uint64_t>();
+    gs_hash_bins_kernel<T><<<grid_for(n), 256, 0, st>>>(xyz_dev, n, voxel, keys, bins, words, bucket_start, status,
+                                                        num_buckets, scalar_u32(ctx, SC_GS_OVERFLOW), ctx->gs_seq);
+    PLS_CHECK_LAUNCH();
+    launch_dependent(gs_bucket_scatter_kernel, grid_for(n), 256, st, (const uint64_t*)keys, n, bins, sorted);
+    launch_dependent(gs_bucket_select_kernel<T>, num_buckets, GS_SELECT_THREADS, st, sorted, keys,
+                     (const uint32_t*)bucket_start, status, words, bins, num_buckets, xyz_dev, out_xyz_dev, out_idx_dev,
+                     scalar_u32(ctx, SC_GS_COUNT));
+}
+
 }  // namespace
 
 // Device-resident grid sample: xyz_dev [n,3] -> out_xyz_dev [<=n,3], out_idx_dev [<=n] (nullable);
@@ -213,6 +584,11 @@ void grid_sample_device(pls_context* ctx, const T* xyz_dev, int64_t n, double vo
     if (compact) {
         ctx->gs_seq += 1;
         if (ctx->gs_seq == 0) ctx->gs_seq = 1;
+    }
+    if (compact && n <= SEL_MAX_N) {
+        grid_sample_buckets(ctx, xyz_dev, n, voxel, out_xyz_dev, out_idx_dev);
+        copy_to_host();
+        return;
     }
     voxel_hash_kernel<T><<<grid_for(n), 256, 0, st>>>(xyz_dev, n, voxel, nullptr, nullptr, ctx->gs_keys.as<uint64_t>(),
                                                       ctx->gs_vals.as<uint32_t>(),

@@ -264,6 +264,8 @@ struct pls_context {
     cudaEvent_t ev_batch = nullptr;     // pls_process_frames: this context's input stage, before the batched ICP
     cudaEvent_t ev_icp_done = nullptr;  // a frame's ICP launches and its map-update decision, before the map stream's update
     pls::DBuf gs_keys, gs_vals, gs_out_xyz, gs_out_idx;
+    pls::DBuf gs_bins;                  // bucket grid sample: 2^16 bin counts + control words, zero between calls
+    pls::DBuf gs_buckets;               // bucket grid sample: bucket starts + look-back words
     uint32_t gs_seq = 0;                // stamp of the last compact-key grid sample (overflow detection)
     pls::HBuf gs_host_xyz, gs_host_idx; // pinned + mapped staging the grid sample's gather writes directly (host callers)
     int64_t last_query_count = 0;

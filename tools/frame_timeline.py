@@ -11,6 +11,8 @@ stderr every 64 frames).
 
 Per frame, the median over the timed frames of:
   grid sample      first grid-sample kernel start -> grid-sample selection end (main stream)
+  gs kernels       the summed device time of the grid-sample kernels and memsets in that span (the rest of the span
+                   is launch latency and idle time between them), then each op's own median below the table
   input stage      grid-sample selection end -> frame_begin_kernel end (main stream)
   map branch       first map-update op start -> kd_finalize_kernel end (map stream; the previous frame's map update)
   map ready -> ICP kd_finalize_kernel end -> first ICP kernel start: the main stream's idle time after the map is ready
@@ -24,6 +26,7 @@ import argparse
 import ctypes as C
 import json
 import os
+import re
 import sys
 import tempfile
 
@@ -84,9 +87,10 @@ def analyse(ops):
     main_s, map_s = main_s.pop(), map_s.pop()
     main = [o for o in ops if o["stream"] == main_s]
     mapq = [o for o in ops if o["stream"] == map_s]
-    # a frame on the main stream starts at its grid sample's voxel_hash_kernel
-    starts = [i for i, o in enumerate(main) if has(o, "voxel_hash_kernel")]
-    rows, gaps_main, gaps_map, n_main, n_map = [], [], [], [], []
+    # a frame on the main stream starts at its grid sample's first kernel (the bucket path's gs_hash_bins_kernel, or
+    # voxel_hash_kernel in front of the radix sort) and its sample ends with the selection
+    starts = [i for i, o in enumerate(main) if has(o, "voxel_hash_kernel") or has(o, "gs_hash_bins_kernel")]
+    rows, gaps_main, gaps_map, n_main, n_map, gs_ops = [], [], [], [], [], {}
     prev_icp0 = None
     for a, b in zip(starts[:-1], starts[1:]):
         fr = main[a:b]
@@ -95,7 +99,13 @@ def analyse(ops):
         if len(ib) != 1:
             continue
         ib = ib[0]
-        gs_end = max(o["t1"] for o in fr[:ib] if has(o, "GridSampleSelect"))
+        sel = [o for o in fr[:ib] if has(o, "GridSampleSelect") or has(o, "gs_bucket_select_kernel")]
+        gs_end = max(o["t1"] for o in sel)
+        gs = [o for o in fr[:ib] if o["t1"] <= gs_end]
+        for o in gs:
+            m = re.search(r"(\w+_kernel)", o["name"]) if o["cat"] == "kernel" else None
+            short = m.group(1) if m else o["cat"]
+            gs_ops.setdefault(short, []).append(o["t1"] - o["t0"])
         icp = fr[ib + 1:]
         icp_k = [o for o in icp if o["cat"] == "kernel"]
         if not icp_k:
@@ -106,7 +116,8 @@ def analyse(ops):
         upd = [o for o in mapq if prev_icp0 is not None and prev_icp0 < o["t0"] < t_icp0]
         prev_icp0 = t_icp0
         fin = [o for o in upd if has(o, "kd_finalize_kernel")]
-        row = {"grid sample": gs_end - fr[0]["t0"], "input stage": fr[ib]["t1"] - gs_end,
+        row = {"grid sample": gs_end - fr[0]["t0"], "gs kernels": sum(o["t1"] - o["t0"] for o in gs),
+               "input stage": fr[ib]["t1"] - gs_end,
                "input -> ICP": t_icp0 - fr[ib]["t1"], "ICP": t_icp1 - t_icp0, "ICP -> next": nxt["t0"] - t_icp1,
                "frame": nxt["t0"] - fr[0]["t0"]}
         if fin:
@@ -120,7 +131,7 @@ def analyse(ops):
         gaps_main += [q["t0"] - p["t1"] for p, q in zip(seq[:-1], seq[1:])]
         gaps_main += [q["t0"] - p["t1"] for p, q in zip(icp[:-1], icp[1:])]
         n_main.append(len(fr))
-    return rows, gaps_main, gaps_map, n_main, n_map
+    return rows, gaps_main, gaps_map, n_main, n_map, gs_ops
 
 
 def main():
@@ -162,9 +173,9 @@ def main():
         prof.export_chrome_trace(path)
         with open(path) as fh:
             trace = json.load(fh)
-    rows, gm, gp, nm, np_ = analyse(ops_of(trace))
+    rows, gm, gp, nm, np_, gs_ops = analyse(ops_of(trace))
     print(f"# pass 2 (torch.profiler): {len(rows)} frames of {args.frames} timed; medians in microseconds")
-    keys = ["grid sample", "input stage", "map branch", "map end - input end", "map ready -> ICP", "input -> ICP", "ICP",
+    keys = ["grid sample", "gs kernels", "input stage", "map branch", "map end - input end", "map ready -> ICP", "input -> ICP", "ICP",
             "ICP -> next", "frame"]
     for k in keys:
         v = [r[k] for r in rows if k in r]
@@ -172,6 +183,8 @@ def main():
             print(f"{k:22s} median {np.median(v):8.1f}   p10 {np.percentile(v, 10):8.1f}   p90 {np.percentile(v, 90):8.1f}")
     print(f"main stream: {np.median(nm):.1f} ops per frame, median gap between consecutive ops {np.median(gm):.2f} us "
           f"(input chain and ICP chain)")
+    for name, v in gs_ops.items():
+        print(f"  grid-sample op {name:34s} {len(v) / len(rows):4.1f} per frame, median {np.median(v):7.2f} us")
     if gp:
         print(f"map stream:  {np.median(np_):.1f} ops per update, median gap between consecutive ops {np.median(gp):.2f} us")
 
